@@ -1,4 +1,4 @@
-/* b200engine.h — C ABI of the in-process B200 inference engine.
+/* b200engine.h — C ABI of the in-process H100 inference engine (the b200 prefix is historical).
  *
  * This is the drop-in boundary described in SURVEY.md §8(b).  The reference (kubeai-project/kubeai)
  * has no FFI: a backend is an HTTP server reached through
@@ -32,7 +32,7 @@ typedef enum {
 } b200_status;
 
 const char* b200_last_error(void);
-/* "kubeai-b200 <version> sm_100a" */
+/* "kubeai-b200 <version> sm_90a" */
 const char* b200_version(void);
 
 /* ------------------------------------------------------------------ engine (one per GPU replica)
@@ -121,6 +121,12 @@ int b200_stats_get(b200_engine* e, b200_stats* out);
 int b200_engine_is_failed(b200_engine* e);
 
 /* manual_step mode: run one scheduler iteration + forward; *info may be NULL. Returns 1 if a step ran, 0 if idle. */
+/* on != 0: requests that arrive between two steps are admitted in a fixed order (prompt content) instead of arrival order,
+ * so concurrent clients that submit the same requests between the same steps get the same batches on every run.
+ * Default 0 (first come, first served). */
+int b200_engine_set_fixed_admission(b200_engine* e, int32_t on);
+/* Submitted requests not yet finished (queued, running, or between chunks of a prompt). */
+int32_t b200_engine_unfinished(b200_engine* e);
 int b200_engine_step(b200_engine* e, b200_step_info* info);
 /* manual_step mode: up to max_steps iterations back to back on the calling thread, pipelined the way the engine's own
  * loop thread runs: the tokens of step N are handed to the waiting API threads after step N+1 has been enqueued on the
@@ -288,14 +294,18 @@ void b200_harness_config_default(b200_harness_config* cfg);
 int64_t b200_harness_synth_threads(const b200_harness_config* cfg, char* buf, size_t cap);
 /* server != NULL: in-process transport (b200_server_handle); else HTTP/1.1 to host:port.
  * threads_json: the reference's input format [{"id":..,"messages":[{"role","content"},..]},..] or NULL = synthetic. */
+/* Requests the load generators running in this process are about to have in flight: conversations in progress plus free
+ * slots that a conversation still waiting to start will take.  Stepping an engine only while b200_engine_unfinished()
+ * equals this makes the batches of a multi-turn run independent of client thread timing. */
+int64_t b200_harness_expected_inflight(void);
 int b200_harness_run(b200_server* server, const char* host, int32_t port, const b200_harness_config* cfg,
                      const char* threads_json, size_t threads_len, b200_harness_result* out);
 
 /* ------------------------------------------------------------------ op-level entry points
  * Raw device pointers (bf16 unless noted) + a cudaStream_t passed as void* (NULL = default stream).
- * These are what the per-kernel parity tests and the ncu captures call. */
-/* GEMM kernel variant for plans/engines created afterwards: 2 = CTA-pair tcgen05 cta_group::2 (default),
- * 1 = single-CTA kernel (kept for A/B measurements).  Returns the active variant. */
+ * These are what the per-kernel parity tests and the microbenchmarks call. */
+/* Schedule of b200_op_gemm: 2 = split-K sized to the device (default), 1 = every tile over its whole K.  Returns the
+ * active variant. */
 int b200_set_gemm_variant(int32_t v);
 /* ---- byte-level BPE tokenizer over a local HF tokenizer.json of the Llama-3 family (csrc/tokenizer.cc).  Replaces, on the
  * host side of this ABI, the tokenizer + chat template the reference's backend pod applies to the model directory it is given
@@ -318,28 +328,28 @@ int64_t b200_tokenizer_stream_push(b200_detok_stream* d, int32_t id, char* buf, 
 int64_t b200_tokenizer_chat_llama3(const b200_tokenizer* t, const char* const* roles, const char* const* contents, int32_t n,
                                    int32_t add_generation_prompt, int32_t* ids, size_t cap);
 
-/* Host-only (no GPU needed): how a projection [N, K] of a step of T > 128 tokens is scheduled on a device with `sms` SMs.
- * out8: [0] token-tile size, [1] token tiles, [2] tiles, [3] CTA pairs launched, [4] 1 = one whole tile per pair, [5] 1 = the
- * engine fuses the elementwise neighbour into the launch, [6] whole-tile waves ahead of the stream-K tail, [7] 0. */
+/* Host-only (no GPU needed): how a projection [N, K] of a step of T tokens is scheduled on a device with `sms` SMs.
+ * out8: [0] token-tile size, [1] token tiles, [2] tiles (128 weight rows x token tile), [3] K-splits per tile, [4] CTAs,
+ * [5] rule that chose the splits (1 one token tile, 2 several), [6] 0, [7] 0. */
 int b200_schedule_query(int32_t N, int32_t K, int32_t T, int32_t sms, int32_t* out8);
 /* Host-only: CTAs per (sequence, KV head) the engine gives decode attention when `num_work` sequences decode. */
 int b200_attn_split_query(int32_t num_work, int32_t kv_heads, int32_t max_ctx, int32_t sms);
-/* Debug: subsequent pair-GEMM launches write 8 clock64() phase stamps per CTA into trace_dev (int64[grid][8]);
- * NULL turns it off.  Stamps: 0 entry, 1 after prologue, 2 first tile accumulated, 3 main loop + partial stores
- * done, 4 peers' partials visible, 5 bulk pull landed, 6 before final cluster sync, 7 exit. */
+/* GEMM phase tracing: the wgmma GEMM records no timestamps, so only NULL (tracing off) is accepted; any buffer is
+ * refused with B200_ERR_INVALID. */
 int b200_op_gemm_trace(void* trace_dev);
-/* Same contraction, but the GEMM only dumps fp32 stream-K partials and a second kernel reduces them to bf16 —
- * the engine's T <= 512 path (there the reduction is fused into the consumer kernels). */
+/* Same contraction in the engine's form whatever the variant: split-K sized to the device, the partials summed in-kernel
+ * in split order; N % 8 == 0 (the elementwise consumers read output rows 16 bytes at a time). */
 int b200_op_gemm_deferred(const void* w, const void* x, void* out, int32_t N, int32_t T, int32_t K, void* stream);
 int b200_op_gemm(const void* w, const void* x, void* out, int32_t N, int32_t T, int32_t K, void* stream);
-/* The decode-shape fused GEMM (T <= 128; csrc/gemm3_tcgen05.cu): acc = X' W^T with the split-K reduction finished in the
- * kernel, a prologue (pro 0: X' = x; 1: X' = RMSNorm(x) from the per-slab sums of squares ssq_in [T, ssq_slabs] and norm_w)
+/* The fused projection GEMM (csrc/gemm_wgmma.cu): acc = X' W^T with the split-K reduction finished in the kernel, a prologue (pro 0: X' = x; 1: X' = RMSNorm(x) from the per-slab sums of squares ssq_in [T, ssq_slabs] and norm_w)
  * and an epilogue on the bf16-rounded result (epi 0: out [T, N]; 1: out (in/out, residual) += acc, ssq_out [T, N/128], and
- * optionally the RMSNorm of the new residual for the next projection;
+ * optionally (T <= 128) the RMSNorm of the new residual for the next projection;
  * 2: out [T, N/2] = silu(gate) * up with gate/up rows interleaved in 64-row blocks of w; 3: neox RoPE of q/k heads, q ->
- * out (the fused qkv buffer, ldo), k/v -> kv_layer pages; 4: argmax_out [T] = argmax_n acc[t, n < n_valid]).
- * force: 0 automatic schedule, 1..4 pairs per tile (cluster split-K through distributed shared memory), < 0 stream-K.
- * schedule_out (optional, 3 ints): pairs per tile, stream-K flag, CTAs launched. */
+ * out (the fused qkv buffer, ldo), k/v -> kv_layer pages; 4 (T <= 128): argmax_out [T] = argmax_n acc[t, n < n_valid]).  pro 1 needs T <= 128.
+ * force, T <= 128: 0 automatic split count, n >= 1 or -n <= -2: n K-splits per tile, -1 automatic; T > 128: 0 automatic
+ * token tile, >= 64 the requested token tile: the largest of 64 / 128 / 256 not above it.
+ * schedule_out (optional, 3 ints): K-splits per tile, rule that chose them (0 force, 1 device-filling for one token tile,
+ * 2 device-filling over several), CTAs launched. */
 typedef struct {
   int32_t N, T, K, x_rows;
   int32_t pro, epi, force;
@@ -380,8 +390,8 @@ int b200_op_paged_attn(const void* q, int32_t ldq, void* out, int32_t ldo, const
 int b200_op_paged_attn_decode_split(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                                     const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
                                     int32_t q_heads, int32_t kv_heads, float scale, int32_t split, void* stream);
-/* Chunked-prefill attention on the tensor cores (csrc/attention_tc.cu): work items (q_tok0, q_count <= 64, q_pos0, seq); q rows
- * are read from the fused qkv buffer [q_rows, ldq] (q heads first) through a 3-D TMA map. */
+/* Chunked-prefill attention on wgmma (csrc/attention_wgmma.cu): work items (q_tok0, q_count <= 64, q_pos0, seq), one CTA per
+ * (work item, q head); q rows are read from the fused qkv buffer [q_rows, ldq] (q heads first). */
 int b200_op_paged_attn_prefill_tc(const void* qkv, int32_t q_rows, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                                   const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
                                   int32_t q_heads, int32_t kv_heads, float scale, void* stream);

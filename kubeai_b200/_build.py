@@ -1,4 +1,4 @@
-"""Build libb200engine.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libb200engine.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
 The shared library is the product: a C-ABI engine (include/b200engine.h) with no Python or torch
 dependency.  Python only loads it through ctypes (kubeai_b200/_lib.py).
@@ -18,12 +18,9 @@ LIB = ROOT / "lib" / "libb200engine.so"
 OBJ = ROOT / "lib" / "obj"
 
 SOURCES = [
-    "gemm_tcgen05.cu",
-    "gemm2_tcgen05.cu",
-    "gemm3_tcgen05.cu",
-    "chain_tcgen05.cu",
+    "gemm_wgmma.cu",
     "attention.cu",
-    "attention_tc.cu",
+    "attention_wgmma.cu",
     "elementwise.cu",
     "abi_ops.cu",
     "engine.cu",
@@ -35,7 +32,7 @@ SOURCES = [
 ]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function",
     "-diag-suppress", "177",

@@ -120,6 +120,9 @@ SYMBOLS = {
     "b200_stats_get": (C.c_int, [_vp, C.POINTER(Stats)]),
     "b200_engine_is_failed": (C.c_int, [_vp]),
     "b200_engine_step": (C.c_int, [_vp, C.POINTER(StepInfo)]),
+    "b200_engine_unfinished": (C.c_int32, [_vp]),
+    "b200_engine_set_fixed_admission": (C.c_int, [_vp, _i32]),
+    "b200_harness_expected_inflight": (C.c_int64, []),
     "b200_engine_run": (C.c_int, [_vp, _i32, _i64, C.POINTER(StepInfo), C.POINTER(_i32)]),
     "b200_engine_replay": (C.c_int, [_vp, _i32, _i32, C.POINTER(C.c_double), C.POINTER(_i64), C.POINTER(_i64),
                                       C.POINTER(_i64), C.POINTER(_i64)]),

@@ -11,8 +11,6 @@
 #include "errors.h"
 #include "gemm.h"
 #include "gemm3.h"
-#include "epi_pass.cuh"
-#include "chain.h"
 #include "kernels.h"
 
 namespace b200 {
@@ -30,7 +28,7 @@ int require_device() {
   int n = 0;
   cudaError_t e = cudaGetDeviceCount(&n);
   if (e != cudaSuccess || n <= 0) {
-    set_error("no CUDA device available (%s): the B200 path has no CPU fallback",
+    set_error("no CUDA device available (%s): the engine has no CPU fallback",
               e == cudaSuccess ? "device count 0" : cudaGetErrorString(e));
     return B200_ERR_NO_DEVICE;
   }
@@ -54,10 +52,7 @@ constexpr int kCounterInts = 1 << 20;
 int ensure_scratch() {
   std::lock_guard<std::mutex> lk(g_mu);
   if (g_ws) return 0;
-  int sms = 0, dev = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  g_ws_bytes = std::max<size_t>(gemm_workspace_bytes(sms), 256ull << 20);
+  g_ws_bytes = 256ull << 20;
   if (cudaMalloc(&g_ws, g_ws_bytes) != cudaSuccess) return -1;
   if (cudaMalloc(&g_counters, kCounterInts * sizeof(int)) != cudaSuccess) return -1;
   cudaMemset(g_counters, 0, kCounterInts * sizeof(int));
@@ -71,7 +66,7 @@ using namespace b200;
 extern "C" {
 
 const char* b200_last_error(void) { return g_err; }
-const char* b200_version(void) { return "kubeai-b200 0.1.0 sm_100a"; }
+const char* b200_version(void) { return "kubeai-b200 0.1.0 sm_90a"; }
 
 int b200_op_gemm(const void* w, const void* x, void* out, int32_t N, int32_t T, int32_t K, void* stream) {
   if (int rc = require_device()) return rc;
@@ -85,48 +80,45 @@ int b200_op_gemm(const void* w, const void* x, void* out, int32_t N, int32_t T, 
     return B200_ERR_OOM;
   }
   GemmPlan plan;
-  int rc = gemm_plan_init(&plan, w, N, K, K, g_ws, g_counters, 0);
+  int rc = gemm_plan_init(&plan, w, N, K, K, g_ws, g_ws_bytes, g_counters, kCounterInts);
   if (rc) return cuda_fail("gemm_plan_init", rc);
   const int bn = gemm_block_n_for(T);
-  const int slabs = (N + 127) / 128, ntt = (T + bn - 1) / bn;
-  if (2ll * slabs * ntt > kCounterInts) {
-    set_error("b200_op_gemm: problem too large for the op-level scratch");
-    return B200_ERR_INVALID;
-  }
   CUtensorMap tmx;
   rc = gemm_make_x_map(&tmx, x, T, K, K, bn);
   if (rc) return cuda_fail("gemm_make_x_map", rc);
   rc = gemm_run(plan, tmx, bn, out, N, T, static_cast<cudaStream_t>(stream));
+  if (rc == -9) {
+    set_error("b200_op_gemm: problem too large for the op-level scratch");
+    return B200_ERR_INVALID;
+  }
   if (rc) return cuda_fail("gemm_run", rc);
   return 0;
 }
 
 int b200_op_gemm_deferred(const void* w, const void* x, void* out, int32_t N, int32_t T, int32_t K, void* stream) {
+  // the engine's form of the product: split-K sized to the device whatever the variant, output rows 16-byte aligned for
+  // the vectorised elementwise consumers
   if (int rc = require_device()) return rc;
-  if (!w || !x || !out || N <= 0 || T <= 0 || K <= 0 || K % 8 || gemm_variant() != 2) {
-    set_error("b200_op_gemm_deferred: bad arguments N=%d T=%d K=%d (needs the pair kernel)", N, T, K);
+  if (!w || !x || !out || N <= 0 || T <= 0 || K <= 0 || K % 8 || N % 8) {
+    set_error("b200_op_gemm_deferred: bad arguments N=%d T=%d K=%d (N %% 8 == 0 required)", N, T, K);
     return B200_ERR_INVALID;
   }
   if (ensure_scratch()) { set_error("workspace allocation failed"); return B200_ERR_OOM; }
-  GemmPlan plan;
-  int rc = gemm_plan_init(&plan, w, N, K, K, g_ws, g_counters, 0);
-  if (rc) return cuda_fail("gemm_plan_init", rc);
-  plan.ws_bytes = g_ws_bytes;
-  if ((rc = gemm_plan_build_table(&plan, T))) return cuda_fail("gemm_plan_build_table", rc);
-  const int bn = gemm_block_n_for(T);
-  CUtensorMap tmx;
-  rc = gemm_make_x_map(&tmx, x, T, K, K, bn);
-  PartialView pv = no_partials();
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // complete tiles land in `out` directly; the reducer then fills in the split tiles (in place)
-  if (!rc) rc = gemm_run_deferred(plan, tmx, bn, out, N, T, st, &pv);
-  if (!rc) rc = reduce_partials(pv, out, N, T, N, st);
-  cudaStreamSynchronize(st);  // the segment table is freed below
-  gemm_plan_destroy(&plan);
+  std::lock_guard<std::mutex> lk(g_mu);
+  const int v = gemm_variant();
+  gemm_set_variant(2);
+  int rc = 0;
+  {
+    GemmPlan plan;
+    rc = gemm_plan_init(&plan, w, N, K, K, g_ws, g_ws_bytes, g_counters, kCounterInts);
+    const int bn = gemm_block_n_for(T);
+    CUtensorMap tmx;
+    if (!rc) rc = gemm_make_x_map(&tmx, x, T, K, K, bn);
+    if (!rc) rc = gemm_run(plan, tmx, bn, out, N, T, static_cast<cudaStream_t>(stream));
+  }
+  gemm_set_variant(v);
   return rc ? cuda_fail("gemm_deferred", rc) : 0;
 }
-
-static long long* g_gemm3_trace = nullptr;
 
 int b200_op_gemm3(const b200_gemm3_args* a, void* stream, int32_t* schedule_out) {
   if (int rc = require_device()) return rc;
@@ -136,53 +128,30 @@ int b200_op_gemm3(const b200_gemm3_args* a, void* stream, int32_t* schedule_out)
   }
   if (ensure_scratch()) { set_error("workspace allocation failed"); return B200_ERR_OOM; }
   static float2* cand = nullptr;          // [128 tokens][slabs]
-  static int* flags = nullptr;            // stream-K neighbour flags [0, 4096) + fused-norm row flags [4096, 8192)
-  static int epoch = 0;
   static std::mutex mu;
   std::lock_guard<std::mutex> lk(mu);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (!flags) {
-    if (cudaMalloc(&flags, 8192 * sizeof(int)) != cudaSuccess || cudaMemset(flags, 0, 8192 * sizeof(int)) != cudaSuccess) return B200_ERR_OOM;
-    if (cudaMalloc(&cand, sizeof(float2) * 128 * 4096) != cudaSuccess) return B200_ERR_OOM;
+  constexpr int kMaxCandSlabs = 4096;
+  if (!cand && cudaMalloc(&cand, sizeof(float2) * 128 * kMaxCandSlabs) != cudaSuccess) return B200_ERR_OOM;
+  const int slabs = (a->N + 127) / 128;
+  if (a->epi == GEMM3_EPI_ARGMAX && (slabs > kMaxCandSlabs || !a->argmax_out || a->T > 128)) {
+    set_error("b200_op_gemm3: argmax needs argmax_out, T <= 128 and N <= 524288");
+    return B200_ERR_INVALID;
   }
-  if (a->epi == GEMM3_EPI_ARGMAX && (a->N / 128 > 4096 || !a->argmax_out)) { set_error("b200_op_gemm3: argmax needs argmax_out and N <= 524288"); return B200_ERR_INVALID; }
-  if (a->T > 128) {
-    // steps of more than 128 tokens: the pair kernel (gemm2) with the same fused epilogues, split tiles finished in-kernel
-    if (a->pro != GEMM3_PRO_NONE || a->epi == GEMM3_EPI_ARGMAX || a->normed_out || gemm_variant() != 2) {
-      set_error("b200_op_gemm3: T > 128 serves PRO_NONE with the PLAIN / RESADD / SILU / ROPE_KV epilogues");
-      return B200_ERR_INVALID;
-    }
-    gemm2_read_env();
-    GemmPlan plan;
-    int rc = gemm_plan_init(&plan, a->w, a->N, a->K, a->K, g_ws, g_counters, 0);
-    if (rc) return cuda_fail("gemm_plan_init", rc);
-    plan.ws_bytes = g_ws_bytes;
-    const int bn = a->force > 0 ? a->force : gemm_block_n_for(a->T);   // force = token-tile size (256 / 512) in this regime
-    CUtensorMap tmx;
-    rc = gemm_make_x_map(&tmx, a->x, a->x_rows, a->K, a->K, bn);
-    if (rc) return cuda_fail("gemm_make_x_map", rc);
-    Gemm2Epi e;
-    memset(&e, 0, sizeof(e));
-    e.epi = a->epi;
-    e.out = static_cast<__nv_bfloat16*>(a->out); e.ldo = a->ldo;
-    e.positions = a->positions; e.slots = a->slots; e.cos_sin = static_cast<const __nv_bfloat16*>(a->cos_sin);
-    e.kv_layer = static_cast<__nv_bfloat16*>(a->kv_layer); e.Hq = a->q_heads; e.Hkv = a->kv_heads; e.max_pos = a->max_pos;
-    e.flags = flags; e.epoch = ++epoch;
-    if (schedule_out) { schedule_out[0] = bn; schedule_out[1] = 2; schedule_out[2] = 2 * gemm2_units_for(plan, (a->T + bn - 1) / bn); }
-    rc = gemm2_run_fused(plan, tmx, bn, a->T, e, st);
-    return rc ? cuda_fail("gemm2_run_fused", rc) : 0;
+  if (a->T > 128 && (a->pro != GEMM3_PRO_NONE || a->normed_out)) {
+    set_error("b200_op_gemm3: T > 128 serves PRO_NONE without the fused norm");
+    return B200_ERR_INVALID;
   }
   Gemm3Schedule sch;
-  int rc = gemm3_schedule(a->N, a->K, a->T, a->pro, a->force, &sch);
+  int rc = gemm3_schedule(a->N, a->K, a->T, a->force, &sch);
   if (rc) { set_error("b200_op_gemm3: shape / schedule not served (rc=%d, N=%d K=%d T=%d force=%d)", rc, a->N, a->K, a->T, a->force); return B200_ERR_INVALID; }
-  if (gemm3_ws_bytes(sch.grid) > g_ws_bytes) { set_error("b200_op_gemm3: workspace too small"); return B200_ERR_INVALID; }
   GemmPlan plan;
-  rc = gemm_plan_init(&plan, a->w, a->N, a->K, a->K, g_ws, g_counters, 0);
+  rc = gemm_plan_init(&plan, a->w, a->N, a->K, a->K, g_ws, g_ws_bytes, g_counters, kCounterInts);
   if (rc) return cuda_fail("gemm_plan_init", rc);
   Gemm3Params p;
   memset(&p, 0, sizeof(p));
   p.tm_w = plan.tm_w;
-  rc = gemm_make_x_map(&p.tm_x, a->x, a->x_rows, a->K, a->K, 128);
+  rc = gemm_make_x_map(&p.tm_x, a->x, a->x_rows, a->K, a->K, sch.block_n);
   if (rc) return cuda_fail("gemm_make_x_map", rc);
   p.N = a->N; p.T = a->T; p.K = a->K; p.pro = a->pro; p.epi = a->epi;
   p.ssq_in = a->ssq_in; p.ssq_slabs = a->ssq_slabs; p.norm_w = static_cast<const __nv_bfloat16*>(a->norm_w); p.eps = a->eps;
@@ -191,19 +160,17 @@ int b200_op_gemm3(const b200_gemm3_args* a, void* stream, int32_t* schedule_out)
   p.kv_layer = static_cast<__nv_bfloat16*>(a->kv_layer); p.Hq = a->q_heads; p.Hkv = a->kv_heads; p.max_pos = a->max_pos;
   p.cand = cand; p.n_valid = a->n_valid > 0 ? a->n_valid : a->N;
   if (a->epi == GEMM3_EPI_RESADD && a->normed_out) {
-    if (sch.streamk || !a->norm_w_out || a->N / 128 > 1024) { set_error("b200_op_gemm3: the fused norm needs the cluster schedule and norm_w_out"); return B200_ERR_INVALID; }
+    if (!a->norm_w_out || !a->ssq_out) { set_error("b200_op_gemm3: the fused norm needs norm_w_out and ssq_out"); return B200_ERR_INVALID; }
     p.normed_out = static_cast<__nv_bfloat16*>(a->normed_out);
     p.norm_w_out = static_cast<const __nv_bfloat16*>(a->norm_w_out);
-    p.row_flags = flags + 4096;
   }
-  p.ws = g_ws; p.flags = flags; p.epoch = ++epoch;
-  p.trace = g_gemm3_trace;
-  { const char* e = getenv("B200_GEMM3_DBG"); p.dbg = e ? atoi(e) : 0; }
-  if (schedule_out) { schedule_out[0] = sch.S; schedule_out[1] = sch.streamk; schedule_out[2] = sch.grid; }
+  p.ws = g_ws; p.ws_bytes = g_ws_bytes;
+  p.counters = g_counters; p.counters_cap = kCounterInts;
+  if (schedule_out) { schedule_out[0] = sch.S; schedule_out[1] = sch.rule; schedule_out[2] = sch.grid; }
   rc = gemm3_launch(p, sch, st);
   if (rc) return cuda_fail("gemm3_launch", rc);
   if (a->epi == GEMM3_EPI_ARGMAX) {
-    rc = argmax_candidates(cand, a->argmax_out, a->T, a->N / 128, st);
+    rc = argmax_candidates(cand, a->argmax_out, a->T, slabs, st);
     if (rc) return cuda_fail("argmax_candidates", rc);
     cudaStreamSynchronize(st);   // the shared candidate buffer is reused by the next call
   }
@@ -212,7 +179,11 @@ int b200_op_gemm3(const b200_gemm3_args* a, void* stream, int32_t* schedule_out)
 
 int b200_schedule_query(int32_t N, int32_t K, int32_t T, int32_t sms, int32_t* out8) {
   if (N <= 0 || K <= 0 || T <= 0 || sms < 2 || !out8) { set_error("b200_schedule_query: bad arguments"); return B200_ERR_INVALID; }
-  gemm2_schedule_query(N, K, T, sms, out8);
+  Gemm3Schedule sch;
+  if (gemm3_schedule_for(N, K, T, 0, sms, &sch)) { set_error("b200_schedule_query: shape not served"); return B200_ERR_INVALID; }
+  const int ntt = (T + sch.block_n - 1) / sch.block_n;
+  const int vals[8] = {sch.block_n, ntt, ((N + 127) / 128) * ntt, sch.S, sch.grid, sch.rule, 0, 0};
+  for (int i = 0; i < 8; ++i) out8[i] = vals[i];
   return 0;
 }
 
@@ -227,10 +198,9 @@ int b200_set_gemm_variant(int32_t v) {
 }
 
 int b200_op_gemm_trace(void* trace_dev) {
-  gemm2_set_trace(static_cast<long long*>(trace_dev));
-  g_gemm3_trace = static_cast<long long*>(trace_dev);   // b200_op_gemm3 launches stamp 8 values per CTA while this is set
-  chain_set_trace(static_cast<long long*>(trace_dev));  // chain launches: 40 slots x 148 CTAs x 32 stamps
-  return 0;
+  if (!trace_dev) return 0;   // tracing off: the only state the GEMM kernels support
+  set_error("b200_op_gemm_trace: the GEMM kernels record no timestamps");
+  return B200_ERR_INVALID;
 }
 
 int b200_op_embed(const void* table, const int32_t* ids, void* out, int32_t T, int32_t H, int32_t vocab,

@@ -3,7 +3,7 @@
 // table, GQA 4:1 — the operation the reference backend delegates to FlashInfer/FlashAttention
 // (vllm/model_executor/models/llama.py:223-233, vllm/v1/attention/backends/flashinfer.py).
 //
-// B200 design: this op is an HBM stream (decode reads 4 KiB of K+V per context token per layer),
+// Design: this op is an HBM stream (decode reads 4 KiB of K+V per context token per layer),
 // so the kernel is organised around the page gather, not around the math:
 //   * KV layout is [block][K|V][kv_head][16 tokens][128] so one (page, head) is a contiguous 4 KiB
 //     run.  A layer is addressed as one 2-D tensor of 256-byte rows; ONE thread per CTA pulls a
@@ -386,14 +386,6 @@ int launch_attn(const CUtensorMap& tm, dim3 grid, cudaStream_t st, const __nv_bf
 }
 
 }  // namespace
-
-int prefill_attn_query_block() {
-  static const int v = [] {
-    const char* e = getenv("B200_ATTN_TC");
-    return (e && atoi(e) == 0) ? 16 : 64;
-  }();
-  return v;
-}
 
 size_t attn_split_ws_bytes(int num_work, int Hkv, int parts) {
   return static_cast<size_t>(num_work) * Hkv * parts * 4 * (kD + 2) * sizeof(float);

@@ -31,7 +31,7 @@ __device__ __forceinline__ float warp_sum(float v) {
 
 // ------------------------------------------------------------------ embedding gather
 // ssq (optional): [T, ssq_slabs] per-slab sums of squares of the row, the form the fused GEMM's RMSNorm prologue reads
-// (gemm3_tcgen05.cu PRO_NORM); the whole row's sum goes to slab 0, the other slabs are zeroed.
+// (gemm_wgmma.cu PRO_NORM); the whole row's sum goes to slab 0, the other slabs are zeroed.
 __global__ void embed_kernel(const __nv_bfloat16* __restrict__ table, const int* __restrict__ ids,
                              __nv_bfloat16* __restrict__ out, int H, int vocab, float* __restrict__ ssq, int ssq_slabs) {
   griddep_enter();
@@ -110,7 +110,7 @@ __global__ void rmsnorm_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat1
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         // residual += x in bf16; variance and normalisation use the ROUNDED sum (vLLM _C fused_add_rms_norm, HF
-        // modeling_llama.py:325 + :62-67) — the decode GEMM epilogues store exactly this bf16 sum (gemm3_tcgen05.cu)
+        // modeling_llama.py:325 + :62-67) — the GEMM residual-add epilogue stores exactly this bf16 sum (gemm_wgmma.cu)
         o.h[j] = __float2bfloat16_rn(xa[i][j] + __bfloat162float(rb[i].h[j]));
         v[i][j] = __bfloat162float(o.h[j]);
       }

@@ -33,8 +33,6 @@
 #include "errors.h"
 #include "gemm.h"
 #include "gemm3.h"
-#include "epi_pass.cuh"
-#include "chain.h"
 #include "kernels.h"
 #include "hostutil.h"
 #include "xxh64.h"
@@ -184,6 +182,7 @@ struct Seq {
   std::vector<int32_t> out;
   size_t drained = 0;
   int finished = 0;
+  uint64_t arrival_key = 0;   // xxh64 of the prompt: admission order among requests that arrive between two steps
   std::atomic<bool> abort_requested{false};
 };
 
@@ -227,7 +226,7 @@ struct Engine {
   int Tcap, Scap, max_blocks_per_seq;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  int sms = 148;
+  int sms = 0;
 
   // weights
   struct Layer {
@@ -246,28 +245,19 @@ struct Engine {
        *last_hidden = nullptr, *logits = nullptr;
   int* sampled = nullptr;
   int32_t* sampled_host = nullptr;  // pinned
-  // decode-shape fused path (gemm3_tcgen05.cu): per-slab sums of squares of the residual, argmax candidates, stream-K flags
-  float* ssq = nullptr;
-  float2* cand = nullptr;
-  int* g3_flags = nullptr;
-  int g3_epoch = 0;
-  bool fused_ok = false;
-  Gemm3Schedule sch_qkv, sch_o, sch_gu, sch_down, sch_lm;
-  // projection chain (chain_tcgen05.cu): o -> norm -> gate_up -> down -> norm -> next qkv -> rope in one persistent launch
-  bool chain_ok = false;
+  // fused epilogues (gemm_wgmma.cu): RoPE + KV write, residual add, SiLU * up and per-slab argmax ride in the projection
+  // that produces their input; off (B200_FUSED_DECODE=0 / B200_FUSED_PREFILL=0) each runs as its own elementwise kernel
+  float2* cand = nullptr;    // argmax candidates [token][V / 128 slab]
+  bool fused_ok = false;     // steps of at most 128 tokens
+  bool fused2_ok = false;    // larger steps
   float* attn_ws = nullptr;  // split-KV decode partials
   int attn_split_force = 0;  // B200_ATTN_SPLIT=<parts> (A/B knob; 1 = never split)
   static constexpr int kSplitMaxWork = 18, kSplitMaxParts = 32;
-  bool fused2_ok = false;   // steps of more than 128 tokens: pair kernel with fused epilogues (gemm2 mode 2)
-  int chain_ctas = 0;
-  unsigned long long* chain_bar = nullptr;
-  unsigned long long chain_bar_count = 0;   // host mirror of the grid-barrier counter
-  XMaps xm_res;
   XMaps xm_normed, xm_attn, xm_act, xm_last;
   float* gemm_ws = nullptr;
   size_t gemm_ws_bytes = 0;
   int* gemm_counters = nullptr;
-  bool deferred_ok = false;  // pair kernel + segment tables available
+  int gemm_counters_cap = 0;
 
   // KV
   bf16* kv = nullptr;
@@ -302,7 +292,8 @@ struct Engine {
   double step_timing_last_end = 0;
   uint32_t skip_mask = 0;  // debug/timing: kernel classes (1 << B200_K_*) NOT launched by forward() (results are garbage)
   bool profiling = false;
-  bool keep_logits = false;  // parity hook: lm_head leaves complete bf16 logits (b200_engine_set_keep_logits)
+  bool keep_logits = false;
+  bool fixed_admission = false;   // b200_engine_set_fixed_admission  // parity hook: lm_head leaves complete bf16 logits (b200_engine_set_keep_logits)
   int last_S = 0;
   std::vector<std::pair<int, cudaEvent_t>> prof_events;  // (class, event) in launch order: start, stop pairs
   size_t prof_used = 0;
@@ -311,8 +302,6 @@ struct Engine {
   int init(const b200_config& c);
   int alloc_all();
   int forward(const StepMeta& m, int32_t* dbuf, bool all_logits, bf16* logits_out);
-  int forward_fused(const StepMeta& m, int32_t* dbuf);
-  int forward_chain(const StepMeta& m, int32_t* dbuf);
   // decode attention; with few sequences the context of each is split over several CTAs (attention.cu attn_decode_split)
   int decode_attention(const StepMeta& m, bf16* kv_l, const int* btab, const AttnWork* dwork, float scale) {
     int split = 1;
@@ -321,9 +310,7 @@ struct Engine {
     return paged_attention(qkv, QKV, attn, Hq * kD, kv_l, btab, max_blocks_per_seq, dwork, m.nd, Hq, Hkv, scale, 1, stream, attn_ws, split);
   }
   int prefill_attention(bf16* kv_l, const int* btab, const AttnWork* pwork, int np, float scale) {
-    if (prefill_attn_query_block() == 64)
-      return paged_attention_prefill_tc(qkv, Tcap, QKV, attn, Hq * kD, kv_l, btab, max_blocks_per_seq, pwork, np, Hq, Hkv, scale, stream);
-    return paged_attention(qkv, QKV, attn, Hq * kD, kv_l, btab, max_blocks_per_seq, pwork, np, Hq, Hkv, scale, 0, stream);
+    return paged_attention_prefill_tc(qkv, Tcap, QKV, attn, Hq * kD, kv_l, btab, max_blocks_per_seq, pwork, np, Hq, Hkv, scale, stream);
   }
   // one scheduler iteration = launch (schedule, pack, H2D, kernels, D2H enqueue) + complete (sync, apply) + publish
   int launch(InFlight* f, StepMeta* m);
@@ -343,16 +330,26 @@ struct Engine {
   void finish(std::shared_ptr<Seq> s, int code);
   void admit_prefix(Seq& s);
   const CUtensorMap& xmap(const XMaps& xm, int bn) const { return xm.m[gemm_block_n_index(bn)]; }
-  int gemm(const GemmPlan& p, const XMaps& xm, void* out, int ldo, int T) {
-    const int bn = gemm_block_n_for(T);
-    ++stats.kernel_launches;
-    return gemm_run(p, xmap(xm, bn), bn, out, ldo, T, stream);
+  // one projection launch: out[t, n] = x[t, :] . W[n, :] with the epilogue `epi`; the caller fills the epilogue's fields of p
+  Gemm3Params proj(const GemmPlan& pl, int epi) const {
+    Gemm3Params p;
+    memset(&p, 0, sizeof(p));
+    p.tm_w = pl.tm_w;
+    p.N = pl.N; p.K = pl.K;
+    p.pro = GEMM3_PRO_NONE; p.epi = epi;
+    p.eps = cfg.rms_eps;
+    p.n_valid = pl.N;
+    p.ws = gemm_ws; p.ws_bytes = gemm_ws_bytes;
+    p.counters = gemm_counters; p.counters_cap = gemm_counters_cap;
+    return p;
   }
-  // GEMM that leaves its stream-K segments as fp32 partials for the next kernel to sum (partials.cuh)
-  int gemm_def(const GemmPlan& p, const XMaps& xm, void* out, int ldo, int T, PartialView* pv) {
-    const int bn = gemm_variant() == 2 ? gemm2_block_n_for_plan(p, T) : gemm_block_n_for(T);
+  int launch_proj(Gemm3Params p, const XMaps& xm, int T) {
+    Gemm3Schedule sch;
+    if (int rc = gemm3_schedule(p.N, p.K, T, 0, &sch)) return rc;
+    p.T = T;
+    p.tm_x = xmap(xm, sch.block_n);
     ++stats.kernel_launches;
-    return gemm_run_deferred(p, xmap(xm, bn), bn, out, ldo, T, stream, pv);
+    return gemm3_launch(p, sch, stream);
   }
 };
 
@@ -388,7 +385,7 @@ Engine::~Engine() {
   cudaSetDevice(cfg.device);
   if (stream) cudaStreamSynchronize(stream);
   void* frees[] = {weights_blob, res, x, normed, qkv, attn, gu, act, last_hidden, logits, sampled, gemm_ws,
-                   gemm_counters, kv, ssq, cand, g3_flags, chain_bar, attn_ws};
+                   gemm_counters, kv, cand, attn_ws};
   for (void* p : frees)
     if (p) cudaFree(p);
   for (auto p : stage_dev)
@@ -503,28 +500,38 @@ int Engine::alloc_all() {
   CK(cudaMemset(act, 0, static_cast<size_t>(Tcap) * I * 2));
   CK(cudaMemset(last_hidden, 0, static_cast<size_t>(Scap) * H * 2));
   CK(cudaMallocHost(&sampled_host, static_cast<size_t>(Scap) * 4));
-  CK(cudaMalloc(&ssq, static_cast<size_t>(Tcap) * (H / 128) * 4));
-  CK(cudaMalloc(&cand, static_cast<size_t>(std::min(Scap, 128)) * (V / 128 + 1) * sizeof(float2)));
+  CK(cudaMalloc(&cand, static_cast<size_t>(std::min(Scap, 128)) * ((V + 127) / 128) * sizeof(float2)));
+  // outputs of the last step, readable by name (b200_engine_tensor_read): sampled ids int32 [S]; the lm_head's per-slab
+  // {best logit, index} candidates float2 [S][ceil(V / 128)] when the step sampled through them, else bf16 logits [S][V]
+  tensors["step.sampled"] = {sampled, static_cast<size_t>(Scap) * 4};
+  tensors["step.argmax_candidates"] = {cand, static_cast<size_t>(std::min(Scap, 128)) * ((V + 127) / 128) * sizeof(float2)};
+  tensors["step.logits"] = {logits, static_cast<size_t>(Scap) * V * 2};
   CK(cudaMalloc(&attn_ws, attn_split_ws_bytes(kSplitMaxWork, Hkv, kSplitMaxParts)));
   { const char* e = getenv("B200_ATTN_SPLIT"); attn_split_force = e ? atoi(e) : 0; }
-  gemm2_read_env();
-  CK(cudaMalloc(&g3_flags, 8192 * 4));     // stream-K neighbour flags [0, 4096) + fused-norm row flags [4096, 8192)
-  CK(cudaMemset(g3_flags, 0, 8192 * 4));
-  // split-K workspace: 2 fp32 slots of 512 tokens x 128 rows per CTA (in-kernel fix-up slots == deferred segments)
-  size_t ws_bytes = std::max(std::max(gemm_workspace_bytes(sms), gemm_deferred_ws_bytes(sms)), gemm3_ws_bytes(sms));
-  gemm_ws_bytes = ws_bytes;
-  CK(cudaMalloc(&gemm_ws, ws_bytes));
-  const int maxN = std::max(std::max(QKV, 2 * I), V);
-  const size_t n_counters = 2ull * (maxN / 128 + 2) * (Tcap / 32 + 2);
-  CK(cudaMalloc(&gemm_counters, n_counters * 4));
-  CK(cudaMemset(gemm_counters, 0, n_counters * 4));
+  // split-K workspace and arrival counters: the largest need of any projection at any step size up to Tcap
+  {
+    const int shapes[5][2] = {{QKV, H}, {H, Hq * kD}, {2 * I, H}, {H, I}, {V, H}};
+    size_t ws_bytes = 1 << 20;
+    int counters = 1024;
+    const int t_max = std::max(Tcap, Scap);
+    for (auto& sh : shapes)
+      for (int T = 1;; T = std::min(T < 64 ? 64 : T + 64, t_max)) {   // every token-tile count up to t_max, t_max itself last
+        Gemm3Schedule sch;
+        if (gemm3_schedule(sh[0], sh[1], T, 0, &sch)) return cuda_fail("gemm3_schedule", -1);
+        ws_bytes = std::max(ws_bytes, gemm3_ws_bytes(sh[0], sch, T));
+        counters = std::max(counters, gemm3_counters_needed(sh[0], sch, T));
+        if (T == t_max) break;
+      }
+    gemm_ws_bytes = ws_bytes;
+    gemm_counters_cap = counters;
+  }
+  CK(cudaMalloc(&gemm_ws, gemm_ws_bytes));
+  CK(cudaMalloc(&gemm_counters, static_cast<size_t>(gemm_counters_cap) * 4));
+  CK(cudaMemset(gemm_counters, 0, static_cast<size_t>(gemm_counters_cap) * 4));
 
   // ---- GEMM plans + activation tensor maps (encoded once; kernels mask rows >= T)
   auto plan = [&](GemmPlan* p, const void* W, int N, int K) {
-    int rc = gemm_plan_init(p, W, N, K, K, gemm_ws, gemm_counters, sms);
-    if (rc) return rc;
-    p->ws_bytes = gemm_ws_bytes;
-    return gemm_variant() == 2 ? gemm_plan_build_table(p, std::max(Tcap, Scap)) : 0;
+    return gemm_plan_init(p, W, N, K, K, gemm_ws, gemm_ws_bytes, gemm_counters, gemm_counters_cap);
   };
   for (int l = 0; l < L; ++l) {
     if (plan(&layers[l].p_qkv, layers[l].wqkv, QKV, H) || plan(&layers[l].p_o, layers[l].wo, H, Hq * kD) ||
@@ -532,44 +539,22 @@ int Engine::alloc_all() {
       return cuda_fail("gemm_plan_init", -2);
   }
   if (plan(&p_lm, lm_head, V, H)) return cuda_fail("gemm_plan_init(lm_head)", -2);
-  deferred_ok = gemm_variant() == 2;
-  const int bns[kGemmNumBlockN] = {32, 64, 128, 256, 512};
+  const int bns[kGemmNumBlockN] = {64, 128, 256};
   for (int i = 0; i < kGemmNumBlockN; ++i) {
     if (gemm_make_x_map(&xm_normed.m[i], normed, Tcap, H, H, bns[i]) ||
         gemm_make_x_map(&xm_attn.m[i], attn, Tcap, Hq * kD, Hq * kD, bns[i]) ||
         gemm_make_x_map(&xm_act.m[i], act, Tcap, I, I, bns[i]) ||
-        gemm_make_x_map(&xm_last.m[i], last_hidden, Scap, H, H, bns[i]) ||
-        gemm_make_x_map(&xm_res.m[i], res, Tcap, H, H, bns[i]))
+        gemm_make_x_map(&xm_last.m[i], last_hidden, Scap, H, H, bns[i]))
       return cuda_fail("gemm_make_x_map", -2);
   }
-  // decode-shape fused path: one schedule per projection (cluster split-K or stream-K, gemm3_schedule); any shape it does
-  // not serve keeps the whole engine on the unfused path
+  // A/B knobs: 0 keeps those steps on plain GEMM outputs + the elementwise kernels.  The fused epilogues need whole
+  // 128-row slabs (one head per slab for RoPE, gate/up pairs for SiLU).
   {
-    const char* e = getenv("B200_FUSED_DECODE");   // A/B knob: 0 keeps every step on the unfused kernels
-    const bool want = !(e && atoi(e) == 0) && gemm_variant() == 2;
-    fused_ok = want && QKV % 256 == 0 && H % 256 == 0 && (2 * I) % 256 == 0 && V % 256 == 0 && H <= 4096 &&
-               !gemm3_schedule(QKV, H, 128, GEMM3_PRO_NONE, 0, &sch_qkv) && !gemm3_schedule(H, Hq * kD, 128, GEMM3_PRO_NONE, 0, &sch_o) &&
-               !gemm3_schedule(2 * I, H, 128, GEMM3_PRO_NONE, 0, &sch_gu) && !gemm3_schedule(H, I, 128, GEMM3_PRO_NONE, 0, &sch_down) &&
-               !gemm3_schedule(V, H, 128, GEMM3_PRO_NONE, 0, &sch_lm) && !sch_o.streamk && !sch_down.streamk && H / 128 <= 1024;
-    cudaGetLastError();
-    // the chain needs every CTA co-resident (software grid barrier), the segment tables of the deferred reduction, at least
-    // as many gate_up tiles as ... units are clamped to the tile count, and one token row per CTA
-    // Opt-in (B200_CHAIN=1): on the same box the chain measured 6.42 ms per decode step against 5.95 ms for one fused launch
-    // per projection and 6.14 ms unfused (profiles/r02_decode_paths.md) — its phases stream at the same in-step rate, but the
-    // four barrier gaps (~10 us each) and the lower SM clock under the power cap cost more than the launches it removes.
-    {
-      const char* pe = getenv("B200_FUSED_PREFILL");   // A/B knob: 0 keeps the larger steps on fp32 segments + elementwise kernels
-      fused2_ok = !(pe && atoi(pe) == 0) && gemm_variant() == 2 && QKV % 256 == 0 && H % 256 == 0 && (2 * I) % 256 == 0 && kD == 128 &&
-                  gemm_ws_bytes >= static_cast<size_t>(sms / 2) * 2 * 512 * 128 * sizeof(float);
-    }
-    const char* ce = getenv("B200_CHAIN");
-    chain_ok = fused_ok && deferred_ok && (ce && atoi(ce) != 0) && chain_max_ctas(&chain_ctas) == 0 && chain_ctas >= 128 && chain_ctas >= sms / 2 * 2 &&
-               gemm_ws_bytes >= (48ull << 20) + static_cast<size_t>(chain_ctas) * 128 * 128 * 4;
-    if (chain_ok) {
-      CK(cudaMalloc(&chain_bar, 64));
-      CK(cudaMemset(chain_bar, 0, 64));
-    }
-    cudaGetLastError();
+    const char* fd = getenv("B200_FUSED_DECODE");
+    const char* fp = getenv("B200_FUSED_PREFILL");
+    const bool shapes_ok = QKV % 128 == 0 && (2 * I) % 128 == 0;
+    fused_ok = shapes_ok && !(fd && atoi(fd) == 0);
+    fused2_ok = shapes_ok && !(fp && atoi(fp) == 0);
   }
 
   // ---- KV pool
@@ -643,6 +628,10 @@ int Engine::init(const b200_config& c) {
 }
 
 // ------------------------------------------------------------------ forward pass (fixed kernel sequence)
+// Per layer: RMSNorm -> qkv (+ RoPE / KV write) -> attention -> o_proj (+ residual add) -> RMSNorm -> gate_up (+ SiLU * up)
+// -> down_proj (+ residual add).  With fused epilogues the elementwise op after a projection runs inside it on the rounded
+// bf16 output; without, the same arithmetic runs as a separate kernel on the bf16 tensor (same rounding points, so both forms
+// give the same bits).
 int Engine::forward(const StepMeta& m, int32_t* dbuf, bool all_logits, bf16* logits_out) {
   const int T = m.T;
   const int* ids = dbuf + m.off_ids;
@@ -670,341 +659,76 @@ int Engine::forward(const StepMeta& m, int32_t* dbuf, bool all_logits, bf16* log
     prof_used += 2;
   };
   auto on = [&](int cls) { return !(skip_mask & (1u << cls)); };
-  // Steps of at most 128 tokens (the decode steps: ~80% of the bench's steps, all of them weight streams) run the fused
-  // chain: 4 GEMMs + attention per layer, the split-K reductions finished inside the GEMMs, RMSNorm / RoPE + KV write /
-  // SiLU / residual add / argmax in their prologues and epilogues (gemm3_tcgen05.cu).
-  if (fused_ok && !all_logits && T <= 128 && m.S <= 128) return chain_ok ? forward_chain(m, dbuf) : forward_fused(m, dbuf);
+  const bool fused = !all_logits && (T <= 128 ? fused_ok : fused2_ok);
   P(B200_K_EMBED); if (on(B200_K_EMBED)) rc |= embed_gather(embed, ids, res, T, H, V, stream); Q(); launched(1);
-  // T <= 512: every GEMM dumps fp32 stream-K partials and its consumer (norm / rope / silu / argmax) sums them while
-  // loading — no in-GEMM reduction handshake.  Larger steps use the in-kernel fix-up and bf16 intermediates.
-  static const int defer_max_t = [] {
-    const char* e = getenv("B200_DEFER_MAX_T");  // A/B knob: 0 disables deferred reduction
-    return e ? atoi(e) : (1 << 30);
-  }();
-  const bool dfr = deferred_ok && !all_logits && T <= defer_max_t;
-  PartialView pv_x = no_partials();  // partials of the GEMM whose output is `x` (o_proj / down_proj)
-  // Steps of more than 128 tokens (prefill bursts and mixed steps), per projection: when the launch has at least one
-  // (256-row x token-tile) tile per CTA pair — gate_up at every T, nothing else at Llama-3-8B's shapes — the pair kernel
-  // finishes its few split tiles in-kernel and the elementwise neighbour rides in its epilogue (gemm2 mode 2, epi_pass.cuh).
-  // With fewer tiles than pairs every tile is cut into several pieces and one finisher per tile would serialise the
-  // reduction: those launches keep the fp32 segments and the elementwise consumer that sums them across all SMs (measured:
-  // fusing them too, with 256-token tiles to get enough tiles, is 1.3% slower per step; profiles/r02_prefill_fused.md).
-  // Both forms round at the same points and add the pieces in the same order
-  // (tests/test_fullsize_gpu.py::test_full_size_prefill_burst_step_matches_oracle compares them bit for bit).
-  auto f2_bn = [&](const GemmPlan& pl) {   // token-tile size of the fused form, 0 = keep the segment form
-    if (!fused2_ok || all_logits || !dfr || T <= 128) return 0;
-    const int bn = gemm_block_n_for(T);    // same tiles, ranges and piece order as the segment form: bit-identical results
-    const int ntt = (T + bn - 1) / bn;
-    const int tiles = (pl.N / 256) * ntt;
-    // A/B knob: also fuse the launches that run one whole tile per pair (qkv / o_proj of a burst).  Measured slower: their
-    // epilogue is the tail of the kernel, +170 us of qkv per step against -95 us of RoPE kernel (profiles/r02_prefill_fused.md)
-    static const int whole = [] { const char* e = getenv("B200_F2_WHOLE"); return e ? atoi(e) : 0; }();
-    return (tiles >= pl.max_ctas / 2 || (whole && gemm2_units_for(pl, ntt) == tiles)) ? bn : 0;
+  bool x_pending = false;   // `x` holds a projection output that the next RMSNorm still has to add to the residual
+  auto norm = [&](const bf16* w, bf16* dst, const int* row_index, int n) {
+    if (!x_pending) rc |= rmsnorm(res, nullptr, w, dst, row_index, n, H, cfg.rms_eps, stream);
+    else rc |= rmsnorm(x, res, w, dst, row_index, n, H, cfg.rms_eps, stream);
+    launched(1);
   };
-  auto run_f2 = [&](const GemmPlan& pl, const XMaps& xm, int bn, Gemm2Epi e) {
-    ++stats.kernel_launches;
-    e.flags = g3_flags;
-    e.epoch = ++g3_epoch;
-    return gemm2_run_fused(pl, xmap(xm, bn), bn, T, e, stream);
+  // o_proj / down_proj: residual add in the epilogue, or a bf16 `x` the next RMSNorm adds
+  auto resadd_proj = [&](const GemmPlan& pl, const XMaps& xm) {
+    if (fused) {
+      Gemm3Params p = proj(pl, GEMM3_EPI_RESADD);
+      p.out = res; p.ldo = H;
+      rc |= launch_proj(p, xm, T);
+      x_pending = false;
+    } else {
+      Gemm3Params p = proj(pl, GEMM3_EPI_PLAIN);
+      p.out = x; p.ldo = H;
+      rc |= launch_proj(p, xm, T);
+      x_pending = true;
+    }
   };
-  bool x_pending = false;   // `x` (+ pv_x) holds a projection output that the next RMSNorm still has to add to the residual
   for (int l = 0; l < L && !rc; ++l) {
     Layer& ly = layers[l];
     bf16* kv_l = kv + static_cast<size_t>(l) * kv_layer_elems;
-    P(B200_K_NORM);
-    if (!on(B200_K_NORM)) {}
-    else if (!x_pending) rc |= rmsnorm(res, nullptr, ly.norm1, normed, nullptr, T, H, cfg.rms_eps, stream);
-    else rc |= rmsnorm(x, res, ly.norm1, normed, nullptr, T, H, cfg.rms_eps, stream, pv_x);
-    Q();
-    launched(1);
-    PartialView pv = no_partials();
-    Gemm2Epi e;
-    memset(&e, 0, sizeof(e));
-    if (const int bn = f2_bn(ly.p_qkv)) {
-      e.epi = GEMM3_EPI_ROPE_KV; e.out = qkv; e.ldo = QKV; e.positions = pos; e.slots = slots; e.cos_sin = cos_sin; e.kv_layer = kv_l;
-      e.Hq = Hq; e.Hkv = Hkv; e.max_pos = cfg.max_model_len;
-      P(B200_K_GEMM_QKV); if (on(B200_K_GEMM_QKV)) rc |= run_f2(ly.p_qkv, xm_normed, bn, e); Q();
-    } else {
-      P(B200_K_GEMM_QKV);
-      if (!on(B200_K_GEMM_QKV)) {}
-      else if (dfr) rc |= gemm_def(ly.p_qkv, xm_normed, qkv, QKV, T, &pv); else rc |= gemm(ly.p_qkv, xm_normed, qkv, QKV, T);
-      Q();
-      P(B200_K_ROPE); if (on(B200_K_ROPE)) rc |= rope_kv_write(qkv, pos, slots, cos_sin, kv_l, T, Hq, Hkv, cfg.max_model_len, stream, pv); Q();
-      launched(1);
+    P(B200_K_NORM); if (on(B200_K_NORM)) norm(ly.norm1, normed, nullptr, T); Q();
+    P(B200_K_GEMM_QKV);
+    if (on(B200_K_GEMM_QKV)) {
+      Gemm3Params p = proj(ly.p_qkv, fused ? GEMM3_EPI_ROPE_KV : GEMM3_EPI_PLAIN);
+      p.out = qkv; p.ldo = QKV;
+      p.positions = pos; p.slots = slots; p.cos_sin = cos_sin; p.kv_layer = kv_l; p.Hq = Hq; p.Hkv = Hkv; p.max_pos = cfg.max_model_len;
+      rc |= launch_proj(p, xm_normed, T);
     }
+    Q();
+    if (!fused) { P(B200_K_ROPE); if (on(B200_K_ROPE)) rc |= rope_kv_write(qkv, pos, slots, cos_sin, kv_l, T, Hq, Hkv, cfg.max_model_len, stream); Q(); launched(1); }
     if (m.nd) { P(B200_K_ATTN_DECODE); if (on(B200_K_ATTN_DECODE)) rc |= decode_attention(m, kv_l, btab, dwork, scale); Q(); launched(1); }
     if (m.np) { P(B200_K_ATTN_PREFILL); if (on(B200_K_ATTN_PREFILL)) rc |= prefill_attention(kv_l, btab, pwork, m.np, scale); Q(); launched(1); }
-    memset(&e, 0, sizeof(e));
-    e.epi = GEMM3_EPI_RESADD; e.out = res; e.ldo = H;
-    P(B200_K_GEMM_O);
-    if (const int bn = f2_bn(ly.p_o)) {
-      if (on(B200_K_GEMM_O)) rc |= run_f2(ly.p_o, xm_attn, bn, e);
-      x_pending = false;
-    } else {
-      if (!on(B200_K_GEMM_O)) {}
-      else if (dfr) rc |= gemm_def(ly.p_o, xm_attn, x, H, T, &pv_x); else { rc |= gemm(ly.p_o, xm_attn, x, H, T); pv_x = no_partials(); }
-      x_pending = true;
+    P(B200_K_GEMM_O); if (on(B200_K_GEMM_O)) resadd_proj(ly.p_o, xm_attn); Q();
+    P(B200_K_NORM); if (on(B200_K_NORM)) norm(ly.norm2, normed, nullptr, T); Q();
+    P(B200_K_GEMM_GU);
+    if (on(B200_K_GEMM_GU)) {
+      Gemm3Params p = proj(ly.p_gu, fused ? GEMM3_EPI_SILU : GEMM3_EPI_PLAIN);
+      p.out = fused ? act : gu; p.ldo = fused ? I : 2 * I;
+      rc |= launch_proj(p, xm_normed, T);
     }
     Q();
-    P(B200_K_NORM);
-    if (!on(B200_K_NORM)) {}
-    else if (!x_pending) rc |= rmsnorm(res, nullptr, ly.norm2, normed, nullptr, T, H, cfg.rms_eps, stream);
-    else rc |= rmsnorm(x, res, ly.norm2, normed, nullptr, T, H, cfg.rms_eps, stream, pv_x);
-    Q();
-    launched(1);
-    pv = no_partials();
-    if (const int bn = f2_bn(ly.p_gu)) {
-      Gemm2Epi g;
-      memset(&g, 0, sizeof(g));
-      g.epi = GEMM3_EPI_SILU; g.out = act; g.ldo = I;
-      P(B200_K_GEMM_GU); if (on(B200_K_GEMM_GU)) rc |= run_f2(ly.p_gu, xm_normed, bn, g); Q();
-    } else {
-      P(B200_K_GEMM_GU);
-      if (!on(B200_K_GEMM_GU)) {}
-      else if (dfr) rc |= gemm_def(ly.p_gu, xm_normed, gu, 2 * I, T, &pv); else rc |= gemm(ly.p_gu, xm_normed, gu, 2 * I, T);
-      Q();
-      P(B200_K_SILU); if (on(B200_K_SILU)) rc |= silu_mul(gu, act, T, I, stream, pv, 1); Q();
-      launched(1);
-    }
-    P(B200_K_GEMM_DOWN);
-    if (const int bn = f2_bn(ly.p_down)) {
-      if (on(B200_K_GEMM_DOWN)) rc |= run_f2(ly.p_down, xm_act, bn, e);
-      x_pending = false;
-    } else {
-      if (!on(B200_K_GEMM_DOWN)) {}
-      else if (dfr) rc |= gemm_def(ly.p_down, xm_act, x, H, T, &pv_x); else { rc |= gemm(ly.p_down, xm_act, x, H, T); pv_x = no_partials(); }
-      x_pending = true;
-    }
-    Q();
+    if (!fused) { P(B200_K_SILU); if (on(B200_K_SILU)) rc |= silu_mul(gu, act, T, I, stream, no_partials(), 1); Q(); launched(1); }
+    P(B200_K_GEMM_DOWN); if (on(B200_K_GEMM_DOWN)) resadd_proj(ly.p_down, xm_act); Q();
   }
   if (rc) return cuda_fail("forward", -2);
   if (all_logits) {
-    rc |= rmsnorm(x, res, final_norm, normed, nullptr, T, H, cfg.rms_eps, stream, pv_x);
-    rc |= gemm(p_lm, xm_normed, logits_out, V, T);
-    launched(1);
+    norm(final_norm, normed, nullptr, T);
+    Gemm3Params p = proj(p_lm, GEMM3_EPI_PLAIN);
+    p.out = logits_out; p.ldo = V;
+    rc |= launch_proj(p, xm_normed, T);
   } else if (m.S > 0) {
-    P(B200_K_NORM);
-    if (x_pending) rc |= rmsnorm(x, res, final_norm, last_hidden, rows, m.S, H, cfg.rms_eps, stream, pv_x);
-    else rc |= rmsnorm(res, nullptr, final_norm, last_hidden, rows, m.S, H, cfg.rms_eps, stream);
-    Q();
-    PartialView pv = no_partials();
-    P(B200_K_GEMM_LM);
-    if (dfr && !keep_logits) rc |= gemm_def(p_lm, xm_last, logits, V, m.S, &pv); else rc |= gemm(p_lm, xm_last, logits, V, m.S);
-    Q();
+    P(B200_K_NORM); norm(final_norm, last_hidden, rows, m.S); Q();
+    // argmax candidates per 128-row slab in the lm_head epilogue (the candidate buffer holds 128 rows), or bf16 logits
+    const bool cand_ok = fused && !keep_logits && m.S <= 128;
+    Gemm3Params p = proj(p_lm, cand_ok ? GEMM3_EPI_ARGMAX : GEMM3_EPI_PLAIN);
+    p.out = logits; p.ldo = V; p.cand = cand;
+    P(B200_K_GEMM_LM); rc |= launch_proj(p, xm_last, m.S); Q();
     last_S = m.S;
-    P(B200_K_ARGMAX); rc |= argmax_rows(logits, sampled, m.S, V, V, stream, pv); Q();
-    launched(2);
+    P(B200_K_ARGMAX);
+    if (cand_ok) rc |= argmax_candidates(cand, sampled, m.S, (V + 127) / 128, stream);
+    else rc |= argmax_rows(logits, sampled, m.S, V, V, stream);
+    Q();
+    launched(1);
   }
   if (rc) return cuda_fail("forward(head)", -2);
-  return 0;
-}
-
-// ------------------------------------------------------------------ forward pass, decode-shape fused chain (T <= 128)
-int Engine::forward_fused(const StepMeta& m, int32_t* dbuf) {
-  const int T = m.T;
-  const int* ids = dbuf + m.off_ids;
-  const int* pos = dbuf + m.off_pos;
-  const int* slots = dbuf + m.off_slots;
-  const int* rows = dbuf + m.off_rows;
-  const AttnWork* dwork = reinterpret_cast<const AttnWork*>(dbuf + m.off_dwork);
-  const AttnWork* pwork = reinterpret_cast<const AttnWork*>(dbuf + m.off_pwork);
-  const int* btab = dbuf + m.off_btab;
-  const float scale = 1.0f / sqrtf(static_cast<float>(kD));
-  const int slabs = H / 128;
-  int rc = 0;
-  auto P = [&](int cls) {
-    if (!profiling) return;
-    if (prof_used + 2 > prof_events.size()) {
-      for (int i = 0; i < 2; ++i) { cudaEvent_t e; cudaEventCreate(&e); prof_events.push_back({cls, e}); }
-    }
-    prof_events[prof_used].first = cls;
-    cudaEventRecord(prof_events[prof_used].second, stream);
-  };
-  auto Q = [&]() {
-    if (!profiling) return;
-    cudaEventRecord(prof_events[prof_used + 1].second, stream);
-    prof_used += 2;
-  };
-  auto on = [&](int cls) { return !(skip_mask & (1u << cls)); };
-  auto base = [&](const GemmPlan& pl, const CUtensorMap& tmx, int Tn, int pro, int epi) {
-    Gemm3Params p;
-    memset(&p, 0, sizeof(p));
-    p.tm_w = pl.tm_w;
-    p.tm_x = tmx;
-    p.N = pl.N; p.T = Tn; p.K = pl.K;
-    p.pro = pro; p.epi = epi;
-    p.ssq_in = ssq; p.ssq_slabs = slabs; p.eps = cfg.rms_eps;
-    p.ws = gemm_ws; p.flags = g3_flags; p.epoch = ++g3_epoch;
-    p.n_valid = pl.N;
-    return p;
-  };
-  // embedding rows are the first residual; layer 0's norm is the one standalone RMSNorm of the step — every later norm
-  // rides in the epilogue of the projection that produces its input (o_proj -> norm2, down_proj -> next layer's norm1)
-  P(B200_K_EMBED); if (on(B200_K_EMBED)) rc |= embed_gather(embed, ids, res, T, H, V, stream); Q();
-  P(B200_K_NORM); if (on(B200_K_NORM)) rc |= rmsnorm(res, nullptr, layers[0].norm1, normed, nullptr, T, H, cfg.rms_eps, stream); Q();
-  stats.kernel_launches += 2;
-  for (int l = 0; l < L && !rc; ++l) {
-    Layer& ly = layers[l];
-    bf16* kv_l = kv + static_cast<size_t>(l) * kv_layer_elems;
-    {
-      Gemm3Params p = base(ly.p_qkv, xmap(xm_normed, 128), T, GEMM3_PRO_NONE, GEMM3_EPI_ROPE_KV);
-      p.out = qkv; p.ldo = QKV;
-      p.positions = pos; p.slots = slots; p.cos_sin = cos_sin; p.kv_layer = kv_l; p.Hq = Hq; p.Hkv = Hkv; p.max_pos = cfg.max_model_len;
-      P(B200_K_GEMM_QKV); if (on(B200_K_GEMM_QKV)) rc |= gemm3_launch(p, sch_qkv, stream); Q();
-    }
-    if (m.nd) { P(B200_K_ATTN_DECODE); if (on(B200_K_ATTN_DECODE)) rc |= decode_attention(m, kv_l, btab, dwork, scale); Q(); ++stats.kernel_launches; }
-    if (m.np) { P(B200_K_ATTN_PREFILL); if (on(B200_K_ATTN_PREFILL)) rc |= prefill_attention(kv_l, btab, pwork, m.np, scale); Q(); ++stats.kernel_launches; }
-    {
-      Gemm3Params p = base(ly.p_o, xmap(xm_attn, 128), T, GEMM3_PRO_NONE, GEMM3_EPI_RESADD);
-      p.out = res; p.ldo = H; p.ssq_out = ssq;
-      p.normed_out = normed; p.norm_w_out = ly.norm2; p.row_flags = g3_flags + 4096;
-      P(B200_K_GEMM_O); if (on(B200_K_GEMM_O)) rc |= gemm3_launch(p, sch_o, stream); Q();
-    }
-    {
-      Gemm3Params p = base(ly.p_gu, xmap(xm_normed, 128), T, GEMM3_PRO_NONE, GEMM3_EPI_SILU);
-      p.out = act; p.ldo = I;
-      P(B200_K_GEMM_GU); if (on(B200_K_GEMM_GU)) rc |= gemm3_launch(p, sch_gu, stream); Q();
-    }
-    {
-      Gemm3Params p = base(ly.p_down, xmap(xm_act, 128), T, GEMM3_PRO_NONE, GEMM3_EPI_RESADD);
-      p.out = res; p.ldo = H; p.ssq_out = ssq;
-      if (l + 1 < L) { p.normed_out = normed; p.norm_w_out = layers[l + 1].norm1; p.row_flags = g3_flags + 4096; }
-      P(B200_K_GEMM_DOWN); if (on(B200_K_GEMM_DOWN)) rc |= gemm3_launch(p, sch_down, stream); Q();
-    }
-    stats.kernel_launches += 4;
-  }
-  if (rc) return cuda_fail("forward_fused", -2);
-  if (m.S > 0) {
-    // the residual already holds the summed stream: the final norm is a plain RMSNorm of the sampled rows
-    P(B200_K_NORM); rc |= rmsnorm(res, nullptr, final_norm, last_hidden, rows, m.S, H, cfg.rms_eps, stream); Q();
-    Gemm3Params p = base(p_lm, xmap(xm_last, 128), m.S, GEMM3_PRO_NONE, keep_logits ? GEMM3_EPI_PLAIN : GEMM3_EPI_ARGMAX);
-    p.out = logits; p.ldo = V; p.cand = cand;
-    P(B200_K_GEMM_LM); rc |= gemm3_launch(p, sch_lm, stream); Q();
-    P(B200_K_ARGMAX);
-    if (keep_logits) rc |= argmax_rows(logits, sampled, m.S, V, V, stream);
-    else rc |= argmax_candidates(cand, sampled, m.S, V / 128, stream);
-    Q();
-    last_S = m.S;
-    stats.kernel_launches += 3;
-  }
-  if (rc) return cuda_fail("forward_fused(head)", -2);
-  return 0;
-}
-
-// ------------------------------------------------------------------ forward pass, decode-shape projection chain (T <= 128)
-// embed -> norm -> qkv(0) [gemm3, RoPE + KV write in its epilogue] -> per layer: attention, then ONE persistent launch for
-// o_proj .. next layer's qkv (chain_tcgen05.cu) -> final norm of the sampled rows -> lm_head [gemm3, argmax candidates].
-int Engine::forward_chain(const StepMeta& m, int32_t* dbuf) {
-  const int T = m.T;
-  const int* ids = dbuf + m.off_ids;
-  const int* pos = dbuf + m.off_pos;
-  const int* slots = dbuf + m.off_slots;
-  const int* rows = dbuf + m.off_rows;
-  const AttnWork* dwork = reinterpret_cast<const AttnWork*>(dbuf + m.off_dwork);
-  const AttnWork* pwork = reinterpret_cast<const AttnWork*>(dbuf + m.off_pwork);
-  const int* btab = dbuf + m.off_btab;
-  const float scale = 1.0f / sqrtf(static_cast<float>(kD));
-  int rc = 0;
-  auto P = [&](int cls) {
-    if (!profiling) return;
-    if (prof_used + 2 > prof_events.size()) {
-      for (int i = 0; i < 2; ++i) { cudaEvent_t e; cudaEventCreate(&e); prof_events.push_back({cls, e}); }
-    }
-    prof_events[prof_used].first = cls;
-    cudaEventRecord(prof_events[prof_used].second, stream);
-  };
-  auto Q = [&]() {
-    if (!profiling) return;
-    cudaEventRecord(prof_events[prof_used + 1].second, stream);
-    prof_used += 2;
-  };
-  auto g3 = [&](const GemmPlan& pl, const CUtensorMap& tmx, int Tn, int epi) {
-    Gemm3Params p;
-    memset(&p, 0, sizeof(p));
-    p.tm_w = pl.tm_w;
-    p.tm_x = tmx;
-    p.N = pl.N; p.T = Tn; p.K = pl.K;
-    p.pro = GEMM3_PRO_NONE; p.epi = epi;
-    p.eps = cfg.rms_eps;
-    p.ws = gemm_ws; p.flags = g3_flags; p.epoch = ++g3_epoch;
-    p.n_valid = pl.N;
-    return p;
-  };
-  float* ws_sk = gemm_ws + (48ull << 20) / 4;   // gate_up neighbour slots live behind the deferred segments
-  auto deferred = [&](ChainGemm* g, const GemmPlan& pl, const CUtensorMap& tmx, bf16* out, int ldo) {
-    g->tm_w = pl.tm_w;
-    g->tm_x = tmx;
-    g->N = pl.N; g->K = pl.K;
-    g->units = gemm2_units_for(pl, 1);
-    g->mode = CHAIN_DEFERRED;
-    g->seg_table = pl.seg_table + pl.table_off[1];
-    g->out = out; g->ldo = ldo;
-  };
-  P(B200_K_EMBED); rc |= embed_gather(embed, ids, res, T, H, V, stream); Q();
-  P(B200_K_NORM); rc |= rmsnorm(res, nullptr, layers[0].norm1, normed, nullptr, T, H, cfg.rms_eps, stream); Q();
-  {
-    Gemm3Params p = g3(layers[0].p_qkv, xmap(xm_normed, 128), T, GEMM3_EPI_ROPE_KV);
-    p.out = qkv; p.ldo = QKV;
-    p.positions = pos; p.slots = slots; p.cos_sin = cos_sin; p.kv_layer = kv; p.Hq = Hq; p.Hkv = Hkv; p.max_pos = cfg.max_model_len;
-    P(B200_K_GEMM_QKV); rc |= gemm3_launch(p, sch_qkv, stream); Q();
-  }
-  stats.kernel_launches += 3;
-  for (int l = 0; l < L && !rc; ++l) {
-    Layer& ly = layers[l];
-    bf16* kv_l = kv + static_cast<size_t>(l) * kv_layer_elems;
-    if (m.nd) { P(B200_K_ATTN_DECODE); rc |= decode_attention(m, kv_l, btab, dwork, scale); Q(); ++stats.kernel_launches; }
-    if (m.np) { P(B200_K_ATTN_PREFILL); rc |= prefill_attention(kv_l, btab, pwork, m.np, scale); Q(); ++stats.kernel_launches; }
-    ChainParams c;
-    memset(&c, 0, sizeof(c));
-    const bool last = l + 1 == L;
-    c.n_gemm = last ? 3 : 4;
-    c.T = T;
-    deferred(&c.g[0], ly.p_o, xmap(xm_attn, 128), x, H);
-    c.g[0].wait_barrier = 0; c.g[0].done_barrier = 1; c.g[0].reduce = CHAIN_REDUCE_RESADD_NORM; c.g[0].reduce_barrier = 2; c.g[0].norm_w = ly.norm2;
-    {
-      ChainGemm& g = c.g[1];
-      g.tm_w = ly.p_gu.tm_w; g.tm_x = xmap(xm_normed, 128);
-      g.N = 2 * I; g.K = H;
-      g.units = std::min(chain_ctas / 2, 2 * I / 256);
-      g.mode = CHAIN_SILU;
-      g.out = act; g.ldo = I;
-      g.wait_barrier = 2; g.done_barrier = 3; g.reduce = CHAIN_REDUCE_NONE;
-    }
-    deferred(&c.g[2], ly.p_down, xmap(xm_act, 128), x, H);
-    c.g[2].wait_barrier = 3; c.g[2].done_barrier = 4; c.g[2].reduce = CHAIN_REDUCE_RESADD_NORM;
-    c.g[2].reduce_barrier = last ? 0 : 5; c.g[2].norm_w = last ? nullptr : layers[l + 1].norm1;
-    if (!last) {
-      deferred(&c.g[3], layers[l + 1].p_qkv, xmap(xm_normed, 128), qkv, QKV);
-      c.g[3].wait_barrier = 5; c.g[3].done_barrier = 6; c.g[3].reduce = CHAIN_REDUCE_ROPE_KV; c.g[3].reduce_barrier = 0;
-      c.kv_layer = kv + static_cast<size_t>(l + 1) * kv_layer_elems;
-    }
-    c.ws_def = gemm_ws; c.ws_sk = ws_sk; c.flags = g3_flags; c.epoch = ++g3_epoch;
-    static const int pf = [] { const char* e = getenv("B200_CHAIN_PREFETCH"); return e ? atoi(e) : 32; }();
-    c.prefetch = pf;
-    static const int cdbg = [] { const char* e = getenv("B200_CHAIN_DBG"); return e ? atoi(e) : 0; }();
-    c.dbg = cdbg;
-    c.bar = chain_bar; c.bar_base = chain_bar_count;
-    chain_bar_count += static_cast<unsigned long long>(chain_ctas) * (last ? 4 : 6);
-    c.res = res; c.normed = normed; c.eps = cfg.rms_eps;
-    c.positions = pos; c.slots = slots; c.cos_sin = cos_sin; c.Hq = Hq; c.Hkv = Hkv; c.max_pos = cfg.max_model_len;
-    // profiling: the chain is timed as one unit under the gate_up class (its dominant phase)
-    P(B200_K_GEMM_GU); rc |= chain_launch(c, chain_ctas, stream); Q();
-    ++stats.kernel_launches;
-  }
-  if (rc) return cuda_fail("forward_chain", -2);
-  if (m.S > 0) {
-    P(B200_K_NORM); rc |= rmsnorm(res, nullptr, final_norm, last_hidden, rows, m.S, H, cfg.rms_eps, stream); Q();
-    Gemm3Params p = g3(p_lm, xmap(xm_last, 128), m.S, keep_logits ? GEMM3_EPI_PLAIN : GEMM3_EPI_ARGMAX);
-    p.out = logits; p.ldo = V; p.cand = cand;
-    P(B200_K_GEMM_LM); rc |= gemm3_launch(p, sch_lm, stream); Q();
-    P(B200_K_ARGMAX);
-    if (keep_logits) rc |= argmax_rows(logits, sampled, m.S, V, V, stream);
-    else rc |= argmax_candidates(cand, sampled, m.S, V / 128, stream);
-    Q();
-    last_S = m.S;
-    stats.kernel_launches += 3;
-  }
-  if (rc) return cuda_fail("forward_chain(head)", -2);
   return 0;
 }
 
@@ -1084,11 +808,19 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
   static const bool timing = [] { const char* e = getenv("B200_STEP_TIMING"); return e && atoi(e) != 0; }();
   f->t_enter = timing ? now_s() : 0.0;
   {
+    // arrival order (vLLM's FCFS); with fixed_admission the requests that arrived since the last step join the queue in
+    // a fixed order (prompt content, then length) instead of the order their client threads reached b200_submit
     std::lock_guard<std::mutex> lk(mu_);
+    const size_t first = waiting.size();
     while (!incoming.empty()) {
       waiting.push_back(incoming.front());
       incoming.pop_front();
     }
+    if (fixed_admission)
+      std::stable_sort(waiting.begin() + static_cast<std::ptrdiff_t>(first), waiting.end(),
+                     [](const std::shared_ptr<Seq>& a, const std::shared_ptr<Seq>& b) {
+                       return a->arrival_key != b->arrival_key ? a->arrival_key < b->arrival_key : a->n_prompt < b->n_prompt;
+                     });
   }
   // aborted requests leave first
   {
@@ -1185,7 +917,7 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
       m.kv_tokens += p0 + 1;
       ++f->ndec_seq;
     } else {
-      const int qb = prefill_attn_query_block();   // 64 query tokens per work item on the tensor-core kernel
+      const int qb = kPrefillQueryBlock;
       for (int j = 0; j < n; j += qb) pwork_.push_back({tok + j, std::min(qb, n - j), p0 + j, si});
       m.kv_tokens += p0 + n;  // unique K/V tokens this sequence streams from HBM (query tiles re-read them from L2)
       ++f->npre_seq;
@@ -1432,7 +1164,7 @@ void b200_config_default(b200_config* c) {
   c->rope_theta = 500000.0f;
   c->max_model_len = 2048;
   c->max_num_seqs = 128;
-  c->max_batched_tokens = 1536;  // three 512-token GEMM tiles; throughput is flat 1024..4096, TTFT grows with it (profiles/r01_token_budget_sweep.md)
+  c->max_batched_tokens = 1536;  // six 256-token GEMM tiles; time to first token grows with the budget
   c->num_kv_blocks = 0;
   c->kv_fraction = 0.85f;
   c->enable_prefix_caching = 1;
@@ -1471,6 +1203,7 @@ int b200_submit(b200_engine* e, const int32_t* prompt_ids, int32_t n, const b200
   auto s = std::make_shared<Seq>();
   s->toks.assign(prompt_ids, prompt_ids + n);
   s->n_prompt = n;
+  s->arrival_key = xxh64(prompt_ids, static_cast<size_t>(n) * sizeof(int32_t), 0);
   s->max_tokens = max_tokens;
   s->ignore_eos = sp && sp->ignore_eos;
   if (sp && sp->num_stop_ids > 0 && sp->stop_ids) s->stop_ids.assign(sp->stop_ids, sp->stop_ids + sp->num_stop_ids);
@@ -1484,6 +1217,25 @@ int b200_submit(b200_engine* e, const int32_t* prompt_ids, int32_t n, const b200
   }
   g.cv_work_.notify_one();
   return 0;
+}
+
+int b200_engine_set_fixed_admission(b200_engine* e, int32_t on) {
+  if (!e) { set_error("null engine"); return B200_ERR_INVALID; }
+  std::lock_guard<std::mutex> lk(e->impl.mu_);
+  e->impl.fixed_admission = on != 0;
+  return 0;
+}
+
+int32_t b200_engine_unfinished(b200_engine* e) {
+  if (!e) { set_error("null engine"); return B200_ERR_INVALID; }
+  Engine& g = e->impl;
+  std::lock_guard<std::mutex> lk(g.mu_);
+  int32_t n = 0;
+  for (auto& kv : g.requests) {
+    std::lock_guard<std::mutex> ls(kv.second->m);
+    if (!kv.second->finished) ++n;
+  }
+  return n;
 }
 
 static std::shared_ptr<Seq> find_req(Engine& g, uint64_t id) {
@@ -1792,7 +1544,7 @@ int b200_engine_forward_logits(b200_engine* e, const int32_t* ids, int32_t n, vo
   if (n == 1) { m.nd = 1; h[w] = 0; h[w + 1] = 1; h[w + 2] = 0; h[w + 3] = 0; w += 4; m.off_pwork = w; }
   else {
     m.off_pwork = w;
-    const int qb = prefill_attn_query_block();
+    const int qb = kPrefillQueryBlock;
     for (int j = 0; j < n; j += qb) { h[w] = j; h[w + 1] = std::min(qb, n - j); h[w + 2] = j; h[w + 3] = 0; w += 4; ++m.np; }
   }
   m.off_btab = w;

@@ -1,10 +1,9 @@
-// Host-side plan for the stream-K tcgen05 projection GEMM (gemm_tcgen05.cu).
+// Host-side plan of the projection GEMM (gemm_wgmma.cu) and the tensor-map helpers shared with the attention kernels.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stddef.h>
-
-#include "partials.cuh"
+#include <stdint.h>
 
 namespace b200 {
 
@@ -13,62 +12,27 @@ struct GemmPlan {
   int N, K;
   const void* w_ptr;  // same tensor, raw pointer
   int ldw;
-  float* ws;      // fp32 partial workspace, gemm_workspace_bytes(max_ctas)
-  int* counters;  // 2 ints per output tile, zero-initialised, self-resetting
-  int max_ctas;   // persistent grid size cap (SM count)
-  // deferred reduction (pair kernel): per token-tile-count schedule, {first partial segment, #segments} per tile
-  int2* seg_table;     // device; tables for ntt = 1..max_ntt concatenated
-  int table_off[65];   // offset of the ntt-th table inside seg_table (index ntt, 1-based)
-  int table_segs[65];  // partial segments the ntt-th schedule produces
-  int max_ntt;
-  size_t ws_bytes;     // capacity of ws
+  float* ws;          // fp32 split-K workspace
+  size_t ws_bytes;
+  int* counters;      // zero-initialised, self-resetting
+  int counters_cap;
 };
 
-// variant 2 (default): CTA-pair kernel (gemm2_tcgen05.cu); variant 1: single-CTA kernel (gemm_tcgen05.cu)
+// variant 2 (default): split-K sized to the device; variant 1: every tile over its whole K (no split)
 void gemm_set_variant(int v);
 int gemm_variant();
-constexpr int kGemmNumBlockN = 5;         // token-tile sizes 32, 64, 128, 256, 512 (512: variant 2 only)
-int gemm_block_n_for(int T);              // token-tile size the active variant uses for T tokens
-int gemm_block_n_index(int block_n);      // 0..4
-int gemm_x_box_rows(int block_n);         // rows of the activation TMA box for that tile size
-size_t gemm_workspace_bytes(int max_ctas);
+constexpr int kGemmNumBlockN = 3;         // token-tile sizes 64, 128, 256
+int gemm_block_n_for(int T);              // token-tile size for T tokens
+int gemm_block_n_index(int block_n);      // 0..2
+int num_sms();
 // W row-major [N, K] with leading dimension ldw (elements).
-int gemm_plan_init(GemmPlan* p, const void* W, int N, int K, int ldw, float* ws, int* counters, int max_ctas);
+int gemm_plan_init(GemmPlan* p, const void* W, int N, int K, int ldw, float* ws, size_t ws_bytes, int* counters, int counters_cap);
 // Activation map over X row-major [rows, K] (rows = buffer capacity), for a given token-tile size.
 int gemm_make_x_map(CUtensorMap* tm, const void* X, int rows, int K, int ldx, int block_n);
 // Generic 2-D bf16 tensor map (used by the attention kernel for the paged KV cache).
 int tmap_encode_bf16_2d(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, int box_rows,
                         int box_cols, int swizzle128);
-// 3-D bf16 map (innermost d0 contiguous; strides in elements), box b2 x b1 x b0 with b0 = 64 (128-byte swizzle): the
-// tensor-core prefill attention reads its (token, head) query rows from the fused qkv buffer through it.
-int tmap_encode_bf16_3d(CUtensorMap* tm, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1, uint64_t stride2,
-                        int b0, int b1, int b2);
-// Output map (TMA-store epilogue of the pair kernel): out row-major [rows, N], rows = the T of the launch.
-int gemm_make_out_map(CUtensorMap* tm, const void* out, int rows, int N, int ldo);
-// variant-2 internals (gemm2_tcgen05.cu)
-int gemm2_block_n_for(int T);
-int gemm2_block_n_for_plan(const GemmPlan& p, int T);   // 384-token tiles where they give one whole tile per pair
-int gemm2_x_box_rows(int block_n);
-void gemm2_set_trace(long long* dev_ptr);  // debug: 8 clock64 stamps per CTA, or nullptr
-int gemm2_run(const GemmPlan& p, const CUtensorMap& tm_x, int block_n, void* out, int ldo, int T, cudaStream_t st);
-int gemm2_units_for(const GemmPlan& p, int ntt);
-void gemm2_schedule_query(int N, int K, int T, int sms, int* out8);   // host-only: see gemm2_tcgen05.cu
-void gemm2_read_env();   // (re)read the pair kernel's A/B knobs; called when an engine is created
-// Deferred mode (variant 2): complete tiles go to `out` as bf16, split tiles stay as fp32 segments in p.ws; the
-// consumer kernel reads both through the returned view (partials.cuh).  No in-kernel reduction handshake.
-int gemm_plan_build_table(GemmPlan* p, int max_tokens);   // allocates/uploads the segment tables (once per plan)
-void gemm_plan_destroy(GemmPlan* p);
-size_t gemm_deferred_ws_bytes(int max_ctas);
-int gemm_run_deferred(const GemmPlan& p, const CUtensorMap& tm_x, int block_n, void* out, int ldo, int T, cudaStream_t st,
-                      PartialView* view);
-// Fused mode (variant 2, steps of more than 128 tokens): split tiles are finished inside the kernel by the unit that owns
-// their head and every tile leaves through the fused epilogue `e` (epi_pass.cuh) — no fp32 segments for a consumer kernel.
-struct Gemm2Epi;
-int gemm2_run_fused(const GemmPlan& p, const CUtensorMap& tm_x, int block_n, int T, const Gemm2Epi& e, cudaStream_t st);
-// Generic consumer: out[t, n] = bf16(sum of segments) — used by tests and by paths without a fused consumer.
-int reduce_partials(const PartialView& v, void* out, int ldo, int T, int N, cudaStream_t st);
 // out[t, n] (bf16, leading dimension ldo) for t < T.
-int gemm_run(const GemmPlan& p, const CUtensorMap& tm_x, int block_n, void* out, int ldo, int T,
-             cudaStream_t st);
+int gemm_run(const GemmPlan& p, const CUtensorMap& tm_x, int block_n, void* out, int ldo, int T, cudaStream_t st);
 
 }  // namespace b200

@@ -1,9 +1,11 @@
-// Host interface of the decode-shape fused GEMM (gemm3_tcgen05.cu): one 256-row x T<=128 tile per CTA pair, split-K
-// reduced in-kernel, prologue/epilogue modes that absorb the elementwise kernels around the projections.
+// Host interface of the projection GEMM (gemm_wgmma.cu): out[t, n] = sum_k X[t, k] * W[n, k], one 128-row weight slab x
+// block_n-token tile per CTA, optional split-K reduced in-kernel in a fixed order, prologue/epilogue modes that absorb the
+// elementwise kernels around the projections.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
 
 namespace b200 {
@@ -13,9 +15,8 @@ enum { GEMM3_EPI_PLAIN = 0, GEMM3_EPI_RESADD = 1, GEMM3_EPI_SILU = 2, GEMM3_EPI_
 
 struct Gemm3Params {
   CUtensorMap tm_w;   // weight [N, K] bf16, box 128 rows x 64 cols, 128B swizzle (GemmPlan::tm_w)
-  CUtensorMap tm_x;   // token tile source [rows, K] bf16, box 64 rows x 64 cols: activations, or the residual for PRO_NORM
+  CUtensorMap tm_x;   // token tile source [rows, K] bf16, box block_n rows x 64 cols: activations, or the residual for PRO_NORM
   int N, T, K;
-  int S, streamk;     // filled by gemm3_launch from the schedule
   int pro, epi;
   // PRO_NORM: per (token, slab) sums of squares of the residual, norm weight [K], eps
   const float* ssq_in;
@@ -25,12 +26,11 @@ struct Gemm3Params {
   // epilogue destination: PLAIN out [T, N]; RESADD residual in/out [T, N]; SILU act [T, N/2]; ROPE_KV the fused qkv buffer
   __nv_bfloat16* out;
   int ldo;
-  float* ssq_out;     // RESADD: [T, N/128]
-  // RESADD with the next projection's RMSNorm fused (cluster mode only): normed_out [T, N] (leading dimension ldo) =
-  // RMSNorm(new residual) * norm_w_out; row_flags [4 chunks][N/128] ints stamped with `epoch` when a slab's sums are out
+  float* ssq_out;     // RESADD (optional): [T, ceil(N/128)] sums of squares of the new residual per 128-column slab
+  // RESADD (optional): normed_out [T, N] (leading dimension ldo) = RMSNorm(new residual) * norm_w_out, written by the last CTA
+  // of each token tile once every slab's sums are out
   __nv_bfloat16* normed_out;
   const __nv_bfloat16* norm_w_out;
-  int* row_flags;
   // ROPE_KV
   const int* positions;
   const int* slots;
@@ -40,28 +40,31 @@ struct Gemm3Params {
   // ARGMAX: per (token, 128-row slab) {best logit, index as int bits}; columns >= n_valid are ignored
   float2* cand;
   int n_valid;
-  // stream-K neighbour exchange: fp32 slots [unit][rank][128 tokens][128 rows], one flag per (unit, rank), launch epoch
+  // split-K partials [tile][split][block_n tokens][128 rows] fp32, and one arrival counter per tile plus one per token tile
+  // (zero-initialised, reset by the kernel that uses them)
   float* ws;
-  int* flags;
-  int epoch;
-  int dbg;            // debug switches of the norm prologue (timing experiments only): 1 skip the math, 2 no proxy fence, 4 plain remote arrive
-  long long* trace;   // debug: 8 %globaltimer stamps per CTA (start, after cluster sync, first MMA, last MMA issued, epilogue
-                      // start, before / after the wait for the peers' partials, epilogue done), or nullptr
+  size_t ws_bytes;
+  int* counters;
+  int counters_cap;
 };
 
 struct Gemm3Schedule {
-  int S;        // CTA pairs per 256-row tile (cluster = 2S CTAs); 1 in stream-K mode
-  int streamk;  // contiguous (tile, k-block) ranges over all co-resident pairs
-  int units;    // pairs launched
+  int block_n;  // tokens per tile: 64, 128 or 256
+  int S;        // K-splits per tile
+  int rule;     // which rule chose S: 0 the caller's split count, 1 the device-filling rule for one token tile (T <= 128),
+                // 2 the device-filling rule over several token tiles (T > 128)
   int grid;     // CTAs
 };
 
-// Picks cluster split-K (few tiles) or stream-K (at least as many tiles as co-resident pairs).  <0: shape not served.
-// force: 0 = automatic; 1..4 = cluster mode with that many pairs per tile; -1 = stream-K; -n (n >= 2) = stream-K over n units.
-int gemm3_schedule(int N, int K, int T, int pro, int force, Gemm3Schedule* out);
-int gemm3_smem_bytes(int K, int pro);
+// force (T <= 128): 0 automatic; 1..8 that many K-splits; -1 splits sized to the device; -n (n >= 2) n K-splits.
+// force (T > 128): 0 automatic; >= 64 the requested token-tile size: the kernel uses the largest of 64 / 128 / 256 that
+// does not exceed it (wgmma N is at most 256).  <0: shape or force not served.
+int gemm3_schedule(int N, int K, int T, int force, Gemm3Schedule* out);
+int gemm3_schedule_for(int N, int K, int T, int force, int sms, Gemm3Schedule* out);   // host-only: for a device of `sms` SMs
 int gemm3_launch(const Gemm3Params& p, const Gemm3Schedule& sch, cudaStream_t st);
-constexpr size_t gemm3_ws_bytes(int max_ctas) { return static_cast<size_t>(max_ctas) * 128 * 128 * sizeof(float); }
+// fp32 workspace and counters a launch of this schedule needs
+size_t gemm3_ws_bytes(int N, const Gemm3Schedule& sch, int T);
+int gemm3_counters_needed(int N, const Gemm3Schedule& sch, int T);
 // out[s] = best index over the candidates of row s
 int argmax_candidates(const void* cand, int* out, int S, int slabs, cudaStream_t st);
 

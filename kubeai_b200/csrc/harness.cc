@@ -235,6 +235,9 @@ finished:
   return ok;
 }
 
+// requests the running load generators of this process are about to have in flight (b200_harness_expected_inflight)
+std::atomic<int64_t> g_expected_inflight{0};
+
 // runner.go:263-352
 void run_thread(Transport& tp, const b200_harness_config& cfg, HThread& t) {
   for (auto& m : t.input) {
@@ -342,6 +345,8 @@ void b200_harness_config_default(b200_harness_config* c) {
   c->vocab = 128256;
 }
 
+int64_t b200_harness_expected_inflight(void) { return g_expected_inflight.load(); }
+
 /* The synthetic thread list as JSON in the reference's input format (for sharding across ranks). */
 int64_t b200_harness_synth_threads(const b200_harness_config* cfg, char* buf, size_t cap) {
   if (!cfg) { set_error("null config"); return B200_ERR_INVALID; }
@@ -384,10 +389,22 @@ int b200_harness_run(b200_server* server, const char* host, int32_t port, const 
   tp.server = server;
   if (!server) { tp.host = host; tp.port = port; }
 
-  // runner.go:153-187: semaphore + one worker per thread
+  // runner.go:153-187: semaphore + one worker per thread.  `expected` = conversations in progress + free slots that a
+  // conversation still waiting to start will take: the requests this run is about to have in flight.  It changes only
+  // when a conversation ends with none left to start, so a caller that steps the engine only while the engine holds
+  // exactly that many unfinished requests sees the same batches on every run (b200_harness_expected_inflight).
   std::mutex mu;
   std::condition_variable cv;
   int slots = cfg->max_concurrent_threads;
+  size_t not_started = threads.size();
+  int64_t expected = static_cast<int64_t>(std::min<size_t>(static_cast<size_t>(slots), not_started));
+  g_expected_inflight.fetch_add(expected);
+  auto set_expected = [&](int64_t active) {   // under mu
+    const int64_t e = active + static_cast<int64_t>(std::min<size_t>(static_cast<size_t>(slots), not_started));
+    g_expected_inflight.fetch_add(e - expected);
+    expected = e;
+  };
+  int64_t active = 0;
   std::vector<std::thread> workers;
   workers.reserve(threads.size());
   const double t0 = now_s();
@@ -396,17 +413,21 @@ int b200_harness_run(b200_server* server, const char* host, int32_t port, const 
       std::unique_lock<std::mutex> lk(mu);
       cv.wait(lk, [&] { return slots > 0; });
       --slots;
+      --not_started;
+      set_expected(++active);
     }
     workers.emplace_back([&, i] {
       run_thread(tp, *cfg, threads[i]);
       {
         std::lock_guard<std::mutex> lk(mu);
         ++slots;
+        set_expected(--active);
       }
       cv.notify_one();
     });
   }
   for (auto& w : workers) w.join();
+  g_expected_inflight.fetch_add(-expected);
   const double duration = now_s() - t0;
 
   // runner.go:189-250

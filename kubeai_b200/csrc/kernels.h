@@ -48,10 +48,10 @@ int paged_attention(const void* q, int ldq, void* out, int ldo, const void* kv_l
 size_t attn_split_ws_bytes(int num_work, int Hkv, int parts);
 int attn_decode_split(int num_work, int Hkv, int max_ctx, int sms);
 
-// Chunked-prefill attention on tcgen05 (attention_tc.cu): work items of up to 64 query tokens; q rows are read from the
-// fused qkv buffer [qkv_rows, ldq] through a 3-D TMA map.
+// Chunked-prefill attention on wgmma (attention_wgmma.cu): work items of up to kPrefillQueryBlock query tokens, one CTA per
+// (work item, query head); q rows are read from the fused qkv buffer [qkv_rows, ldq].
+constexpr int kPrefillQueryBlock = 64;
 int paged_attention_prefill_tc(const void* qkv, int qkv_rows, int ldq, void* out, int ldo, const void* kv_layer, const int* block_tables,
                                int max_blocks, const AttnWork* work, int num_work, int Hq, int Hkv, float scale, cudaStream_t st);
-int prefill_attn_query_block();   // query tokens per prefill work item: 64 (tensor-core kernel) or 16 (B200_ATTN_TC=0)
 
 }  // namespace b200

@@ -1,4 +1,4 @@
-// Deferred stream-K reduction: the pair GEMM (gemm2_tcgen05.cu) never reduces split tiles in-kernel.
+// Deferred split-K reduction: a GEMM may leave split tiles unreduced for its consumer kernel.
 // A tile computed entirely by one CTA pair is written as bf16 to the output tensor; a tile whose
 // k-range is shared by several pairs is left as one fp32 segment per pair in an L2-resident
 // workspace.  The consumer kernel (RMSNorm, RoPE, SiLU*mul, argmax, or the generic reducer) sums the

@@ -33,7 +33,7 @@ def gemm(x: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
 
 
 def gemm_deferred(x: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
-    """Pair GEMM in deferred-reduction mode + the generic partial reducer (T <= 512)."""
+    """The engine's form of the product (split-K sized to the device whatever the variant; N % 8 == 0)."""
     _chk(x), _chk(w)
     T, K = x.shape
     N = w.shape[0]
@@ -49,8 +49,9 @@ EPI_PLAIN, EPI_RESADD, EPI_SILU, EPI_ROPE_KV, EPI_ARGMAX = 0, 1, 2, 3, 4
 def gemm3(x, w, T=None, pro=PRO_NONE, epi=EPI_PLAIN, force=0, ssq_in=None, norm_w=None, eps=1e-5, out=None, ssq_out=None,
           positions=None, slots=None, cos_sin=None, kv_layer=None, q_heads=0, kv_heads=0, argmax_out=None, n_valid=0,
           normed_out=None, norm_w_out=None):
-    """The decode-shape fused GEMM (b200_op_gemm3).  x: [rows >= T, K] activations (or the residual for PRO_NORM),
-    w: [N, K].  Returns (out, schedule) with schedule = (pairs per tile, stream-K flag, CTAs)."""
+    """The fused projection GEMM (b200_op_gemm3).  x: [rows >= T, K] activations (or the residual for PRO_NORM),
+    w: [N, K].  Returns (out, schedule) with schedule = (K-splits per tile, rule that chose them: 0 given by `force`,
+    1 device-filling for one token tile, 2 device-filling over several token tiles (T > 128), CTAs)."""
     from ._lib import Gemm3Args
     _chk(x), _chk(w)
     T = x.shape[0] if T is None else T
@@ -145,7 +146,7 @@ def paged_attn(qkv, kv_layer, block_tables, work, q_heads, kv_heads, decode: boo
 
 
 def paged_attn_prefill_tc(qkv, kv_layer, block_tables, work, q_heads, kv_heads, out=None):
-    """Tensor-core chunked-prefill attention; work: int32 [n, 4] = (q_tok0, q_count <= 64, q_pos0, seq)."""
+    """wgmma chunked-prefill attention; work: int32 [n, 4] = (q_tok0, q_count <= 64, q_pos0, seq)."""
     _chk(qkv), _chk(kv_layer), _chk(block_tables, torch.int32), _chk(work, torch.int32)
     T = qkv.shape[0]
     if out is None:

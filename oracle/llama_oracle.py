@@ -56,8 +56,8 @@ def fused_add_rms_norm(x, residual, w, eps):
     (vllm/_custom_ops.py:323-327 -> torch.ops._C.fused_add_rms_norm: `z = input + residual` in scalar_t,
     variance and normalisation from z) and of HF transformers (modeling_llama.py:325,328-329 + :62-67).
     vLLM's python IR op (vllm/ir/ops/layernorm.py:42-60) keeps the fp32 sum instead; the two differ by one
-    double rounding of the normalised value.  The engine follows the CUDA-op form because its decode GEMM epilogues
-    store the summed residual in bf16 and the next GEMM normalises it on load (gemm3_tcgen05.cu)."""
+    double rounding of the normalised value.  The engine follows the CUDA-op form because its GEMM residual-add epilogue
+    stores the summed residual in bf16 and the next RMSNorm normalises that (gemm_wgmma.cu)."""
     z = r(x + residual)
     var = z.pow(2).mean(dim=-1, keepdim=True)
     y = z * torch.rsqrt(var + eps)

@@ -1,4 +1,4 @@
-"""Per-kernel timings on the B200 (CUDA events, L2 flushed between iterations), with cuBLAS /
+"""Per-kernel timings on the GPU (CUDA events, L2 flushed between iterations), with cuBLAS /
 FlashInfer on the same box as the bars to beat (SURVEY.md Appendix B).  Not a bench.py number."""
 import json
 import math
@@ -31,7 +31,7 @@ def timeit(fn, iters=10, warm=3):
 
 
 def gemm_bench():
-    print("== GEMM (stream-K tcgen05) vs cuBLAS, us median, L2 flushed")
+    print("== GEMM (wgmma, split-K) vs cuBLAS, us median, L2 flushed")
     shapes = [("qkv", 6144, 4096), ("o", 4096, 4096), ("gate_up", 28672, 4096), ("down", 4096, 14336),
               ("lm_head", 128256, 4096)]
     for T in (16, 128, 256, 512, 2048):
@@ -50,7 +50,7 @@ def gemm_bench():
 
 
 def gemm3_bench():
-    """decode-shape fused GEMM (plain epilogue) vs the stream-K pair kernel with deferred partials vs cuBLAS, T <= 128"""
+    """fused GEMM (plain epilogue) vs the engine's op-level form vs cuBLAS, T <= 128"""
     print("== gemm3 (in-kernel split-K, T<=128) vs gemm2 deferred (+reducer) vs cuBLAS, us median, L2 flushed")
     shapes = [("qkv", 6144, 4096), ("o", 4096, 4096), ("gate_up", 28672, 4096), ("down", 4096, 14336), ("lm_head", 128256, 4096)]
     for T in (16, 64, 128):
@@ -75,10 +75,10 @@ def gemm3_bench():
 
 
 def large_bench():
-    """steps of more than 128 tokens: the pair kernel with in-kernel finished split tiles (the engine's gate_up form, plain and
+    """steps of more than 128 tokens: the wgmma GEMM with its fused epilogue (the engine's gate_up form, plain and
     SiLU epilogue) and with fp32 segments + the generic reducer (an upper bound for the engine's segment form, whose
     consumer does useful work while it sums) vs cuBLAS"""
-    print("== large steps: pair kernel (fused form / segments+reducer) vs cuBLAS, us median, L2 flushed")
+    print("== large steps: wgmma GEMM (fused epilogue / plain) vs cuBLAS, us median, L2 flushed")
     tf_peak = json.load(open("MEASURED_PEAKS.json")).get("bf16_tflops", 0) if __import__("os").path.exists("MEASURED_PEAKS.json") else 0
     shapes = [("qkv", 6144, 4096), ("o", 4096, 4096), ("gate_up", 28672, 4096), ("down", 4096, 14336)]
     for T in (256, 512, 1408, 2048):
@@ -98,7 +98,7 @@ def large_bench():
 def attn_prefill_bench():
     """chunked-prefill attention (tensor-core kernel, 64-query work items) vs FlashInfer's paged prefill on burst-like shapes:
     (requests, cached prefix, new tokens)"""
-    print("== paged prefill attention, Hq=32/Hkv=8: (requests x [cached + new]) mine (tcgen05) / mine (mma.sync) / FlashInfer")
+    print("== paged prefill attention, Hq=32/Hkv=8: (requests x [cached + new]) mine (wgmma) / mine (mma.sync) / FlashInfer")
     Hq, Hkv, D = 32, 8, 128
     for nreq, cached, new in ((10, 320, 130), (4, 0, 384), (1, 0, 1536), (3, 1500, 500), (24, 400, 64)):
         ctx = cached + new
@@ -120,7 +120,7 @@ def attn_prefill_bench():
                 res[name] = (timeit(lambda: fn(qkv, kv, perm, wt, Hq, Hkv, out=out)), out)
             else:
                 res[name] = (timeit(lambda: ops.paged_attn(qkv, kv, perm, wt, Hq, Hkv, False, out=out)), out)
-        line = f"{nreq:3d} x [{cached:4d} + {new:4d}]  tcgen05 {res['tc'][0]:7.1f} us   mma.sync {res['mma'][0]:7.1f} us"
+        line = f"{nreq:3d} x [{cached:4d} + {new:4d}]  wgmma {res['tc'][0]:7.1f} us   mma.sync {res['mma'][0]:7.1f} us"
         try:
             import flashinfer
             ws = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")

@@ -7,7 +7,7 @@ x = torch.randn(T, K, device="cuda").bfloat16()
 w = (torch.randn(N, K, device="cuda") / math.sqrt(K)).bfloat16()
 flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
 mode = sys.argv[4] if len(sys.argv) > 4 else "plain"
-if mode == "gemm3_silu":      # the decode path's dominant launch: gate_up, stream-K, SiLU*up epilogue
+if mode == "gemm3_silu":      # the decode path's dominant launch: gate_up with the SiLU*up epilogue
     fn = lambda x, w: ops.gemm3(x, w, epi=ops.EPI_SILU)
 elif mode == "gemm3_resadd":  # o_proj / down_proj: cluster split-K, residual add + fused RMSNorm
     res = torch.randn(T, N, device="cuda").bfloat16()

@@ -1,5 +1,5 @@
 // Package b200engine is the cgo binding a KubeAI maintainer adds (internal/b200engine/engine.go) to serve
-// /openai/v1/chat/completions and /openai/v1/completions from the in-process B200 engine instead of proxying to a backend
+// /openai/v1/chat/completions and /openai/v1/completions from the in-process H100 engine instead of proxying to a backend
 // pod (internal/modelproxy/handler.go:96-159, internal/manager/run.go:267-275).
 //
 // It binds include/b200engine.h one to one; no logic lives here.  This image has no Go toolchain, so the file is

@@ -336,15 +336,15 @@ def test_create_time_validation_of_pool_and_shapes():
 
 
 def test_decode_paths_agree_token_for_token(oracle, monkeypatch):
-    """The three decode paths — unfused kernels (B200_FUSED_DECODE=0), one fused launch per projection (default) and the
-    persistent projection chain (B200_CHAIN=1) — keep the same rounding points and segment orders: same greedy streams, and
-    all of them the oracle's wherever its margin is not a rounding coin-flip."""
+    """The two decode paths — unfused kernels (B200_FUSED_DECODE=0) and one fused launch per projection (default) — keep
+    the same rounding points and split-K orders: same greedy streams, and both the oracle's wherever its margin is not a
+    rounding coin-flip."""
     from kubeai_b200.engine import Engine, mini_config
     rng = np.random.default_rng(11)
     prompts = [rng.integers(0, 512, size=n).tolist() for n in (5, 17, 40, 64, 90, 121, 33, 8)]
     outs = {}
-    for name, env in (("unfused", {"B200_FUSED_DECODE": "0"}), ("per_gemm", {}), ("chain", {"B200_CHAIN": "1"})):
-        for k in ("B200_FUSED_DECODE", "B200_CHAIN"):
+    for name, env in (("unfused", {"B200_FUSED_DECODE": "0"}), ("per_gemm", {})):
+        for k in ("B200_FUSED_DECODE",):
             monkeypatch.delenv(k, raising=False)
         for k, v in env.items():
             monkeypatch.setenv(k, v)
@@ -353,9 +353,8 @@ def test_decode_paths_agree_token_for_token(oracle, monkeypatch):
             st = e.stats()
             outs[name + "_launches"] = st.kernel_launches
     assert outs["per_gemm"] == outs["unfused"]
-    assert outs["chain"] == outs["unfused"]
-    assert outs["chain_launches"] < outs["per_gemm_launches"] < outs["unfused_launches"]
-    for p, o in zip(prompts, outs["chain"]):
+    assert outs["per_gemm_launches"] < outs["unfused_launches"]
+    for p, o in zip(prompts, outs["per_gemm"]):
         w, rows = oracle.generate(p, 20)
         for j, (a, b) in enumerate(zip(o, w)):
             srt = torch.sort(rows[j])[0]

@@ -1,6 +1,6 @@
-"""GPU parity of the decode-shape fused GEMM (kubeai_b200/csrc/gemm3_tcgen05.cu) through the C ABI (b200_op_gemm3):
-the plain product against the oracle's GEMM for every reduction schedule (cluster split-K with 1..4 CTA pairs per tile
-through distributed shared memory, stream-K with the neighbour exchange through L2), then every prologue / epilogue mode
+"""GPU parity of the fused projection GEMM (kubeai_b200/csrc/gemm_wgmma.cu) through the C ABI (b200_op_gemm3): the plain
+product against the oracle's GEMM for every reduction schedule (1..4 K-splits per tile, split counts sized to the device,
+chosen split counts; the partials summed in-kernel in split order), then every prologue / epilogue mode
 against the oracle's op applied to the kernel's own plain output — bit-exact, because the fused modes must round exactly
 where the separate kernels (and the reference backend) round."""
 import math
@@ -64,7 +64,7 @@ def test_plain_product_matches_oracle_for_every_cluster_schedule(T, N, K, force)
     try:
         got, sch = ops.gemm3(x, w, force=force)
     except B200Error:
-        if force in (3, 4):       # this many pairs per tile do not fit the device for this tile count (or K too shallow)
+        if force in (3, 4):       # more splits than k-blocks
             pytest.skip(f"schedule {force} not available for N={N} K={K}")
         raise
     torch.cuda.synchronize()
@@ -74,20 +74,21 @@ def test_plain_product_matches_oracle_for_every_cluster_schedule(T, N, K, force)
 
 
 @pytest.mark.parametrize("T,N,K,force", [
-    (128, 28672, 4096, 0),      # gate_up: automatic choice must be stream-K
+    (128, 28672, 4096, 0),      # gate_up: more slabs than SMs, whole-K tiles
     (77, 128256, 4096, 0),      # lm_head
-    (128, 20480, 256, -1),      # 80 tiles x 4 k-blocks over all pairs: almost every tile is shared
-    (50, 20480, 512, -7),       # few units: long runs of complete tiles between shared ones
-    (128, 2560, 1024, -10),     # exactly one tile per unit: no shared tile at all
+    (128, 20480, 256, -1),      # split count from the device rule, 4 k-blocks per tile
+    (50, 20480, 512, -7),       # 7 splits of 8 k-blocks: uneven pieces
+    (128, 2560, 1024, -10),     # 10 splits of 16 k-blocks
     (16, 5120, 640, -9),
 ])
 def test_plain_product_matches_oracle_under_stream_k(T, N, K, force):
+    """Split-K over many tiles (the name predates the split-K kernel): device-sized and given split counts."""
     from kubeai_b200 import ops
     x, w = rnd(T, K, seed=3), rnd(N, K, scale=1 / math.sqrt(K), seed=4)
-    for rep in range(3):          # repeated launches: the epoch-stamped flags must never leak between launches
+    for rep in range(3):          # repeated launches: the split-K arrival counters must reset after every launch
         got, sch = ops.gemm3(x, w, force=force)
         torch.cuda.synchronize()
-        assert sch[1] == 1
+        assert sch[1] == (1 if force in (0, -1) else 0) and (force in (0, -1) or sch[0] == -force)
         close(got, ref_gemm(x, w), f"T={T} N={N} K={K} schedule {sch} rep {rep}")
 
 
@@ -103,7 +104,7 @@ def test_norm_prologue_equals_rmsnorm_then_gemm(T, N, K, force):
     """PRO_NORM: the B operand is RMSNorm(residual) computed in shared memory from the per-slab sums of squares."""
     from kubeai_b200 import B200Error, ops
     if (force == -1) != (N >= 20480):
-        pytest.skip("stream-K shapes with the stream-K schedule, cluster shapes with cluster schedules")
+        pytest.skip("the wide shapes with the device-sized split count, the narrow ones with given split counts")
     res = rnd(T, K, scale=2.0, seed=5)
     nw = (1.0 + 0.1 * torch.randn(K, device="cuda", generator=torch.Generator(device="cuda").manual_seed(6))).bfloat16()
     w = rnd(N, K, scale=1 / math.sqrt(K), seed=7)
@@ -111,7 +112,7 @@ def test_norm_prologue_equals_rmsnorm_then_gemm(T, N, K, force):
         got, sch = ops.gemm3(res, w, pro=ops.PRO_NORM, ssq_in=_ssq(res), norm_w=nw, eps=1e-5, force=force)
     except B200Error:
         if force == 4:
-            pytest.skip("4 pairs per tile not available here")
+            pytest.skip("4 splits need at least 4 k-blocks")
         raise
     torch.cuda.synchronize()
     h = O.rms_norm(res.float(), nw.float(), 1e-5)
@@ -136,7 +137,7 @@ def test_residual_add_epilogue(T, N, K, force):
         (res, ssq), sch = ops.gemm3(x, w, epi=ops.EPI_RESADD, out=res, force=force)
     except B200Error:
         if force == 4:
-            pytest.skip("4 pairs per tile not available here")
+            pytest.skip("4 splits need at least 4 k-blocks")
         raise
     torch.cuda.synchronize()
     want = O.r(plain.float() + res0.float())                 # bf16(bf16(acc) + residual): the rounded sum is the new residual
@@ -255,20 +256,21 @@ def test_argmax_epilogue_equals_argmax_of_the_plain_logits(T, N, K, force, n_val
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# steps of more than 128 tokens: the pair kernel (gemm2) in fused mode — several 256/512-token tiles, stream-K over all
-# pairs, split tiles finished in-kernel by the unit that owns their head, the same epilogues
+# steps of more than 128 tokens: several token tiles per launch (force = requested token-tile size: the largest of
+# 64 / 128 / 256 that does not exceed it),
+# the same epilogues
 LARGE = [
-    (300, 4096, 4096, 0),       # one 512-token tile per weight tile: 16 tiles over 74 units, every tile split 4-5 ways
-    (1408, 4096, 4096, 0),      # 3 token tiles, the last one ragged (384)
+    (300, 4096, 4096, 0),       # two 256-token tiles, the last one ragged (44)
+    (1408, 4096, 4096, 0),      # 6 token tiles, the last one ragged (128)
     (1536, 6144, 4096, 0),
     (700, 4096, 14336, 0),      # down_proj, deep K
     (129, 512, 512, 0),         # mini-model shapes
     (513, 768, 512, 0),
-    (1000, 2560, 1024, 256),    # 256-token tiles (two accumulator stages)
-    (2048, 28672, 4096, 0),     # gate_up at the largest step: 448 tiles, ~6 per unit
-    (1408, 4096, 4096, 384),    # 384-token tiles (256 + 128 tokens per k-step): o_proj of a burst as 64 whole tiles
+    (1000, 2560, 1024, 256),    # 256-token tiles given explicitly
+    (2048, 28672, 4096, 0),     # gate_up at the largest step: 1792 tiles
+    (1408, 4096, 4096, 384),    # a wider request than the widest tile: 256-token tiles (the largest supported <= 384)
     (1340, 6144, 4096, 384),    # ragged last tile
-    (900, 28672, 4096, 384),    # three 384-token tiles per weight tile, waves + stream-K tail
+    (900, 28672, 4096, 384),
 ]
 
 
@@ -279,7 +281,7 @@ def test_large_step_plain_product_matches_oracle(T, N, K, bn):
     for rep in range(2):
         got, sch = ops.gemm3(x, w, force=bn)
         torch.cuda.synchronize()
-        assert sch[1] == 2
+        assert sch[1] == 2 and sch[2] % ((N + 127) // 128) == 0
         close(got, ref_gemm(x, w), f"T={T} N={N} K={K} schedule {sch} rep {rep}")
 
 

@@ -1,6 +1,5 @@
 """AddressSanitizer + UndefinedBehaviorSanitizer and ThreadSanitizer builds of the host-only parts of the library (router,
-tokenizer, JSON parser) driven by tests/native/host_sanitize.cc (SURVEY.md §5: race detection / memory checking on the path;
-the GPU side has compute-sanitizer runs under profiles/).  CPU only; skipped when g++ has no sanitizer runtime."""
+tokenizer, JSON parser) driven by tests/native/host_sanitize.cc (SURVEY.md §5: race detection / memory checking on the path).  CPU only; skipped when g++ has no sanitizer runtime."""
 import shutil
 import subprocess
 from pathlib import Path

@@ -34,7 +34,7 @@ def rnd(*shape, scale=1.0, seed=0):
 
 @pytest.fixture(params=[2, 1], ids=["pair", "single"])
 def gemm_variant(request):
-    """2 = CTA-pair kernel (default product path), 1 = single-CTA kernel kept for A/B measurements."""
+    """2 = split-K sized to the device (default product path), 1 = every tile over its whole K."""
     from kubeai_b200 import lib
     lib().b200_set_gemm_variant(request.param)
     yield request.param
@@ -74,7 +74,7 @@ def test_gemm_matches_oracle(T, N, K, gemm_variant):
                                    (2048, 4096, 4096), (1100, 768, 512), (700, 6144, 4096),
                                    (2048, 6144, 4096), (1800, 28672, 4096)])
 def test_gemm_deferred_reduction_matches_oracle(T, N, K):
-    """The engine's path: complete tiles as bf16, split tiles as fp32 stream-K segments summed by the consumer."""
+    """The engine's path: split-K partials summed in-kernel in split order."""
     from kubeai_b200 import ops
     x, w = rnd(T, K, seed=1), rnd(N, K, scale=1 / math.sqrt(K), seed=2)
     got = ops.gemm_deferred(dev(x), dev(w))
@@ -268,7 +268,7 @@ def test_paged_attention_prefill(case):
 ])
 @pytest.mark.parametrize("Hkv", [1, 2])
 def test_paged_attention_prefill_tensor_core(case, Hkv):
-    """attention_tc.cu: 64-query blocks, S and P V on tcgen05 (V as an MN-major operand), against the oracle."""
+    """64-query prefill work items (each served by four 16-query mma.sync CTAs), against the oracle."""
     from kubeai_b200 import ops
     Hq = 4 * Hkv
     seq_lens = [c[0] for c in case]

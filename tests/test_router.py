@@ -254,7 +254,7 @@ def test_hash_lookup_metrics_follow_the_reference_instruments():
 
 
 def test_closed_loop_least_load_is_sticky_like_prefix_hash():
-    """The routing experiment's side finding (profiles/r02_routing.md): in a closed-loop load generator a conversation's next
+    """A side finding of the live routing experiment (DESIGN.md §6): in a closed-loop load generator a conversation's next
     turn is issued when its previous turn finishes, i.e. on the endpoint that just lost one in-flight request — so LeastLoad
     keeps most conversations where their KV prefix is, without looking at the prefix.  Event simulation on the native
     router: 8 endpoints, 64 conversations of 12 turns, service times with jitter."""

@@ -1,67 +1,58 @@
-"""Host-side scheduling rules of the large-step projection GEMM and of split-KV decode attention, through the C ABI without
-a GPU (b200_schedule_query / b200_attn_split_query are pure host functions).  These are the decisions DESIGN.md §4 and
-profiles/r02_prefill_fused.md describe for Llama-3-8B on a 148-SM part; the test pins them so that a change of a threshold
-shows up as a diff here and not as a silent 5 % in the bench."""
+"""Host-side scheduling rules of the projection GEMM and of split-KV decode attention, through the C ABI without a GPU
+(b200_schedule_query / b200_attn_split_query are pure host functions).  These are the decisions DESIGN.md §4 describes for
+Llama-3-8B on a 132-SM H100; the test pins them so that a change of a threshold shows up as a diff here and not as a silent
+few percent in the bench."""
 import ctypes as C
 
 import pytest
 
 from kubeai_b200._lib import lib
 
-SMS = 148
-QKV, O, GATE_UP, DOWN = (6144, 4096), (4096, 4096), (28672, 4096), (4096, 14336)
+SMS = 132
+QKV, O, GATE_UP, DOWN, LM_HEAD = (6144, 4096), (4096, 4096), (28672, 4096), (4096, 14336), (128256, 4096)
 
 
 def q(shape, T, sms=SMS):
     out = (C.c_int32 * 8)()
     assert lib().b200_schedule_query(shape[0], shape[1], T, sms, out) == 0
-    keys = ("block_n", "token_tiles", "tiles", "pairs", "whole", "fused", "waves")
-    return dict(zip(keys, list(out)[:7]))
+    keys = ("block_n", "token_tiles", "tiles", "splits", "ctas", "rule")
+    return dict(zip(keys, list(out)[:6]))
+
+
+def test_decode_step_splits_k_until_the_device_is_full():
+    # o_proj / down_proj: 32 slabs of 128 rows -> 4 K-splits = 128 CTAs on 132 SMs
+    for shape in (O, DOWN):
+        s = q(shape, 128)
+        assert (s["block_n"], s["tiles"], s["splits"], s["ctas"], s["rule"]) == (128, 32, 4, 128, 1), (shape, s)
+    # qkv: 48 slabs -> 2 splits (3 would need a second wave of 12 CTAs)
+    assert (q(QKV, 128)["splits"], q(QKV, 128)["ctas"]) == (2, 96)
+    # gate_up and lm_head have more slabs than SMs: whole-K tiles, the split count is the device's choice
+    for shape in (GATE_UP, LM_HEAD):
+        s = q(shape, 77)
+        assert (s["splits"], s["rule"]) == (1, 1), (shape, s)
 
 
 def test_prefill_burst_of_1340_tokens():
-    # qkv: 24 weight tiles x 3 token tiles = 72 for 74 pairs -> one whole tile per pair, no split tile, not fused
-    s = q(QKV, 1340)
-    assert (s["block_n"], s["tiles"], s["pairs"], s["whole"], s["fused"]) == (512, 72, 72, 1, 0)
-    # o_proj: 48 tiles of 512 tokens would idle a third of the pairs -> 384-token tiles, 64 whole tiles
+    # the token tile follows the step size; a 1340-token burst is 6 tiles of 256 per slab, more tiles than SMs: no split
+    assert [q(O, T)["block_n"] for T in (1, 64, 65, 128, 129, 2048)] == [64, 64, 128, 128, 256, 256]
     s = q(O, 1340)
-    assert (s["block_n"], s["token_tiles"], s["tiles"], s["pairs"], s["whole"], s["fused"]) == (384, 4, 64, 64, 1, 0)
-    # gate_up: 336 tiles -> fused SiLU epilogue, 4 whole-tile waves (296 tiles) + stream-K over the last 40
-    s = q(GATE_UP, 1340)
-    assert (s["block_n"], s["tiles"], s["pairs"], s["whole"], s["fused"], s["waves"]) == (512, 336, 74, 0, 1, 4)
-    # down_proj: deep K (224 k-blocks per tile), 48 tiles: stream-K over all pairs, fp32 segments for the RMSNorm that follows
-    s = q(DOWN, 1340)
-    assert (s["block_n"], s["tiles"], s["pairs"], s["whole"], s["fused"]) == (512, 48, 74, 0, 0)
+    assert (s["token_tiles"], s["tiles"], s["splits"], s["rule"]) == (6, 192, 1, 2)
 
 
-def test_a_short_stream_k_tail_takes_a_whole_wave_with_it():
-    # T = 2048: 448 gate_up tiles = 6 waves + 4 tiles; 4 tiles over 74 pairs would be ~18 pieces each -> 5 waves + 78 tiles
-    s = q(GATE_UP, 2048)
-    assert (s["tiles"], s["pairs"], s["waves"]) == (448, 74, 5)
-    # exactly a multiple of the pairs: no tail at all
-    assert q((74 * 256, 4096), 512 * 3)["waves"] == 3
+def test_every_split_keeps_at_least_four_k_blocks():
+    s = q((256, 512), 16)            # 2 slabs would take 66 splits; 8 k-blocks allow 2
+    assert (s["splits"], s["ctas"]) == (2, 4)
+    assert q((256, 128), 16)["splits"] == 1
 
 
-def test_mid_size_steps_fuse_only_gate_up():
-    for T in (129, 200, 256, 257, 400, 512):
-        assert q(GATE_UP, T)["fused"] == 1 and q(GATE_UP, T)["token_tiles"] == 1
-        for shape in (QKV, O, DOWN):
-            s = q(shape, T)
-            assert s["fused"] == 0 and s["whole"] == 0 and s["pairs"] == 74, (shape, T, s)
-    assert q(GATE_UP, 200)["block_n"] == 256 and q(GATE_UP, 300)["block_n"] == 512
-
-
-def test_384_token_tiles_only_where_they_fill_more_pairs_with_whole_tiles():
-    s = q(O, 1100)                                                              # 3 x 16 tiles either way: stays at 512
-    assert (s["block_n"], s["tiles"], s["whole"]) == (512, 48, 1)
-    assert q(O, 1200)["block_n"] == 384 and q(O, 1200)["tiles"] == 64           # 4 x 16 of 384 against 3 x 16 of 512
-    assert q(QKV, 1340)["block_n"] == 512                                       # 96 tiles of 384 would exceed the 74 pairs
-    assert q(DOWN, 1340)["block_n"] == 512                                      # deep K: balance matters more than pieces
-    assert q(O, 600)["block_n"] == 512                                          # 2 x 16 tiles: too few either way
+def test_split_count_scales_with_the_device():
+    assert q(O, 128, sms=148)["splits"] == 4 and q(O, 128, sms=64)["splits"] == 2 and q(QKV, 128, sms=16)["splits"] == 1
 
 
 @pytest.mark.parametrize("nwork,ctx,want", [(128, 450, 1), (19, 2000, 1), (1, 2000, 16), (1, 100, 1), (4, 2000, 10), (16, 2000, 3),
                                             (1, 300, 3), (8, 1000, 5)])
 def test_split_kv_parts(nwork, ctx, want):
-    # about two CTAs per SM, at least two 64-token tiles per part, never when the grid already fills the device
-    assert lib().b200_attn_split_query(nwork, 8, ctx, SMS) == want
+    # about two CTAs per SM, at least two 64-token tiles per part, never when the grid already fills the device (a pure
+    # function of the SM count: pinned for 148 SMs; the H100's 132 gives 9 parts instead of 10 for 4 sequences)
+    assert lib().b200_attn_split_query(nwork, 8, ctx, 148) == want
+    assert lib().b200_attn_split_query(4, 8, 2000, SMS) == 9

@@ -7,9 +7,8 @@ minutes to start).  Two things are compared on >= 32 prompts:
     next token and its top-k) against log_softmax of the engine's bf16 logits at that position.  Stated tolerance:
     |d logprob| <= LOGPROB_ULPS bf16 ulps of the position's largest |logit| (ulp_bf16(x) = 2^(floor(log2|x|) - 7): 0.0625 at
     |x| in 8..16, 0.125 at 16..32) — two correct bf16 pipelines differ by the rounding of the final 4096-term dot product
-    (1 ulp) plus what the layers' bf16 intermediates feed into it.  First run on a B200 (profiles/r02_vllm_parity.md): max
-    |d logprob| 0.20 on the 2-layer model (3.2 ulps), 0.50 on the 32-layer Llama-3-8B shape (4 ulps), means 0.03 / 0.08,
-    i.e. under one ulp.  The measured maxima of every run go to gpurun_out/vllm_parity.json.
+    (1 ulp) plus what the layers' bf16 intermediates feed into it.  The measured maxima of every run go to the JSON
+    report (REPORT).
   * greedy TOKENS: streams may part only where vLLM's own top-2 candidates are within MARGIN_ULPS bf16 ulps of the top
     logit of each other.  MARGIN_ULPS = 4 is the measured bound on how far ONE logit of the 32-layer model moves between the
     two pipelines (max |d logprob| 3.7-4 ulps over three runs): a margin below it can flip.  Observed first-difference
