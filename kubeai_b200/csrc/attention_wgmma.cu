@@ -109,7 +109,7 @@ __global__ void __launch_bounds__(128) prefill_attn_wgmma_kernel(const __nv_bflo
       wgmma_m64n64(s, gmma_desc(aq + off), gmma_desc(ak + off));
     }
     wgmma_commit();
-    wgmma_wait0();
+    wgmma_wait<0>();
 
     // ---- causal mask + online softmax (scaled to log2 units)
     float mx0 = m0, mx1 = m1;
@@ -164,7 +164,7 @@ __global__ void __launch_bounds__(128) prefill_attn_wgmma_kernel(const __nv_bflo
 #pragma unroll
       for (int j = 0; j < 2; ++j) wgmma_m64n64_rs(o[j], pa[kk], gmma_desc(av + j * kHalf + kk * 32));
     wgmma_commit();
-    wgmma_wait0();
+    wgmma_wait<0>();
   }
 
   // ---- normalise and store

@@ -21,6 +21,8 @@
 #include <stdint.h>
 #include <string.h>
 
+#include <type_traits>
+
 #include "gemm.h"
 #include "gemm3.h"
 #include "launch.h"
@@ -56,6 +58,15 @@ __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;"
 __device__ __forceinline__ float bf16r(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
 __device__ __forceinline__ float ldbf(const __nv_bfloat16* p) { return __bfloat162float(*p); }
 
+// f(integral_constant<W>) with W the narrowest of 64, 128, .., BN that is >= nw (nw a multiple of 64, <= BN)
+template <int BN, class F>
+__device__ __forceinline__ void dispatch_width(int nw, F&& f) {
+  if constexpr (BN > 64) {
+    if (nw <= BN - 64) return dispatch_width<BN - 64>(nw, f);
+  }
+  f(std::integral_constant<int, BN>{});
+}
+
 template <int BN>
 __global__ void __launch_bounds__(kThreads, 1) gemm_wgmma_kernel(const __grid_constant__ Gemm3Params P, int S) {
   using C = Cfg<BN>;
@@ -70,8 +81,11 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_wgmma_kernel(const __grid_co
   float* stg = reinterpret_cast<float*>(smem);                                         // [BN][kPitch] after the main loop
 
   const int tid = threadIdx.x;
-  const int tiles_n = gridDim.x, ntt = gridDim.y;
-  const int n0 = blockIdx.x * kSlab, t0 = blockIdx.y * BN, split = blockIdx.z;
+  const int tiles_n = (P.N + kSlab - 1) / kSlab, ntt = (P.T + BN - 1) / BN;
+  // several token tiles: the token tile is the fastest-varying CTA index (grid (ntt, slabs, S)), so the CTAs that share a
+  // weight slab run together and read it from HBM once.  One token tile: grid (slabs, 1, S).
+  const int slab = ntt > 1 ? blockIdx.y : blockIdx.x, tt = ntt > 1 ? blockIdx.x : 0;
+  const int n0 = slab * kSlab, t0 = tt * BN, split = blockIdx.z;
   const int KB = (P.K + kBlockK - 1) / kBlockK;
   const int kb0 = static_cast<int>(static_cast<long long>(split) * KB / S);
   const int kb1 = static_cast<int>(static_cast<long long>(split + 1) * KB / S);
@@ -92,13 +106,15 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_wgmma_kernel(const __grid_co
   if (tid < 128) {
     // ---------------- producer
     if (tid == 0) {
+      // a decode step reads each weight byte once; several token tiles read a slab once per tile, close together in time
+      const uint64_t w_hint = ntt > 1 ? kEvictNormal : kEvictFirst;
       int stage = 0;
       uint32_t phase = 0;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(empty_bar(stage), phase ^ 1);
         const uint32_t a = sbase + stage * C::kStageBytes;
         mbar_arrive_expect_tx(full_bar(stage), C::kStageBytes);
-        tma_load_2d(a, &P.tm_w, full_bar(stage), kb * kBlockK, n0, kEvictFirst);
+        tma_load_2d(a, &P.tm_w, full_bar(stage), kb * kBlockK, n0, w_hint);
         tma_load_2d(a + kABytes, &P.tm_x, full_bar(stage), kb * kBlockK, t0, kEvictLast);
         if (++stage == C::kStages) {
           stage = 0;
@@ -120,69 +136,72 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_wgmma_kernel(const __grid_co
     }
     consumer_sync();
   }
-  float acc[BN / 64][32];
+  float acc[BN / 2];   // acc[j * 32 + ..]: the m64n64 fragment of tokens [64 j, 64 j + 64) (ptx.cuh wgmma_m64nk16)
 #pragma unroll
-  for (int j = 0; j < BN / 64; ++j)
-#pragma unroll
-    for (int i = 0; i < 32; ++i) acc[j][i] = 0.f;
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
 
-  int stage = 0;
-  uint32_t phase = 0;
-  for (int kb = kb0; kb < kb1; ++kb) {
-    mbar_wait(full_bar(stage), phase);
-    const uint32_t a = sbase + stage * C::kStageBytes;
-    if (P.pro == GEMM3_PRO_NORM) {
-      // B tile := RMSNorm(residual) in place, rounded like rmsnorm_kernel: bf16(bf16(x * inv) * w)
-      uint8_t* b = smem + stage * C::kStageBytes + kABytes;
-      for (int c = ctid; c < BN * 8; c += kConsumers) {
-        const int r = c >> 3, k = kb * kBlockK + (((c & 7) ^ (r & 7)) << 3);
-        uint4* p = reinterpret_cast<uint4*>(b + r * 128 + (c & 7) * 16);
-        uint4 u = *p;
-        __nv_bfloat16* h = reinterpret_cast<__nv_bfloat16*>(&u);
-        const float inv = inv_s[r];
+  // One wgmma per k16 step covers NW tokens: the whole tile, or for the ragged last token tile the narrowest width that
+  // covers its tokens (the accumulators past NW keep their zeros).  Each output is the same fp32 chain whatever NW is.
+  // k-block kb is issued before kb - 1 is waited for: one k-block in flight, then kb - 1's ring stage goes back.
+  auto mainloop = [&](auto width) {
+    constexpr int NW = decltype(width)::value;
+    float(&d)[NW / 2] = *reinterpret_cast<float(*)[NW / 2]>(acc);
+    int stage = 0, prev = -1;
+    uint32_t phase = 0;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(full_bar(stage), phase);
+      const uint32_t a = sbase + stage * C::kStageBytes;
+      if (P.pro == GEMM3_PRO_NORM) {
+        // B tile := RMSNorm(residual) in place, rounded like rmsnorm_kernel: bf16(bf16(x * inv) * w)
+        uint8_t* b = smem + stage * C::kStageBytes + kABytes;
+        for (int c = ctid; c < BN * 8; c += kConsumers) {
+          const int r = c >> 3, k = kb * kBlockK + (((c & 7) ^ (r & 7)) << 3);
+          uint4* p = reinterpret_cast<uint4*>(b + r * 128 + (c & 7) * 16);
+          uint4 u = *p;
+          __nv_bfloat16* h = reinterpret_cast<__nv_bfloat16*>(&u);
+          const float inv = inv_s[r];
 #pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const float w = k + e < P.K ? ldbf(P.norm_w + k + e) : 0.f;
-          h[e] = __float2bfloat16_rn(bf16r(__bfloat162float(h[e]) * inv) * w);
+          for (int e = 0; e < 8; ++e) {
+            const float w = k + e < P.K ? ldbf(P.norm_w + k + e) : 0.f;
+            h[e] = __float2bfloat16_rn(bf16r(__bfloat162float(h[e]) * inv) * w);
+          }
+          *p = u;
         }
-        *p = u;
+        fence_proxy_async();
+        consumer_sync();
       }
-      fence_proxy_async();
-      consumer_sync();
-    }
-    wgmma_fence();
+      wgmma_fence();
 #pragma unroll
-    for (int k16 = 0; k16 < kBlockK / 16; ++k16) {
-      const uint64_t da = gmma_desc(a + wg * (64 * 128) + k16 * 32);
-#pragma unroll
-      for (int j = 0; j < BN / 64; ++j) wgmma_m64n64(acc[j], da, gmma_desc(a + kABytes + j * (64 * 128) + k16 * 32));
+      for (int k16 = 0; k16 < kBlockK / 16; ++k16)
+        wgmma_m64nk16<NW>(d, gmma_desc(a + wg * (64 * 128) + k16 * 32), gmma_desc(a + kABytes + k16 * 32));
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
+      prev = stage;
+      if (++stage == C::kStages) {
+        stage = 0;
+        phase ^= 1;
+      }
     }
-    wgmma_commit();
-    wgmma_wait0();
-    if (lane == 0) mbar_arrive(empty_bar(stage));
-    if (++stage == C::kStages) {
-      stage = 0;
-      phase ^= 1;
-    }
-  }
+    wgmma_wait<0>();   // the last stage is not handed back: the producer has no more loads
+  };
+  dispatch_width<BN>(min(BN, (P.T - t0 + 63) & ~63), mainloop);
 
   // ---------------- stage the fp32 tile: stg[token][row]
   consumer_sync();   // every wgmma of both warpgroups has read its stages: the ring is free
   {
     const int r0 = wg * 64 + (wtid >> 5) * 16 + (lane >> 2);
 #pragma unroll
-    for (int j = 0; j < BN / 64; ++j)
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const int t = j * 64 + q * 8 + (lane & 3) * 2;
-        stg[t * kPitch + r0] = acc[j][q * 4 + 0];
-        stg[(t + 1) * kPitch + r0] = acc[j][q * 4 + 1];
-        stg[t * kPitch + r0 + 8] = acc[j][q * 4 + 2];
-        stg[(t + 1) * kPitch + r0 + 8] = acc[j][q * 4 + 3];
-      }
+    for (int q = 0; q < BN / 8; ++q) {
+      const int t = q * 8 + (lane & 3) * 2;
+      stg[t * kPitch + r0] = acc[q * 4 + 0];
+      stg[(t + 1) * kPitch + r0] = acc[q * 4 + 1];
+      stg[t * kPitch + r0 + 8] = acc[q * 4 + 2];
+      stg[(t + 1) * kPitch + r0 + 8] = acc[q * 4 + 3];
+    }
   }
   consumer_sync();
-  const int tile = blockIdx.y * tiles_n + blockIdx.x;
+  const int tile = tt * tiles_n + slab;
   if (S > 1) {
     float* my = P.ws + (static_cast<size_t>(tile) * S + split) * (BN * kSlab);
     for (int i = ctid; i < BN * kSlab / 4; i += kConsumers) {
@@ -214,7 +233,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_wgmma_kernel(const __grid_co
   }
 
   // ---------------- epilogue: one warp per token, each lane 4 consecutive rows of the slab
-  const int slab = blockIdx.x, slabs = (P.N + kSlab - 1) / kSlab;
+  const int slabs = tiles_n;
   const int t_end = min(BN, P.T - t0);
   for (int tl = warp; tl < t_end; tl += kConsumers / 32) {
     const int t = t0 + tl;
@@ -311,7 +330,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_wgmma_kernel(const __grid_co
     __threadfence();
     consumer_sync();
     if (ctid == 0) {
-      int* c = P.counters + tiles_n * ntt + blockIdx.y;
+      int* c = P.counters + tiles_n * ntt + tt;
       const int prev = atomicAdd(c, 1);
       const int last = prev == tiles_n - 1;
       if (last) *c = 0;
@@ -403,7 +422,8 @@ int launch(const Gemm3Params& p, const Gemm3Schedule& sch, cudaStream_t st) {
   using C = Cfg<BN>;
   static std::atomic<unsigned long long> attr_done{0};
   if (!ensure_dynamic_smem(gemm_wgmma_kernel<BN>, C::kSmem, &attr_done)) return -3;
-  const dim3 grid((p.N + kSlab - 1) / kSlab, (p.T + BN - 1) / BN, sch.S);
+  const int slabs = (p.N + kSlab - 1) / kSlab, ntt = (p.T + BN - 1) / BN;
+  const dim3 grid = ntt > 1 ? dim3(ntt, slabs, sch.S) : dim3(slabs, 1, sch.S);   // see the kernel's CTA order
   cudaError_t e = launch_pdl(gemm_wgmma_kernel<BN>, grid, dim3(kThreads), C::kSmem, st, p, sch.S);
   return e == cudaSuccess ? 0 : -4;
 }

@@ -137,7 +137,11 @@ __device__ __forceinline__ uint64_t gmma_desc(uint32_t addr) {
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// at most N of this warpgroup's committed wgmma groups may still be in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
 // D[64 x 64] fp32 += A[64 x 16] * B[64 x 16]^T, both bf16 K-major in shared memory
 __device__ __forceinline__ void wgmma_m64n64(float (&d)[32], uint64_t a, uint64_t b) {
   asm volatile(
@@ -151,6 +155,61 @@ __device__ __forceinline__ void wgmma_m64n64(float (&d)[32], uint64_t a, uint64_
       : "l"(a), "l"(b)
       : "memory");
 }
+// D[64 x N] fp32 += A[64 x 16] * B[N x 16]^T, both bf16 K-major in shared memory, N = 64 / 128 / 192 / 256.  Thread
+// fragment: d[q * 4 + e] holds row (warp % 4) * 16 + lane / 4 + (e / 2) * 8, column q * 8 + (lane % 4) * 2 + e % 2, so
+// the first 32 * j values are the fragment of columns [0, 64 * j): an m64n64 instruction on the same rows.
+#define B200_WGMMA_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), \
+                         "+f"(d[i + 6]), "+f"(d[i + 7])
+template <int N>
+__device__ __forceinline__ void wgmma_m64nk16(float (&d)[N / 2], uint64_t a, uint64_t b);
+template <>
+__device__ __forceinline__ void wgmma_m64nk16<64>(float (&d)[32], uint64_t a, uint64_t b) { wgmma_m64n64(d, a, b); }
+template <>
+__device__ __forceinline__ void wgmma_m64nk16<128>(float (&d)[64], uint64_t a, uint64_t b) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, 1, 1, 1, 0, 0;"
+      : B200_WGMMA_D8(0), B200_WGMMA_D8(8), B200_WGMMA_D8(16), B200_WGMMA_D8(24), B200_WGMMA_D8(32), B200_WGMMA_D8(40), B200_WGMMA_D8(48), B200_WGMMA_D8(56)
+      : "l"(a), "l"(b)
+      : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_m64nk16<192>(float (&d)[96], uint64_t a, uint64_t b) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n192k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95"
+      "}, %96, %97, 1, 1, 1, 0, 0;"
+      : B200_WGMMA_D8(0), B200_WGMMA_D8(8), B200_WGMMA_D8(16), B200_WGMMA_D8(24), B200_WGMMA_D8(32), B200_WGMMA_D8(40), B200_WGMMA_D8(48), B200_WGMMA_D8(56), B200_WGMMA_D8(64), B200_WGMMA_D8(72), B200_WGMMA_D8(80), B200_WGMMA_D8(88)
+      : "l"(a), "l"(b)
+      : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_m64nk16<256>(float (&d)[128], uint64_t a, uint64_t b) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+      "}, %128, %129, 1, 1, 1, 0, 0;"
+      : B200_WGMMA_D8(0), B200_WGMMA_D8(8), B200_WGMMA_D8(16), B200_WGMMA_D8(24), B200_WGMMA_D8(32), B200_WGMMA_D8(40), B200_WGMMA_D8(48), B200_WGMMA_D8(56), B200_WGMMA_D8(64), B200_WGMMA_D8(72), B200_WGMMA_D8(80), B200_WGMMA_D8(88), B200_WGMMA_D8(96), B200_WGMMA_D8(104), B200_WGMMA_D8(112), B200_WGMMA_D8(120)
+      : "l"(a), "l"(b)
+      : "memory");
+}
+#undef B200_WGMMA_D8
 // D[64 x 64] fp32 += A[64 x 16] (bf16, registers: the m16n8k16 A-fragment layout per warp) * B[64 x 16]^T (smem descriptor)
 __device__ __forceinline__ void wgmma_m64n64_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b) {
   asm volatile(
