@@ -24,6 +24,7 @@ int main(int argc, char** argv) {
   std::string model = "llama-3-8b", model_dir, strategy = "LeastLoad", host = "0.0.0.0", adapters, tokenizer_path;
   double kv_fraction = 0.85;
   unsigned long long seed = 0;
+  bool greedy_only = false;
   for (int i = 1; i < argc; ++i) {
     std::string a = argv[i];
     auto next = [&]() -> const char* { return i + 1 < argc ? argv[++i] : ""; };
@@ -40,6 +41,7 @@ int main(int argc, char** argv) {
     else if (a == "--max-num-batched-tokens") budget = atoi(next());
     else if (a == "--gpu-memory-utilization") kv_fraction = atof(next());
     else if (a == "--seed") seed = strtoull(next(), nullptr, 10);
+    else if (a == "--greedy-only") greedy_only = true;   // refuse temperature >= 1e-5 with a 400
     else { fprintf(stderr, "unknown flag %s\n", a.c_str()); return 2; }
   }
   b200_config cfg;
@@ -67,6 +69,7 @@ int main(int argc, char** argv) {
   sc.max_retries = 3;
   sc.vocab = cfg.vocab;
   sc.max_model_len = cfg.max_model_len;
+  sc.enable_sampling = greedy_only ? 0 : 1;
   b200_server* srv = nullptr;
   if (b200_server_create(&sc, engines.data(), gpus, &srv)) { fprintf(stderr, "server: %s\n", b200_last_error()); return 1; }
   // the checkpoint's tokenizer + Llama-3 chat template when there is one; the synthetic tokenizer otherwise

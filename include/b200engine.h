@@ -66,12 +66,19 @@ typedef struct {
   int32_t rope_original_max_pos;
 } b200_config;
 
+/* Sampling follows vLLM V1 (vllm/v1/sample/sampler.py, ops/topk_topp_sampler.py), made deterministic: the token is a pure
+ * function of the logits row, these parameters, the seed and the index of the token in the generation (csrc/sampling.cu).
+ * Zero means "off" for every field after stop_ids, so a zero-initialised struct asks for greedy decoding. */
 typedef struct {
   int32_t max_tokens;
-  float temperature;          /* only greedy (temperature < 1e-5, vllm/v1/sample/sampler.py:17) is implemented */
+  float temperature;          /* finite, >= 0; < 1e-5 (vllm/v1/sample/sampler.py _SAMPLING_EPS) = greedy argmax */
   int32_t ignore_eos;
   int32_t num_stop_ids;
   const int32_t* stop_ids;
+  float top_p;                /* in [0, 1]; 0 or 1 = off */
+  int32_t top_k;              /* >= -1; 0, -1 or >= vocab = off */
+  int32_t has_seed;           /* 0: the engine draws a seed for the request (not reproducible, as in vLLM and OpenAI) */
+  uint64_t seed;
 } b200_sampling;
 
 typedef struct {
@@ -166,7 +173,8 @@ int b200_engine_tensor_write(b200_engine* e, const char* name, const void* host_
 int b200_engine_forward_logits(b200_engine* e, const int32_t* ids, int32_t n, void* host_logits_bf16);
 /* Parity hook for decode steps (manual_step mode): with keep != 0 the lm_head of every later step leaves the complete
  * bf16 logits of its sampled rows in HBM (the serving path only keeps what the argmax needs); read_logits copies the
- * first `rows` rows [rows, vocab] of the last step, in the order the step sampled them (scheduling order). */
+ * first `rows` rows [rows, vocab] of the last step, in the order the step sampled them (scheduling order).  For a step
+ * with a row at temperature >= 1e-5 these are the exact rows the sampler read. */
 int b200_engine_set_keep_logits(b200_engine* e, int32_t keep);
 int b200_engine_read_logits(b200_engine* e, void* host_logits_bf16, int32_t rows);
 
@@ -232,6 +240,9 @@ typedef struct {
   int32_t default_max_tokens;  /* when the request has no max_tokens */
   int32_t vocab;               /* tokenizer range == engine vocab */
   int32_t max_model_len;
+  /* 1: requests with temperature >= 1e-5 are sampled (temperature / top_p / top_k / seed, see b200_sampling); 0: they get
+   * a 400 and the server decodes greedily only, as before sampling existed (a zero-initialised config keeps that) */
+  int32_t enable_sampling;
 } b200_server_config;
 int b200_server_create(const b200_server_config* cfg, b200_engine* const* replicas, int32_t n, b200_server** out);
 void b200_server_destroy(b200_server* s);
@@ -381,6 +392,19 @@ int b200_op_rope_kvwrite(void* qkv, const int32_t* positions, const int32_t* slo
                          void* kv_layer, int32_t T, int32_t q_heads, int32_t kv_heads, int32_t max_pos, void* stream);
 int b200_op_silu_mul(const void* gate_up, void* out, int32_t T, int32_t I, void* stream);
 int b200_op_argmax(const void* logits, int32_t* out, int32_t S, int32_t V, int32_t ld, void* stream);
+/* One sampled row's parameters, as the engine packs them into a step: temperature < 1e-5 = greedy; top_k <= 0 or >= V and
+ * top_p <= 0 or >= 1 = off; the noise is Philox4x32-10 with key (seed_lo, seed_hi) and counter (v / 4, n, 0, 0), n = the
+ * index of the token being generated. */
+typedef struct {
+  float temperature;
+  int32_t top_k;
+  float top_p;
+  uint32_t seed_lo, seed_hi;
+  int32_t n;
+} b200_sample_row;
+/* out[s] = the token sampled from bf16 logits row s ([S, ld], ld % 8 == 0, V <= ld) under rows[s]; rows and out are device
+ * memory.  Greedy rows give the same token as b200_op_argmax. */
+int b200_op_sample(const void* logits, int32_t ld, const b200_sample_row* rows, int32_t S, int32_t V, int32_t* out, void* stream);
 /* work: int32[num_work][4] = {q_tok0, q_count, q_pos0, seq}; kv_layer: [block][2][kv_heads][16][128] */
 int b200_op_paged_attn(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                        const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,

@@ -22,6 +22,7 @@ SOURCES = [
     "attention.cu",
     "attention_wgmma.cu",
     "elementwise.cu",
+    "sampling.cu",
     "abi_ops.cu",
     "engine.cu",
     "router.cc",

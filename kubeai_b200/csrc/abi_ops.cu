@@ -238,6 +238,17 @@ int b200_op_argmax(const void* logits, int32_t* out, int32_t S, int32_t V, int32
   return rc ? cuda_fail("argmax_rows", rc) : 0;
 }
 
+int b200_op_sample(const void* logits, int32_t ld, const b200_sample_row* rows, int32_t S, int32_t V, int32_t* out, void* stream) {
+  if (int rc = require_device()) return rc;
+  static_assert(sizeof(b200_sample_row) == sizeof(SampleRow), "b200_sample_row is SampleRow on the wire");
+  if (!logits || !rows || !out || S < 0 || V < 1 || ld < V || ld % 8) {
+    set_error("b200_op_sample: bad arguments (S=%d V=%d ld=%d; ld %% 8 == 0 and V <= ld required)", S, V, ld);
+    return B200_ERR_INVALID;
+  }
+  int rc = sample_rows(logits, ld, reinterpret_cast<const SampleRow*>(rows), S, V, out, static_cast<cudaStream_t>(stream));
+  return rc ? cuda_fail("sample_rows", rc) : 0;
+}
+
 int b200_op_paged_attn(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                        const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
                        int32_t q_heads, int32_t kv_heads, float scale, int32_t decode, void* stream) {

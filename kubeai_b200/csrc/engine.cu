@@ -7,7 +7,8 @@
 // scheduler with chunked prefill under a per-step token budget (semantics of vLLM's
 // v1/core/sched/scheduler.py: running first, then waiting; preempt-by-recompute on KV exhaustion;
 // 16-token blocks; a prefix hit covers at most len-1 tokens), the Llama forward as a fixed kernel
-// sequence on one CUDA stream, greedy sampling, thread-safe submit/poll/wait/abort.
+// sequence on one CUDA stream, greedy or seeded temperature / top-k / top-p sampling (sampling.cu), thread-safe
+// submit/poll/wait/abort.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <nvtx3/nvToolsExt.h>
@@ -24,6 +25,7 @@
 #include <deque>
 #include <memory>
 #include <mutex>
+#include <random>
 #include <string>
 #include <thread>
 #include <unordered_map>
@@ -172,6 +174,10 @@ struct Seq {
   int max_tokens = 16;
   bool ignore_eos = false;
   std::vector<int32_t> stop_ids;
+  // sampling (sampling.cu): temperature < 1e-5 = greedy; top_k <= 0 / top_p >= 1 = off; every request has a seed
+  float temperature = 0.f, top_p = 1.f;
+  int top_k = 0;
+  uint64_t seed = 0;
   int n_generated = 0;
   std::atomic<int> n_cached{-1};  // prefix-hit tokens at first admission
   bool admitted = false;
@@ -207,6 +213,7 @@ struct Pub {
 struct StepMeta {
   int T = 0, nd = 0, np = 0, S = 0, nseq = 0;
   int off_ids = 0, off_pos = 0, off_slots = 0, off_rows = 0, off_dwork = 0, off_pwork = 0, off_btab = 0;
+  int off_samp = -1;   // SampleRow per sampled row, packed only when one of them has temperature >= 1e-5
   int words = 0;
   int64_t kv_tokens = 0;
   int out_tokens = 0;  // sampled rows that produce a generated token
@@ -282,6 +289,7 @@ struct Engine {
   std::deque<std::shared_ptr<Seq>> incoming;
   std::unordered_map<uint64_t, std::shared_ptr<Seq>> requests;
   uint64_t next_id = 1;
+  uint64_t seed_state = 0;   // splitmix64 stream of the seeds of requests that bring none (seeded from std::random_device)
   std::atomic<bool> stop{false};
   std::thread worker;
   b200_stats stats;
@@ -324,6 +332,7 @@ struct Engine {
   InFlight inflight_;
   std::vector<AttnWork> dwork_, pwork_;  // packing scratch (kept across steps: no per-step allocation)
   std::vector<int> rows_;
+  std::vector<SampleRow> samp_;          // parameters of the rows in rows_ order
   bool ensure_blocks(Seq& s, int upto);
   void release_blocks(Seq& s);
   void preempt(std::shared_ptr<Seq> s);
@@ -398,6 +407,13 @@ Engine::~Engine() {
 }
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+static uint64_t splitmix64(uint64_t* state) {
+  uint64_t z = (*state += 0x9E3779B97F4A7C15ull);
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
 
 int Engine::alloc_all() {
   // ---- weights: one blob, 1 KiB-aligned tensors
@@ -583,7 +599,8 @@ int Engine::alloc_all() {
 
   // ---- step input ring
   max_blocks_per_seq = (cfg.max_model_len + kPage - 1) / kPage;
-  step_words_cap = 3 * Tcap + Scap + 4 * Scap + 4 * (Tcap / 16 + Scap + 1) + Scap * max_blocks_per_seq + 64;
+  step_words_cap = 3 * Tcap + Scap + 4 * Scap + 4 * (Tcap / 16 + Scap + 1) + Scap * max_blocks_per_seq + 6 * Scap + 64;
+  static_assert(sizeof(SampleRow) == 6 * sizeof(int32_t), "SampleRow is 6 words of the step input");
   ring_n = std::max(1, cfg.record_steps) + 1;  // last slot = scratch for unrecorded steps
   CK(cudaMallocHost(&stage_host, static_cast<size_t>(step_words_cap) * 4));
   stage_dev.assign(ring_n, nullptr);
@@ -615,6 +632,10 @@ int Engine::init(const b200_config& c) {
   Tcap = (c.max_batched_tokens + 15) / 16 * 16;
   Scap = c.max_num_seqs;
   memset(&stats, 0, sizeof(stats));
+  {
+    std::random_device rd;
+    seed_state = (static_cast<uint64_t>(rd()) << 32) ^ rd();
+  }
   CK(cudaSetDevice(c.device));
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c.device));
   CK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
@@ -716,14 +737,18 @@ int Engine::forward(const StepMeta& m, int32_t* dbuf, bool all_logits, bf16* log
     rc |= launch_proj(p, xm_normed, T);
   } else if (m.S > 0) {
     P(B200_K_NORM); norm(final_norm, last_hidden, rows, m.S); Q();
-    // argmax candidates per 128-row slab in the lm_head epilogue (the candidate buffer holds 128 rows), or bf16 logits
-    const bool cand_ok = fused && !keep_logits && m.S <= 128;
+    // argmax candidates per 128-row slab in the lm_head epilogue (the candidate buffer holds 128 rows), or bf16 logits.
+    // A step with a sampled row (temperature >= 1e-5) writes the logits and selects every row's token in one sample_rows
+    // launch, greedy rows included.
+    const bool samp = m.off_samp >= 0;
+    const bool cand_ok = !samp && fused && !keep_logits && m.S <= 128;
     Gemm3Params p = proj(p_lm, cand_ok ? GEMM3_EPI_ARGMAX : GEMM3_EPI_PLAIN);
     p.out = logits; p.ldo = V; p.cand = cand;
     P(B200_K_GEMM_LM); rc |= launch_proj(p, xm_last, m.S); Q();
     last_S = m.S;
     P(B200_K_ARGMAX);
-    if (cand_ok) rc |= argmax_candidates(cand, sampled, m.S, (V + 127) / 128, stream);
+    if (samp) rc |= sample_rows(logits, V, reinterpret_cast<const SampleRow*>(dbuf + m.off_samp), m.S, V, sampled, stream);
+    else if (cand_ok) rc |= argmax_candidates(cand, sampled, m.S, (V + 127) / 128, stream);
     else rc |= argmax_rows(logits, sampled, m.S, V, V, stream);
     Q();
     launched(1);
@@ -899,6 +924,8 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
   dwork_.clear();
   pwork_.clear();
   rows_.clear();
+  samp_.clear();
+  bool any_sampled = false;
   int32_t* h = stage_host;
   m.off_ids = 0; m.off_pos = m.T; m.off_slots = 2 * m.T;
   int tok = 0;
@@ -922,7 +949,13 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
       m.kv_tokens += p0 + n;  // unique K/V tokens this sequence streams from HBM (query tiles re-read them from L2)
       ++f->npre_seq;
     }
-    if (p0 + n == static_cast<int>(s.toks.size())) rows_.push_back(tok + n - 1);
+    if (p0 + n == static_cast<int>(s.toks.size())) {
+      rows_.push_back(tok + n - 1);
+      // n = the index of the token this row generates: a request recomputed after preemption draws the same noise
+      samp_.push_back({s.temperature, s.top_k, s.top_p, static_cast<uint32_t>(s.seed), static_cast<uint32_t>(s.seed >> 32),
+                       s.n_generated});
+      any_sampled |= s.temperature >= 1e-5f;
+    }
     tok += n;
   }
   // longest-context work first: CTAs are dispatched in blockIdx order, so the tail of the attention grid is made of
@@ -946,6 +979,11 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
     memcpy(h + w + static_cast<size_t>(si) * max_blocks_per_seq, s.blocks.data(), s.blocks.size() * 4);
   }
   w += m.nseq * max_blocks_per_seq;
+  if (any_sampled) {   // greedy-only steps carry no sampling section: the same words as without one
+    m.off_samp = w;
+    memcpy(h + w, samp_.data(), samp_.size() * sizeof(SampleRow));
+    w += 6 * m.S;
+  }
   m.words = w;
   if (w > step_words_cap) {
     set_error("step staging overflow (%d > %d words)", w, step_words_cap);
@@ -1198,7 +1236,9 @@ int b200_submit(b200_engine* e, const int32_t* prompt_ids, int32_t n, const b200
   Engine& g = e->impl;
   const int max_tokens = sp && sp->max_tokens > 0 ? sp->max_tokens : 16;
   if (n + 1 > g.cfg.max_model_len) { set_error("prompt (%d tokens) exceeds max_model_len %d", n, g.cfg.max_model_len); return B200_ERR_INVALID; }
-  if (sp && sp->temperature >= 1e-5f) { set_error("only greedy sampling (temperature < 1e-5) is implemented"); return B200_ERR_INVALID; }
+  if (sp && !(std::isfinite(sp->temperature) && sp->temperature >= 0.f)) { set_error("temperature must be finite and >= 0"); return B200_ERR_INVALID; }
+  if (sp && !(sp->top_p >= 0.f && sp->top_p <= 1.f)) { set_error("top_p must be in [0, 1]"); return B200_ERR_INVALID; }
+  if (sp && sp->top_k < -1) { set_error("top_k must be >= -1"); return B200_ERR_INVALID; }
   for (int i = 0; i < n; ++i) if (prompt_ids[i] < 0 || prompt_ids[i] >= g.V) { set_error("token id out of range"); return B200_ERR_INVALID; }
   auto s = std::make_shared<Seq>();
   s->toks.assign(prompt_ids, prompt_ids + n);
@@ -1207,9 +1247,15 @@ int b200_submit(b200_engine* e, const int32_t* prompt_ids, int32_t n, const b200
   s->max_tokens = max_tokens;
   s->ignore_eos = sp && sp->ignore_eos;
   if (sp && sp->num_stop_ids > 0 && sp->stop_ids) s->stop_ids.assign(sp->stop_ids, sp->stop_ids + sp->num_stop_ids);
+  if (sp) {
+    s->temperature = sp->temperature;
+    s->top_p = sp->top_p > 0.f ? sp->top_p : 1.f;   // 0 = off at this ABI
+    s->top_k = sp->top_k > 0 ? sp->top_k : 0;
+  }
   {
     std::lock_guard<std::mutex> lk(g.mu_);
     if (g.fatal) { set_error("engine is in a failed state"); return B200_ERR_CUDA; }
+    s->seed = sp && sp->has_seed ? sp->seed : splitmix64(&g.seed_state);
     s->id = g.next_id++;
     g.requests[s->id] = s;
     g.incoming.push_back(s);

@@ -27,6 +27,19 @@ int permute_gate_up(void* dst, const void* src, int I, int H, int to_physical, c
 int argmax_rows(const void* logits, int* out, int S, int V, int ld, cudaStream_t st, PartialView pv = no_partials());
 int init_uniform(void* p, size_t n, uint32_t seed, float scale, float offset, cudaStream_t st);
 
+// Per-row sampling parameters (sampling.cu; b200_sample_row at the ABI): temperature < 1e-5 is greedy, top_k <= 0 or >= V
+// and top_p <= 0 or >= 1 are off; the noise of the row is Philox4x32-10 keyed by the seed and counted by n, the index of
+// the token being generated.
+struct SampleRow {
+  float temperature;
+  int top_k;
+  float top_p;
+  uint32_t seed_lo, seed_hi;
+  int n;
+};
+// out[s] = the token sampled from bf16 logits row s ([S, ld], ld % 8 == 0) under rows[s] (device memory)
+int sample_rows(const void* logits, int ld, const SampleRow* rows, int S, int V, int* out, cudaStream_t st);
+
 // One unit of attention work: q_count query tokens of one sequence starting at row q_tok0 of the
 // step's token batch; the first of them sits at absolute position q_pos0 in the sequence.
 struct AttnWork {

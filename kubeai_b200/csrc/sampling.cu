@@ -1,0 +1,334 @@
+// Token selection for sampled rows (SURVEY.md §8a K11): temperature, top-k, top-p and a seeded exponential race over
+// bf16 logits.  Semantics are vLLM V1's (vllm/v1/sample/sampler.py:223-297, ops/topk_topp_sampler.py:328-416), made
+// deterministic:
+//   - temperature < 1e-5: argmax, lowest index on ties (the same token as argmax_kernel in elementwise.cu);
+//   - z_v = float(l_v) / temperature (fp32);
+//   - top-k keeps every token whose z is >= the k-th largest z (ties at the k-th value are kept);
+//   - top-p keeps token v iff the softmax mass of the top-k-kept tokens with z strictly greater than z_v is < p, so tie
+//     groups are kept or dropped whole;
+//   - the token is the argmax over the kept tokens of z_v - log(E_v), E_v = -log(u_v) ~ Exp(1) (the probs / q race of
+//     vLLM's random_sample), lowest index on ties.  u_v = ((x >> 9) + 0.5) * 2^-23 is exact in fp32 and strictly inside
+//     (0, 1); x is word v & 3 of Philox4x32-10 with counter (v >> 2, n, 0, 0) and key (seed_lo, seed_hi).
+// The result is a pure function of (logits row, parameters, seed, n): it does not depend on the batch, the row's place in
+// it, or the order in which threads run.
+//
+// One CTA per row, no sort.  bf16 logits have at most 65536 distinct values, each with an order-preserving 16-bit key, and
+// temperature is monotonic, so both thresholds are keys.  They are found with a 256-bin histogram over the high byte of the
+// key, then one over the low byte inside the bin that holds the threshold.  Each bin holds a count and a fixed-point mass
+// floor(exp(z_v - z_max) * 2^40); both are summed with integer shared-memory atomics, whose result does not depend on
+// arrival order (2^40 * 2^17 tokens fits in 64 bits).  The passes re-read the row (250 KB at Llama-3's vocabulary), which
+// is still in L2 right after the lm_head:
+//   1 row max (top-p only)   2 high-byte histogram   3 low-byte histogram of the top-k bin   4 the same for the top-p bin
+//   (skipped when it is the top-k bin)   5 the race over the tokens at or above the threshold.
+// Rows with temperature only run pass 5 alone.
+#include <cuda_bf16.h>
+#include <cuda_runtime.h>
+#include <math.h>
+#include <stdint.h>
+
+#include "kernels.h"
+#include "launch.h"
+#include "ptx.cuh"
+
+namespace b200 {
+
+namespace {
+
+constexpr int kThreads = 1024;
+constexpr float kSamplingEps = 1e-5f;            // vllm/v1/sample/sampler.py _SAMPLING_EPS
+constexpr float kMassScale = 1099511627776.0f;   // 2^40
+constexpr int kPrivSmem = 256 * 32 * (8 + 4);     // 32 copies of a 256-bin (mass, count) histogram: 96 KiB
+
+__device__ __forceinline__ void philox4x32_10(uint32_t c[4], uint32_t k0, uint32_t k1) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    if (r) {
+      k0 += 0x9E3779B9u;
+      k1 += 0xBB67AE85u;
+    }
+    const uint32_t lo0 = 0xD2511F53u * c[0], hi0 = __umulhi(0xD2511F53u, c[0]);
+    const uint32_t lo1 = 0xCD9E8D57u * c[2], hi1 = __umulhi(0xCD9E8D57u, c[2]);
+    const uint32_t n0 = hi1 ^ c[1] ^ k0, n2 = hi0 ^ c[3] ^ k1;
+    c[0] = n0;
+    c[1] = lo1;
+    c[2] = n2;
+    c[3] = lo0;
+  }
+}
+
+// order-preserving key of a bf16 bit pattern (-0 and +0 share one key: they are the same logit)
+__device__ __forceinline__ uint32_t key_of(uint32_t b) {
+  if (b == 0x8000u) b = 0;
+  return (b & 0x8000u) ? (~b & 0xFFFFu) : (b | 0x8000u);
+}
+__device__ __forceinline__ uint32_t bits_of_key(uint32_t k) { return (k & 0x8000u) ? (k & 0x7FFFu) : (~k & 0xFFFFu); }
+__device__ __forceinline__ float bf16_bits_to_f32(uint32_t b) { return __uint_as_float(b << 16); }
+
+// Visit every token of the row, 8 at a time from 16-byte loads (two loads in flight per thread), then the scalar tail.
+template <class F>
+__device__ __forceinline__ void visit_row(const uint16_t* __restrict__ row, int V, F&& f) {
+  const int nvec = V >> 3;
+  const uint4* r4 = reinterpret_cast<const uint4*>(row);
+  for (int i = threadIdx.x; i < nvec; i += 2 * kThreads) {
+    const int i2 = i + kThreads;
+    const uint4 a = r4[i];
+    const uint4 c = i2 < nvec ? r4[i2] : make_uint4(0, 0, 0, 0);
+    const uint32_t wa[4] = {a.x, a.y, a.z, a.w}, wc[4] = {c.x, c.y, c.z, c.w};
+#pragma unroll
+    for (int j = 0; j < 8; ++j) f(i * 8 + j, (wa[j >> 1] >> ((j & 1) * 16)) & 0xFFFFu);
+    if (i2 < nvec) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) f(i2 * 8 + j, (wc[j >> 1] >> ((j & 1) * 16)) & 0xFFFFu);
+    }
+  }
+  for (int v = nvec * 8 + threadIdx.x; v < V; v += kThreads) f(v, static_cast<uint32_t>(row[v]));
+}
+
+// (score, index) argmax over the CTA, lowest index on ties (argmax_kernel's reduction)
+__device__ __forceinline__ int block_argmax(float best, int bi, float* sb, int* si) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (ob > best || (ob == best && oi < bi)) {
+      best = ob;
+      bi = oi;
+    }
+  }
+  if ((threadIdx.x & 31) == 0) {
+    sb[threadIdx.x >> 5] = best;
+    si[threadIdx.x >> 5] = bi;
+  }
+  __syncthreads();
+  best = sb[threadIdx.x & 31];
+  bi = si[threadIdx.x & 31];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (ob > best || (ob == best && oi < bi)) {
+      best = ob;
+      bi = oi;
+    }
+  }
+  return bi;
+}
+
+// One warp: the largest bin b with pred(above + sum(h[b..255])), or -1.  The suffix sum does not increase with b and pred
+// is true for large sums, so the answer is the top of the run of bins where it holds.  *above_b gets sum(h[b+1..255]).
+template <class T, class Pred>
+__device__ __forceinline__ int warp_last_bin(const T* h, unsigned long long above, Pred pred, unsigned long long* above_b) {
+  const int lane = threadIdx.x & 31;
+  unsigned long long loc[8], chunk = 0;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    loc[j] = static_cast<unsigned long long>(h[lane * 8 + j]);
+    chunk += loc[j];
+  }
+  unsigned long long incl = chunk;   // sum over lanes >= this lane
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned long long v = __shfl_down_sync(0xffffffffu, incl, o);
+    if (lane + o < 32) incl += v;
+  }
+  unsigned long long run = incl - chunk, before = 0;
+  int best = -1;
+#pragma unroll
+  for (int j = 7; j >= 0; --j) {
+    const unsigned long long prev = run;
+    run += loc[j];
+    if (best < 0 && pred(above + run)) {
+      best = lane * 8 + j;
+      before = prev;
+    }
+  }
+  const unsigned bal = __ballot_sync(0xffffffffu, best >= 0);
+  if (!bal) return -1;
+  const int src = 31 - __clz(bal);
+  *above_b = __shfl_sync(0xffffffffu, before, src);
+  return __shfl_sync(0xffffffffu, best, src);
+}
+
+__global__ void __launch_bounds__(kThreads) sample_kernel(const uint16_t* __restrict__ logits, int ld,
+                                                          const SampleRow* __restrict__ rows, int V, int* __restrict__ out) {
+  __shared__ uint32_t cnt_hi[256], cnt_lo[256];
+  __shared__ unsigned long long mass_hi[256], mass_lo[256];
+  __shared__ float sb[32];
+  __shared__ int si[32];
+  __shared__ uint32_t s_kmax, s_thr;
+  extern __shared__ __align__(16) unsigned char dyn_smem[];   // kPrivSmem: per-lane histogram copies
+  unsigned long long* priv_mass = reinterpret_cast<unsigned long long*>(dyn_smem);
+  uint32_t* priv_cnt = reinterpret_cast<uint32_t*>(dyn_smem + 256 * 32 * sizeof(unsigned long long));
+  griddep_enter();
+  const int s = blockIdx.x;
+  const uint16_t* row = logits + static_cast<size_t>(s) * ld;
+  const SampleRow P = rows[s];
+
+  if (!(P.temperature >= kSamplingEps)) {
+    // greedy: argmax_kernel's comparisons, so the same token
+    float best = -INFINITY;
+    int bi = 0x7fffffff;
+    visit_row(row, V, [&](int v, uint32_t b) {
+      const float f = bf16_bits_to_f32(b);
+      if (f > best || (f == best && v < bi)) {
+        best = f;
+        bi = v;
+      }
+    });
+    bi = block_argmax(best, bi, sb, si);
+    if (threadIdx.x == 0) out[s] = bi == 0x7fffffff ? 0 : bi;
+    return;
+  }
+
+  const float T = P.temperature;
+  const bool topk_on = P.top_k > 0 && P.top_k < V;
+  const bool topp_on = P.top_p > 0.f && P.top_p < 1.f;
+  uint32_t thr = 0;   // the race runs over the tokens with key >= thr
+  if (topk_on || topp_on) {
+    float zmax = 0.f;
+    if (topp_on) {
+      // pass 1: row max, as a key (an integer max does not depend on order)
+      uint32_t km = 0;
+      visit_row(row, V, [&](int, uint32_t b) { km = max(km, key_of(b)); });
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) km = max(km, __shfl_xor_sync(0xffffffffu, km, o));
+      if (threadIdx.x == 0) s_kmax = 0;
+      __syncthreads();
+      if ((threadIdx.x & 31) == 0) atomicMax(&s_kmax, km);
+      __syncthreads();
+      zmax = __fdiv_rn(bf16_bits_to_f32(bits_of_key(s_kmax)), T);
+    }
+    auto fixed_mass = [&](uint32_t b) {
+      const float m = expf(__fsub_rn(__fdiv_rn(bf16_bits_to_f32(b), T), zmax));   // in [0, 1]
+      return __float2ull_rz(__fmul_rn(m, kMassScale));
+    };
+    // bin < 0: histogram of the high byte of every key; else of the low byte of the keys whose high byte is `bin`.
+    // Logits fall into a dozen high-byte bins (sign and exponent), so every lane adds into its own copy of the
+    // histogram (copy = lane, bank = lane: no two lanes of an atomic instruction collide); the copies are then summed.
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    auto histogram = [&](int bin, uint32_t* c, unsigned long long* m) {
+      for (int i = threadIdx.x; i < 256 * 32; i += kThreads) {
+        priv_cnt[i] = 0;
+        priv_mass[i] = 0;
+      }
+      __syncthreads();
+      visit_row(row, V, [&](int, uint32_t b) {
+        const uint32_t k = key_of(b);
+        if (bin >= 0 && static_cast<int>(k >> 8) != bin) return;
+        const uint32_t slot = (bin >= 0 ? (k & 0xFFu) : (k >> 8)) * 32 + lane;
+        if (topk_on) atomicAdd(&priv_cnt[slot], 1u);          // counts serve top-k, masses top-p
+        if (topp_on) atomicAdd(&priv_mass[slot], fixed_mass(b));
+      });
+      __syncthreads();
+      for (int j = warp; j < 256; j += kThreads / 32) {
+        uint32_t cs = priv_cnt[j * 32 + lane];
+        unsigned long long ms = priv_mass[j * 32 + lane];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+          cs += __shfl_xor_sync(0xffffffffu, cs, o);
+          ms += __shfl_xor_sync(0xffffffffu, ms, o);
+        }
+        if (lane == 0) {
+          c[j] = cs;
+          m[j] = ms;
+        }
+      }
+      __syncthreads();
+    };
+    const bool lead = threadIdx.x < 32;
+    histogram(-1, cnt_hi, mass_hi);   // pass 2
+    // top-k: the k-th largest key = the largest key t with count(key >= t) >= k
+    int bk = -1;
+    uint32_t tk = 0;
+    unsigned long long z = 0;   // fixed-point mass of the top-k-kept tokens
+    if (topk_on) {
+      const unsigned long long k = static_cast<unsigned long long>(P.top_k);
+      auto reach = [&](unsigned long long c) { return c >= k; };
+      unsigned long long cab = 0, unused = 0;
+      if (lead) bk = warp_last_bin(cnt_hi, 0ull, reach, &cab);   // k <= V - 1: always found
+      if (threadIdx.x == 0) s_thr = static_cast<uint32_t>(bk);
+      __syncthreads();
+      bk = static_cast<int>(s_thr);
+      histogram(bk, cnt_lo, mass_lo);   // pass 3
+      if (lead) {
+        const int lo = warp_last_bin(cnt_lo, cab, reach, &unused);
+        tk = (static_cast<uint32_t>(bk) << 8) | static_cast<uint32_t>(lo);
+        if (topp_on) {
+          // mass of the kept tokens: the bins above bk and the keys >= tk inside it
+          unsigned long long m = 0;
+          for (int i = threadIdx.x; i < 256; i += 32) m += (i > bk ? mass_hi[i] : 0ull) + (i >= lo ? mass_lo[i] : 0ull);
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) m += __shfl_xor_sync(0xffffffffu, m, o);
+          z = m;
+        }
+      }
+    } else if (topp_on && lead) {
+      unsigned long long m = 0;
+      for (int i = threadIdx.x; i < 256; i += 32) m += mass_hi[i];
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) m += __shfl_xor_sync(0xffffffffu, m, o);
+      z = m;
+    }
+    uint32_t tp = 0;
+    if (topp_on) {
+      // top-p: keep v iff mass(kept, key > key_v) < p * z, i.e. key_v >= the largest key t with mass(kept, key >= t) >=
+      // p * z.  Every high-byte bin at or below bk holds at least z >= p * z of kept mass, so the search over the whole-row
+      // histogram lands at or above bk, and above bk every token is kept.
+      const double X = static_cast<double>(P.top_p) * static_cast<double>(z);
+      auto reach = [&](unsigned long long m) { return static_cast<double>(m) >= X; };
+      unsigned long long mab = 0, unused = 0;
+      int bp = 0;
+      if (lead) bp = warp_last_bin(mass_hi, 0ull, reach, &mab);
+      if (threadIdx.x == 0) s_thr = static_cast<uint32_t>(bp);
+      __syncthreads();
+      bp = static_cast<int>(s_thr);
+      if (bp != bk) histogram(bp, cnt_lo, mass_lo);   // pass 4 (pass 3 already holds bin bk)
+      if (lead) {
+        const int lo = warp_last_bin(mass_lo, mab, reach, &unused);
+        tp = (static_cast<uint32_t>(bp) << 8) | static_cast<uint32_t>(lo);
+      }
+    }
+    __syncthreads();   // every reader of s_thr is past it
+    if (threadIdx.x == 0) s_thr = max(tk, tp);
+    __syncthreads();
+    thr = s_thr;
+  }
+
+  // pass 5: the exponential race over the tokens with key >= thr
+  const uint32_t seed_lo = P.seed_lo, seed_hi = P.seed_hi, n = static_cast<uint32_t>(P.n);
+  float best = -INFINITY;
+  int bi = 0x7fffffff;
+  int group = -1;
+  uint32_t w[4] = {0, 0, 0, 0};
+  visit_row(row, V, [&](int v, uint32_t b) {
+    if (key_of(b) < thr) return;
+    if ((v >> 2) != group) {
+      group = v >> 2;
+      w[0] = static_cast<uint32_t>(group); w[1] = n; w[2] = 0; w[3] = 0;
+      philox4x32_10(w, seed_lo, seed_hi);
+    }
+    const uint32_t x = w[v & 3];
+    const float u = __fmul_rn(__fadd_rn(static_cast<float>(x >> 9), 0.5f), 1.0f / 8388608.0f);   // exact, in (0, 1)
+    const float e = -logf(u);
+    const float score = __fsub_rn(__fdiv_rn(bf16_bits_to_f32(b), T), logf(e));
+    if (score > best || (score == best && v < bi)) {
+      best = score;
+      bi = v;
+    }
+  });
+  bi = block_argmax(best, bi, sb, si);
+  if (threadIdx.x == 0) out[s] = bi == 0x7fffffff ? 0 : bi;
+}
+
+}  // namespace
+
+int sample_rows(const void* logits, int ld, const SampleRow* rows, int S, int V, int* out, cudaStream_t st) {
+  if (S <= 0) return 0;
+  if (V < 1 || ld < V || ld % 8 || (reinterpret_cast<uintptr_t>(logits) & 15)) return -1;
+  static std::atomic<unsigned long long> smem_set{0};
+  if (!ensure_dynamic_smem(sample_kernel, kPrivSmem, &smem_set)) return -2;
+  launch_pdl(sample_kernel, dim3(S), dim3(kThreads), kPrivSmem, st, static_cast<const uint16_t*>(logits), ld, rows, V, out);
+  return cudaGetLastError() == cudaSuccess ? 0 : -2;
+}
+
+}  // namespace b200

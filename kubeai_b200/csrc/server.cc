@@ -19,6 +19,7 @@
 #include <unistd.h>
 
 #include <atomic>
+#include <cmath>
 #include <map>
 #include <mutex>
 #include <random>
@@ -46,6 +47,7 @@ struct Server {
   b200_router* router = nullptr;
   Tokenizer tok;
   int max_model_len = 2048;
+  bool sampling = false;   // b200_server_config.enable_sampling: serve temperature >= 1e-5 (else greedy only)
   // optional real tokenizer (b200_server_set_tokenizer): a checkpoint's tokenizer.json instead of the synthetic byte/word ids
   const b200_tokenizer* real_tok = nullptr;
 
@@ -156,8 +158,11 @@ struct ParsedRequest {
   bool prompt_is_ids = false;
   int max_tokens = -1;
   bool stream = false, include_usage = false, ignore_eos = false;
-  double temperature = 0.0;
-  bool has_temperature = false;
+  double temperature = 0.0;   // absent = greedy
+  double top_p = 1.0;
+  int top_k = 0;
+  bool has_seed = false;
+  int64_t seed = 0;
   std::vector<int32_t> stop_ids;
 };
 
@@ -250,9 +255,31 @@ int parse_request(Server& sv, const std::string& path, const std::string& ctype,
   if (const JVal* so = root.get("stream_options"))
     if (const JVal* iu = so->get("include_usage"); iu && iu->type == JVal::Bool) pr->include_usage = iu->b;
   if (const JVal* v = root.get("ignore_eos"); v && v->type == JVal::Bool) pr->ignore_eos = v->b;
+  // sampling (vLLM's request fields; top_k is its extension).  The JSON numbers are doubles: an integer field that is not
+  // an exact integer, or a seed beyond 2^53, is refused rather than rounded.
+  const char* bad_sampling = nullptr;
   if (const JVal* v = root.get("temperature"); v && v->type == JVal::Num) {
     pr->temperature = v->num;
-    pr->has_temperature = true;
+    if (!(v->num >= 0 && v->num <= 3.0e38)) bad_sampling = "temperature must be a finite number >= 0";   // finite as a float too
+  }
+  if (const JVal* v = root.get("top_p"); v && v->type == JVal::Num) {
+    pr->top_p = v->num;
+    if (!(v->num > 0 && v->num <= 1)) bad_sampling = "top_p must be in (0, 1]";
+  }
+  if (const JVal* v = root.get("top_k"); v && v->type == JVal::Num) {
+    if (!(v->num >= -1 && v->num == std::floor(v->num) && v->num <= 2147483647.0)) bad_sampling = "top_k must be an integer >= -1";
+    else pr->top_k = static_cast<int>(v->num);
+  }
+  if (const JVal* v = root.get("seed"); v && v->type == JVal::Num) {
+    if (!(v->num == std::floor(v->num) && std::fabs(v->num) <= 9007199254740992.0)) bad_sampling = "seed must be an integer of magnitude <= 2^53";
+    else {
+      pr->seed = static_cast<int64_t>(v->num);
+      pr->has_seed = true;
+    }
+  }
+  if (bad_sampling) {
+    *err = std::string("bad request: ") + bad_sampling;
+    return 400;
   }
   if (const JVal* v = root.get("stop_token_ids"); v && v->type == JVal::Arr)
     for (auto& e : v->arr)
@@ -280,6 +307,7 @@ int parse_request(Server& sv, const std::string& path, const std::string& ctype,
   else if (nonempty("logit_bias")) bad = "logit_bias";
   else if (nonempty("tools") || nonempty("functions")) bad = "tool calling";
   else if (truthy("min_tokens")) bad = "min_tokens";
+  else if (num_of("min_p", 0) > 0 && pr->temperature >= 1e-5) bad = "min_p";   // harmless under greedy decoding only
   else if (const JVal* rf = root.get("response_format"); rf && rf->type == JVal::Obj) {
     const JVal* ty = rf->get("type");
     if (ty && ty->type == JVal::Str && ty->str != "text") bad = "response_format other than text";
@@ -345,9 +373,9 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
   ParsedRequest pr;
   std::string err;
   if (int st = parse_request(sv, path, ctype, body, len, &pr, &err)) return send_error(w, st, err);
-  if (pr.has_temperature && pr.temperature >= 1e-5) {
-    // greedy only (north star); refuse rather than silently change semantics
-    return send_error(w, 400, "bad request: only greedy sampling is implemented: set \"temperature\": 0");
+  if (!sv.sampling && pr.temperature >= 1e-5) {
+    // a greedy-only server (enable_sampling 0) refuses rather than silently decoding greedily
+    return send_error(w, 400, "bad request: only greedy sampling is enabled on this server: set \"temperature\": 0");
   }
   // tokenise (K13)
   std::vector<int32_t> ids;
@@ -399,9 +427,13 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
     tokens_held.push_back(ep_token);
     const int replica = atoi(addr + 4);  // "gpu:<i>"
     b200_engine* eng = sv.replicas[replica];
-    b200_sampling sp;
+    b200_sampling sp{};
     sp.max_tokens = max_tokens;
-    sp.temperature = 0.f;
+    sp.temperature = static_cast<float>(pr.temperature);
+    sp.top_p = static_cast<float>(pr.top_p);
+    sp.top_k = pr.top_k;
+    sp.has_seed = pr.has_seed ? 1 : 0;
+    sp.seed = static_cast<uint64_t>(pr.seed);
     sp.ignore_eos = pr.ignore_eos ? 1 : 0;
     std::vector<int32_t> stops = pr.stop_ids;
     if (sv.real_tok && !pr.ignore_eos) {   // the checkpoint's end-of-turn / end-of-text tokens end the generation
@@ -725,6 +757,7 @@ int b200_server_create(const b200_server_config* cfg, b200_engine* const* replic
   sv.default_max_tokens = cfg->default_max_tokens > 0 ? cfg->default_max_tokens : 256;
   sv.tok.vocab = cfg->vocab > 258 ? cfg->vocab : 128256;
   sv.max_model_len = cfg->max_model_len > 0 ? cfg->max_model_len : 2048;
+  sv.sampling = cfg->enable_sampling != 0;
   if (b200_router_create(sv.replication, &sv.router)) { delete s; return B200_ERR_INVALID; }
   std::vector<std::string> names;
   std::string ad = cfg->adapters ? cfg->adapters : "";

@@ -77,12 +77,16 @@ class Engine:
         except Exception:
             pass
 
-    def submit(self, prompt_ids, max_tokens=16, ignore_eos=True, stop_ids=()) -> int:
+    def submit(self, prompt_ids, max_tokens=16, ignore_eos=True, stop_ids=(), temperature=0.0, top_p=1.0, top_k=0,
+               seed=None) -> int:
+        """temperature < 1e-5 is greedy; top_k 0 / -1 and top_p 1 are off; seed None = one drawn by the engine."""
         ids = np.ascontiguousarray(prompt_ids, dtype=np.int32)
         stops = np.ascontiguousarray(stop_ids, dtype=np.int32)
-        sp = Sampling(max_tokens=max_tokens, temperature=0.0, ignore_eos=1 if ignore_eos else 0,
+        sp = Sampling(max_tokens=max_tokens, temperature=temperature, ignore_eos=1 if ignore_eos else 0,
                       num_stop_ids=len(stops),
-                      stop_ids=stops.ctypes.data_as(C.POINTER(C.c_int32)) if len(stops) else None)
+                      stop_ids=stops.ctypes.data_as(C.POINTER(C.c_int32)) if len(stops) else None,
+                      top_p=top_p, top_k=top_k, has_seed=0 if seed is None else 1,
+                      seed=0 if seed is None else seed & 0xFFFFFFFFFFFFFFFF)
         rid = C.c_uint64()
         check(self._l.b200_submit(self._h, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), C.byref(sp),
                                   C.byref(rid)))

@@ -5,6 +5,7 @@ from __future__ import annotations
 
 import ctypes as C
 
+import numpy as np
 import torch
 
 from ._lib import check, lib
@@ -123,6 +124,27 @@ def argmax(logits):
     _chk(logits)
     out = torch.empty(logits.shape[0], dtype=torch.int32, device=logits.device)
     check(lib().b200_op_argmax(_p(logits), _p(out), logits.shape[0], logits.shape[1], logits.stride(0), _stream()))
+    return out
+
+
+def sample(logits, temperature, top_k=0, top_p=1.0, seed=0, n=0):
+    """Token per row of bf16 logits [S, V] (b200_op_sample).  Each parameter is a scalar or one value per row:
+    temperature < 1e-5 = greedy; top_k 0 / -1 / >= V and top_p 1 = off; seed (uint64) keys the row's Philox stream and
+    n (the index of the token being generated) counts it."""
+    _chk(logits)
+    S = logits.shape[0]
+    rows = np.empty(S, dtype=[("temperature", "<f4"), ("top_k", "<i4"), ("top_p", "<f4"), ("seed_lo", "<u4"),
+                              ("seed_hi", "<u4"), ("n", "<i4")])
+    seed = np.broadcast_to(np.asarray(seed, dtype=object), (S,))
+    rows["temperature"] = np.broadcast_to(np.asarray(temperature, dtype=np.float32), (S,))
+    rows["top_k"] = np.broadcast_to(np.asarray(top_k, dtype=np.int32), (S,))
+    rows["top_p"] = np.broadcast_to(np.asarray(top_p, dtype=np.float32), (S,))
+    rows["seed_lo"] = [int(s) & 0xFFFFFFFF for s in seed]
+    rows["seed_hi"] = [(int(s) >> 32) & 0xFFFFFFFF for s in seed]
+    rows["n"] = np.broadcast_to(np.asarray(n, dtype=np.int32), (S,))
+    rows_dev = torch.from_numpy(rows.view(np.int32).reshape(S, 6).copy()).to(logits.device)
+    out = torch.empty(S, dtype=torch.int32, device=logits.device)
+    check(lib().b200_op_sample(_p(logits), logits.stride(0), _p(rows_dev), S, logits.shape[1], _p(out), _stream()))
     return out
 
 

@@ -39,9 +39,12 @@ class Response:
 
 
 class Server:
+    """enable_sampling: serve requests with temperature >= 1e-5 (temperature / top_p / top_k / seed); off, they get a 400
+    and the server decodes greedily only (the serving shell's behaviour before sampling existed)."""
+
     def __init__(self, engines, model="llama-3-8b", adapters=None, strategy=LEAST_LOAD, mean_load_pct=125,
                  replication=256, prefix_char_length=100, max_retries=3, default_max_tokens=256, vocab=128256,
-                 max_model_len=2048):
+                 max_model_len=2048, enable_sampling=False):
         self._l = lib()
         self._engines = list(engines)   # keep alive; entries may be None for parse-path-only tests
         n = len(self._engines)
@@ -49,7 +52,8 @@ class Server:
         cfg = ServerConfig(model=model.encode(), adapters=",".join(adapters).encode() if adapters else None,
                            strategy=strategy, mean_load_pct=mean_load_pct, replication=replication,
                            prefix_char_length=prefix_char_length, max_retries=max_retries,
-                           default_max_tokens=default_max_tokens, vocab=vocab, max_model_len=max_model_len)
+                           default_max_tokens=default_max_tokens, vocab=vocab, max_model_len=max_model_len,
+                           enable_sampling=1 if enable_sampling else 0)
         self._h = C.c_void_p()
         check(self._l.b200_server_create(C.byref(cfg), arr, n, C.byref(self._h)))
 
