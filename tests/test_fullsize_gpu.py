@@ -20,6 +20,7 @@ import torch
 
 from oracle import llama_oracle as O
 from oracle.weights import ModelCfg, bf16_bits_to_f32, cos_sin_cache
+from test_attention_exact_gpu import assert_rms_close
 
 pytestmark = pytest.mark.gpu
 LOGIT_ULPS = 6.0          # hard bound; all but 1e-5 of the logits must be within LOGIT_ULPS_BULK
@@ -207,6 +208,7 @@ def _attn_close(got, want, what):
     err = (got - want).abs()
     tol = 4e-3 + 1.6e-2 * want.abs()          # vLLM bf16 tolerance (rtol 1.6e-2) + bf16 rounding of P and of the output
     assert bool((err <= tol).all()), f"{what}: max err {float(err.max()):.4g}, {int((err > tol).sum())} outside tolerance"
+    assert_rms_close(got, want, what)         # and per (row, head) relative to the output's size: catches one wrong token
 
 
 def test_decode_attention_at_production_shape():
@@ -279,3 +281,39 @@ def test_chunked_prefill_attention_at_production_shape_with_cached_prefix(kernel
         qi = q[t0:t0 + n, :Hq * 128].float().reshape(n, Hq, 128)
         want = O.attention(qi, ks[i], vs[i], torch.arange(L - n, L, device="cuda"), 128 ** -0.5).reshape(n, Hq * 128)
         _attn_close(got[t0:t0 + n], want, f"prefill seq {i} ctx {L} new {n}")
+
+
+@pytest.mark.parametrize("kernel", ["decode", "decode_split_7", "tensor_core", "mma_sync"])
+def test_peaky_attention_at_production_shape(kernel):
+    """Random data with queries x 4: a few tokens carry most of each softmax, so P's bf16 rounding lands on large weights."""
+    from kubeai_b200 import ops
+    Hq, Hkv = 32, 8
+    case = [(2048, 1 if kernel.startswith("decode") else 200), (1023, 1 if kernel.startswith("decode") else 64), (65, 1), (4097, 1)]
+    lens = [c[0] for c in case]
+    kv, btab, ks, vs = _pool(lens, Hkv, seed=24)
+    qb = 64 if kernel == "tensor_core" else 16
+    T = sum(n for _, n in case)
+    q = 4 * torch.randn(T, Hq * 128, generator=torch.Generator(device="cuda").manual_seed(6), device="cuda").bfloat16()
+    work, spans, tok = [], [], 0
+    for i, (L, n) in enumerate(case):
+        for j in range(0, n, 1 if kernel.startswith("decode") else qb):
+            work.append([tok + j, min(qb, n - j), L - n + j, i])
+        spans.append(tok)
+        tok += n
+    wt = torch.tensor(work, dtype=torch.int32).cuda()
+    if kernel == "decode":
+        got = ops.paged_attn(q, kv, btab, wt, Hq, Hkv, decode=True)
+    elif kernel == "decode_split_7":
+        got = ops.paged_attn(q, kv, btab, wt, Hq, Hkv, decode=True, split=7)
+    elif kernel == "tensor_core":
+        got = ops.paged_attn_prefill_tc(q, kv, btab, wt, Hq, Hkv)
+    else:
+        got = ops.paged_attn(q, kv, btab, wt, Hq, Hkv, decode=False)
+    got = got.float()
+    torch.cuda.synchronize()
+    for i, (L, n) in enumerate(case):
+        t0 = spans[i]
+        qi = q[t0:t0 + n].float().reshape(n, Hq, 128)
+        want = O.attention(qi.double(), ks[i].double(), vs[i].double(), torch.arange(L - n, L, device="cuda"),
+                           128 ** -0.5).reshape(n, Hq * 128)
+        _attn_close(got[t0:t0 + n], want, f"peaky {kernel} seq {i} ctx {L} new {n}")

@@ -7,6 +7,7 @@ import torch
 
 from oracle import llama_oracle as O
 from oracle.weights import init_uniform as np_init_uniform
+from test_attention_exact_gpu import assert_rms_close
 
 pytestmark = pytest.mark.gpu
 
@@ -229,6 +230,7 @@ def test_paged_attention_decode(seq_lens, Hkv):
         _, q, k, v, _ = seqs[i]
         want = O.attention(q[-1:], k, v, torch.tensor([L - 1]), 128 ** -0.5).reshape(1, Hq * 128)
         close(got[i:i + 1], want, atol=4e-3, what=f"decode attn seq {i} len {L}")
+        assert_rms_close(got[i:i + 1], want, f"decode attn seq {i} len {L}")
 
 
 @pytest.mark.parametrize("case", [
@@ -257,6 +259,7 @@ def test_paged_attention_prefill(case):
         want = O.attention(q[L - n:], k, v, torch.arange(L - n, L), 128 ** -0.5).reshape(n, Hq * 128)
         t0 = spans[i][0]
         close(got[t0:t0 + n], want, atol=4e-3, what=f"prefill attn seq {i}")
+        assert_rms_close(got[t0:t0 + n], want, f"prefill attn seq {i}")
 
 
 @pytest.mark.parametrize("case", [
@@ -289,3 +292,4 @@ def test_paged_attention_prefill_tensor_core(case, Hkv):
         want = O.attention(q[L - n:], k, v, torch.arange(L - n, L), 128 ** -0.5).reshape(n, Hq * 128)
         t0 = spans[i][0]
         close(got[t0:t0 + n], want, atol=4e-3, what=f"tensor-core prefill attn seq {i} (ctx {L}, new {n})")
+        assert_rms_close(got[t0:t0 + n], want, f"tensor-core prefill attn seq {i} (ctx {L}, new {n})")
