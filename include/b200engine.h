@@ -79,7 +79,13 @@ typedef struct {
   int32_t top_k;              /* >= -1; 0, -1 or >= vocab = off */
   int32_t has_seed;           /* 0: the engine draws a seed for the request (not reproducible, as in vLLM and OpenAI) */
   uint64_t seed;
+  /* Log-probabilities of every generated token (vLLM's raw_logprobs: log_softmax in fp32 of the bf16 logits, before
+   * temperature / top-k / top-p; the sampled tokens do not change), read with b200_poll_logprobs. */
+  int32_t logprobs;           /* 0 = off */
+  int32_t top_logprobs;       /* 0..B200_MAX_LOGPROBS most likely tokens per position; > 0 needs logprobs */
 } b200_sampling;
+
+#define B200_MAX_LOGPROBS 20  /* vLLM's default max_logprobs */
 
 typedef struct {
   int32_t prompt_tokens;
@@ -117,6 +123,12 @@ int b200_submit(b200_engine* e, const int32_t* prompt_ids, int32_t n, const b200
 /* Drain newly generated token ids (at most cap).  *finished gets a B200_FINISH_* code or 0. */
 int b200_poll(b200_engine* e, uint64_t req_id, int32_t* out_ids, int32_t cap, int32_t* n_out, int32_t* finished,
               b200_usage* usage);
+/* b200_poll with each token's log-probability record (the request must have been submitted with logprobs, else
+ * B200_ERR_INVALID).  Both calls drain the same cursor.  For token k: out_logprob[k] is its own log-probability,
+ * out_top_ids / out_top_logprob[k * B200_MAX_LOGPROBS + j], j < top_logprobs, the most likely tokens in descending order
+ * (lowest id on equal logits); the rest of each row is left as it was. */
+int b200_poll_logprobs(b200_engine* e, uint64_t req_id, int32_t* out_ids, float* out_logprob, int32_t* out_top_ids,
+                       float* out_top_logprob, int32_t cap, int32_t* n_out, int32_t* finished, b200_usage* usage);
 /* Block until the request has undrained tokens or is finished (B200_ERR_TIMEOUT otherwise). */
 int b200_wait(b200_engine* e, uint64_t req_id, int64_t timeout_us);
 int b200_abort(b200_engine* e, uint64_t req_id);
@@ -243,6 +255,9 @@ typedef struct {
   /* 1: requests with temperature >= 1e-5 are sampled (temperature / top_p / top_k / seed, see b200_sampling); 0: they get
    * a 400 and the server decodes greedily only, as before sampling existed (a zero-initialised config keeps that) */
   int32_t enable_sampling;
+  /* 1: serve logprobs (chat: "logprobs": true + "top_logprobs" 0..20; completions: "logprobs" 0..20) in vLLM's response
+   * format; 0: they get a 400, as before logprobs existed (a zero-initialised config keeps that) */
+  int32_t enable_logprobs;
 } b200_server_config;
 int b200_server_create(const b200_server_config* cfg, b200_engine* const* replicas, int32_t n, b200_server** out);
 void b200_server_destroy(b200_server* s);
@@ -405,6 +420,12 @@ typedef struct {
 /* out[s] = the token sampled from bf16 logits row s ([S, ld], ld % 8 == 0, V <= ld) under rows[s]; rows and out are device
  * memory.  Greedy rows give the same token as b200_op_argmax. */
 int b200_op_sample(const void* logits, int32_t ld, const b200_sample_row* rows, int32_t S, int32_t V, int32_t* out, void* stream);
+/* Log-probabilities of bf16 logits rows [S, ld] (ld % 8 == 0, V <= ld), as the engine computes them: out_logprob[s] for
+ * tokens[s]; out_top_ids / out_top_logprob [S][B200_MAX_LOGPROBS], entries j < top_n[s] (clamped to 0..20), the most
+ * likely tokens in descending order, lowest id on equal logits.  Entries past a row's N are left as they were.  Every
+ * pointer is device memory. */
+int b200_op_logprobs(const void* logits, int32_t ld, int32_t S, int32_t V, const int32_t* tokens, const int32_t* top_n,
+                     float* out_logprob, int32_t* out_top_ids, float* out_top_logprob, void* stream);
 /* work: int32[num_work][4] = {q_tok0, q_count, q_pos0, seq}; kv_layer: [block][2][kv_heads][16][128] */
 int b200_op_paged_attn(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                        const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,

@@ -44,7 +44,8 @@ class Gemm3Args(C.Structure):
 class Sampling(C.Structure):
     _fields_ = [("max_tokens", C.c_int32), ("temperature", C.c_float), ("ignore_eos", C.c_int32),
                 ("num_stop_ids", C.c_int32), ("stop_ids", C.POINTER(C.c_int32)),
-                ("top_p", C.c_float), ("top_k", C.c_int32), ("has_seed", C.c_int32), ("seed", C.c_uint64)]
+                ("top_p", C.c_float), ("top_k", C.c_int32), ("has_seed", C.c_int32), ("seed", C.c_uint64),
+                ("logprobs", C.c_int32), ("top_logprobs", C.c_int32)]
 
 
 class SampleRow(C.Structure):
@@ -82,7 +83,7 @@ class ServerConfig(C.Structure):
     _fields_ = [("model", C.c_char_p), ("adapters", C.c_char_p), ("strategy", C.c_int32),
                 ("mean_load_pct", C.c_int32), ("replication", C.c_int32), ("prefix_char_length", C.c_int32),
                 ("max_retries", C.c_int32), ("default_max_tokens", C.c_int32), ("vocab", C.c_int32),
-                ("max_model_len", C.c_int32), ("enable_sampling", C.c_int32)]
+                ("max_model_len", C.c_int32), ("enable_sampling", C.c_int32), ("enable_logprobs", C.c_int32)]
 
 
 class HarnessConfig(C.Structure):
@@ -120,6 +121,7 @@ SYMBOLS = {
     "b200_engine_destroy": (None, [_vp]),
     "b200_submit": (C.c_int, [_vp, _pi32, _i32, C.POINTER(Sampling), C.POINTER(_u64)]),
     "b200_poll": (C.c_int, [_vp, _u64, _pi32, _i32, _pi32, _pi32, C.POINTER(Usage)]),
+    "b200_poll_logprobs": (C.c_int, [_vp, _u64, _pi32, _vp, _pi32, _vp, _i32, _pi32, _pi32, C.POINTER(Usage)]),
     "b200_wait": (C.c_int, [_vp, _u64, _i64]),
     "b200_abort": (C.c_int, [_vp, _u64]),
     "b200_release": (C.c_int, [_vp, _u64]),
@@ -184,6 +186,7 @@ SYMBOLS = {
     "b200_op_silu_mul": (C.c_int, [_vp, _vp, _i32, _i32, _vp]),
     "b200_op_argmax": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _vp]),
     "b200_op_sample": (C.c_int, [_vp, _i32, _vp, _i32, _i32, _vp, _vp]),
+    "b200_op_logprobs": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "b200_op_paged_attn": (C.c_int, [_vp, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _f, _i32, _vp]),
     "b200_server_set_tokenizer": (C.c_int, [C.c_void_p, C.c_void_p]),
     "b200_server_render_prompt": (C.c_int64, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_size_t, _vp, C.c_size_t]),

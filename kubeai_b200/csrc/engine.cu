@@ -163,6 +163,13 @@ class BlockPool {
 };
 
 // ------------------------------------------------------------------ sequences
+// one generated token's log-probabilities (sampling.cu logprobs_rows): its own, then its request's top N
+struct LogprobRecord {
+  float lp;
+  float top_lp[kMaxLogprobs];
+  int32_t top_ids[kMaxLogprobs];
+};
+
 struct Seq {
   uint64_t id = 0;
   std::vector<int32_t> toks;  // prompt + generated
@@ -178,6 +185,7 @@ struct Seq {
   float temperature = 0.f, top_p = 1.f;
   int top_k = 0;
   uint64_t seed = 0;
+  int top_logprobs = -1;   // -1: no logprobs; else the N of every generated token's record
   int n_generated = 0;
   std::atomic<int> n_cached{-1};  // prefix-hit tokens at first admission
   bool admitted = false;
@@ -186,6 +194,7 @@ struct Seq {
   std::mutex m;
   std::condition_variable cv;
   std::vector<int32_t> out;
+  std::vector<LogprobRecord> lp_out;   // one per token of `out` when top_logprobs >= 0
   size_t drained = 0;
   int finished = 0;
   uint64_t arrival_key = 0;   // xxh64 of the prompt: admission order among requests that arrive between two steps
@@ -208,12 +217,15 @@ struct Pub {
   int32_t tok;
   bool has_tok;
   int code;
+  int lp = -1;   // index of the token's record in Engine::pending_lp
 };
 
 struct StepMeta {
   int T = 0, nd = 0, np = 0, S = 0, nseq = 0;
   int off_ids = 0, off_pos = 0, off_slots = 0, off_rows = 0, off_dwork = 0, off_pwork = 0, off_btab = 0;
   int off_samp = -1;   // SampleRow per sampled row, packed only when one of them has temperature >= 1e-5
+  int off_lp = -1;     // logprobs rows: n_lp row indices into [0, S), then their n_lp N values; packed only when n_lp > 0
+  int n_lp = 0;
   int words = 0;
   int64_t kv_tokens = 0;
   int out_tokens = 0;  // sampled rows that produce a generated token
@@ -252,6 +264,12 @@ struct Engine {
        *last_hidden = nullptr, *logits = nullptr;
   int* sampled = nullptr;
   int32_t* sampled_host = nullptr;  // pinned
+  // logprobs of the rows that asked, in step order: [Scap][1 + kMaxLogprobs] floats (the token's lp, then the top N) and
+  // [Scap][kMaxLogprobs] ids; device and pinned host copies
+  float* lp_dev = nullptr;
+  int* lp_ids_dev = nullptr;
+  float* lp_host = nullptr;
+  int32_t* lp_ids_host = nullptr;
   // fused epilogues (gemm_wgmma.cu): RoPE + KV write, residual add, SiLU * up and per-slab argmax ride in the projection
   // that produces their input; off (B200_FUSED_DECODE=0 / B200_FUSED_PREFILL=0) each runs as its own elementwise kernel
   float2* cand = nullptr;    // argmax candidates [token][V / 128 slab]
@@ -329,10 +347,12 @@ struct Engine {
   void fail_all();
   void loop();
   std::vector<Pub> pending_pub;
+  std::vector<LogprobRecord> pending_lp;   // records of pending_pub entries (Pub::lp)
   InFlight inflight_;
   std::vector<AttnWork> dwork_, pwork_;  // packing scratch (kept across steps: no per-step allocation)
   std::vector<int> rows_;
   std::vector<SampleRow> samp_;          // parameters of the rows in rows_ order
+  std::vector<int> lp_rows_, lp_n_;      // logprobs rows (indices into rows_) and their N
   bool ensure_blocks(Seq& s, int upto);
   void release_blocks(Seq& s);
   void preempt(std::shared_ptr<Seq> s);
@@ -394,13 +414,15 @@ Engine::~Engine() {
   cudaSetDevice(cfg.device);
   if (stream) cudaStreamSynchronize(stream);
   void* frees[] = {weights_blob, res, x, normed, qkv, attn, gu, act, last_hidden, logits, sampled, gemm_ws,
-                   gemm_counters, kv, cand, attn_ws};
+                   gemm_counters, kv, cand, attn_ws, lp_dev, lp_ids_dev};
   for (void* p : frees)
     if (p) cudaFree(p);
   for (auto p : stage_dev)
     if (p) cudaFree(p);
   if (stage_host) cudaFreeHost(stage_host);
   if (sampled_host) cudaFreeHost(sampled_host);
+  if (lp_host) cudaFreeHost(lp_host);
+  if (lp_ids_host) cudaFreeHost(lp_ids_host);
   if (ev0) cudaEventDestroy(ev0);
   if (ev1) cudaEventDestroy(ev1);
   if (stream) cudaStreamDestroy(stream);
@@ -516,6 +538,10 @@ int Engine::alloc_all() {
   CK(cudaMemset(act, 0, static_cast<size_t>(Tcap) * I * 2));
   CK(cudaMemset(last_hidden, 0, static_cast<size_t>(Scap) * H * 2));
   CK(cudaMallocHost(&sampled_host, static_cast<size_t>(Scap) * 4));
+  CK(cudaMalloc(&lp_dev, static_cast<size_t>(Scap) * (1 + kMaxLogprobs) * sizeof(float)));
+  CK(cudaMalloc(&lp_ids_dev, static_cast<size_t>(Scap) * kMaxLogprobs * sizeof(int)));
+  CK(cudaMallocHost(&lp_host, static_cast<size_t>(Scap) * (1 + kMaxLogprobs) * sizeof(float)));
+  CK(cudaMallocHost(&lp_ids_host, static_cast<size_t>(Scap) * kMaxLogprobs * sizeof(int32_t)));
   CK(cudaMalloc(&cand, static_cast<size_t>(std::min(Scap, 128)) * ((V + 127) / 128) * sizeof(float2)));
   // outputs of the last step, readable by name (b200_engine_tensor_read): sampled ids int32 [S]; the lm_head's per-slab
   // {best logit, index} candidates float2 [S][ceil(V / 128)] when the step sampled through them, else bf16 logits [S][V]
@@ -599,7 +625,7 @@ int Engine::alloc_all() {
 
   // ---- step input ring
   max_blocks_per_seq = (cfg.max_model_len + kPage - 1) / kPage;
-  step_words_cap = 3 * Tcap + Scap + 4 * Scap + 4 * (Tcap / 16 + Scap + 1) + Scap * max_blocks_per_seq + 6 * Scap + 64;
+  step_words_cap = 3 * Tcap + Scap + 4 * Scap + 4 * (Tcap / 16 + Scap + 1) + Scap * max_blocks_per_seq + 6 * Scap + 2 * Scap + 64;
   static_assert(sizeof(SampleRow) == 6 * sizeof(int32_t), "SampleRow is 6 words of the step input");
   ring_n = std::max(1, cfg.record_steps) + 1;  // last slot = scratch for unrecorded steps
   CK(cudaMallocHost(&stage_host, static_cast<size_t>(step_words_cap) * 4));
@@ -739,9 +765,9 @@ int Engine::forward(const StepMeta& m, int32_t* dbuf, bool all_logits, bf16* log
     P(B200_K_NORM); norm(final_norm, last_hidden, rows, m.S); Q();
     // argmax candidates per 128-row slab in the lm_head epilogue (the candidate buffer holds 128 rows), or bf16 logits.
     // A step with a sampled row (temperature >= 1e-5) writes the logits and selects every row's token in one sample_rows
-    // launch, greedy rows included.
+    // launch, greedy rows included.  A step with a logprobs row writes the logits too, for logprobs_rows.
     const bool samp = m.off_samp >= 0;
-    const bool cand_ok = !samp && fused && !keep_logits && m.S <= 128;
+    const bool cand_ok = !samp && m.n_lp == 0 && fused && !keep_logits && m.S <= 128;
     Gemm3Params p = proj(p_lm, cand_ok ? GEMM3_EPI_ARGMAX : GEMM3_EPI_PLAIN);
     p.out = logits; p.ldo = V; p.cand = cand;
     P(B200_K_GEMM_LM); rc |= launch_proj(p, xm_last, m.S); Q();
@@ -752,6 +778,14 @@ int Engine::forward(const StepMeta& m, int32_t* dbuf, bool all_logits, bf16* log
     else rc |= argmax_rows(logits, sampled, m.S, V, V, stream);
     Q();
     launched(1);
+    if (m.n_lp > 0) {   // after the token selection: it reads the sampled ids
+      const int* lr = dbuf + m.off_lp;
+      P(B200_K_ARGMAX);
+      rc |= logprobs_rows(logits, V, V, lr, lr + m.n_lp, m.n_lp, sampled, lp_dev, 1 + kMaxLogprobs, lp_dev + 1,
+                          1 + kMaxLogprobs, lp_ids_dev, stream);
+      Q();
+      launched(1);
+    }
   }
   if (rc) return cuda_fail("forward(head)", -2);
   return 0;
@@ -794,11 +828,13 @@ void Engine::publish() {
     {
       std::lock_guard<std::mutex> lk(p.s->m);
       if (p.has_tok) p.s->out.push_back(p.tok);
+      if (p.lp >= 0) p.s->lp_out.push_back(pending_lp[p.lp]);
       if (p.code) p.s->finished = p.code;
     }
     p.s->cv.notify_all();
   }
   pending_pub.clear();
+  pending_lp.clear();
 }
 
 void Engine::admit_prefix(Seq& s) {
@@ -925,6 +961,8 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
   pwork_.clear();
   rows_.clear();
   samp_.clear();
+  lp_rows_.clear();
+  lp_n_.clear();
   bool any_sampled = false;
   int32_t* h = stage_host;
   m.off_ids = 0; m.off_pos = m.T; m.off_slots = 2 * m.T;
@@ -955,6 +993,10 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
       samp_.push_back({s.temperature, s.top_k, s.top_p, static_cast<uint32_t>(s.seed), static_cast<uint32_t>(s.seed >> 32),
                        s.n_generated});
       any_sampled |= s.temperature >= 1e-5f;
+      if (s.top_logprobs >= 0) {
+        lp_rows_.push_back(static_cast<int>(rows_.size()) - 1);
+        lp_n_.push_back(s.top_logprobs);
+      }
     }
     tok += n;
   }
@@ -984,6 +1026,13 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
     memcpy(h + w, samp_.data(), samp_.size() * sizeof(SampleRow));
     w += 6 * m.S;
   }
+  m.n_lp = static_cast<int>(lp_rows_.size());
+  if (m.n_lp > 0) {   // likewise steps without a logprobs row carry no logprobs section
+    m.off_lp = w;
+    memcpy(h + w, lp_rows_.data(), lp_rows_.size() * 4);
+    memcpy(h + w + m.n_lp, lp_n_.data(), lp_n_.size() * 4);
+    w += 2 * m.n_lp;
+  }
   m.words = w;
   if (w > step_words_cap) {
     set_error("step staging overflow (%d > %d words)", w, step_words_cap);
@@ -1010,6 +1059,10 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
   if (frc) return frc;
   CK(cudaEventRecord(ev1, stream));
   if (m.S) CK(cudaMemcpyAsync(sampled_host, sampled, static_cast<size_t>(m.S) * 4, cudaMemcpyDeviceToHost, stream));
+  if (m.n_lp) {
+    CK(cudaMemcpyAsync(lp_host, lp_dev, static_cast<size_t>(m.n_lp) * (1 + kMaxLogprobs) * sizeof(float), cudaMemcpyDeviceToHost, stream));
+    CK(cudaMemcpyAsync(lp_ids_host, lp_ids_dev, static_cast<size_t>(m.n_lp) * kMaxLogprobs * sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
+  }
   f->t_launched = timing ? now_s() : 0.0;
   f->words = w;
   *mp = m;
@@ -1025,7 +1078,7 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
   float ms = 0.f;
   cudaEventElapsedTime(&ms, ev0, ev1);
 
-  int ri = 0;
+  int ri = 0, li = 0;
   int64_t gen = 0;
   bool any_done = false;
   for (int si = 0; si < m.nseq; ++si) {
@@ -1050,7 +1103,18 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
     for (int sid : s.stop_ids) if (t == sid) code = B200_FINISH_STOP;
     if (!code && s.n_generated >= s.max_tokens) code = B200_FINISH_LENGTH;
     if (!code && static_cast<int>(s.toks.size()) >= cfg.max_model_len) code = B200_FINISH_LENGTH;
-    pending_pub.push_back({sp, t, true, code});
+    int lp = -1;
+    if (s.top_logprobs >= 0) {   // records come back in step order, as the ids do
+      LogprobRecord r;
+      const float* src = lp_host + static_cast<size_t>(li) * (1 + kMaxLogprobs);
+      r.lp = src[0];
+      memcpy(r.top_lp, src + 1, sizeof(r.top_lp));
+      memcpy(r.top_ids, lp_ids_host + static_cast<size_t>(li) * kMaxLogprobs, sizeof(r.top_ids));
+      ++li;
+      lp = static_cast<int>(pending_lp.size());
+      pending_lp.push_back(r);
+    }
+    pending_pub.push_back({sp, t, true, code, lp});
     if (code) {
       release_blocks(s);
       s.leaving = true;
@@ -1071,7 +1135,7 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
     stats.total_device_us += ms * 1000.0;
     stats.last_step_tokens = m.T;
     stats.h2d_bytes += static_cast<int64_t>(f.words) * 4;
-    stats.d2h_bytes += static_cast<int64_t>(m.S) * 4;
+    stats.d2h_bytes += static_cast<int64_t>(m.S) * 4 + static_cast<int64_t>(m.n_lp) * (1 + 2 * kMaxLogprobs) * 4;
     stats.running = static_cast<int>(running.size());
     stats.waiting = static_cast<int>(waiting.size());
     stats.kv_blocks_free = pool.free_count();
@@ -1153,6 +1217,7 @@ void Engine::fail_all() {
     incoming.clear();
   }
   pending_pub.clear();
+  pending_lp.clear();
   for (auto& s : all) {
     { std::lock_guard<std::mutex> lk(s->m); s->finished = B200_FINISH_ERROR; }
     s->cv.notify_all();
@@ -1239,6 +1304,8 @@ int b200_submit(b200_engine* e, const int32_t* prompt_ids, int32_t n, const b200
   if (sp && !(std::isfinite(sp->temperature) && sp->temperature >= 0.f)) { set_error("temperature must be finite and >= 0"); return B200_ERR_INVALID; }
   if (sp && !(sp->top_p >= 0.f && sp->top_p <= 1.f)) { set_error("top_p must be in [0, 1]"); return B200_ERR_INVALID; }
   if (sp && sp->top_k < -1) { set_error("top_k must be >= -1"); return B200_ERR_INVALID; }
+  if (sp && (sp->top_logprobs < 0 || sp->top_logprobs > B200_MAX_LOGPROBS)) { set_error("top_logprobs must be in 0..%d", B200_MAX_LOGPROBS); return B200_ERR_INVALID; }
+  if (sp && sp->top_logprobs > 0 && !sp->logprobs) { set_error("top_logprobs needs logprobs"); return B200_ERR_INVALID; }
   for (int i = 0; i < n; ++i) if (prompt_ids[i] < 0 || prompt_ids[i] >= g.V) { set_error("token id out of range"); return B200_ERR_INVALID; }
   auto s = std::make_shared<Seq>();
   s->toks.assign(prompt_ids, prompt_ids + n);
@@ -1251,6 +1318,7 @@ int b200_submit(b200_engine* e, const int32_t* prompt_ids, int32_t n, const b200
     s->temperature = sp->temperature;
     s->top_p = sp->top_p > 0.f ? sp->top_p : 1.f;   // 0 = off at this ABI
     s->top_k = sp->top_k > 0 ? sp->top_k : 0;
+    s->top_logprobs = sp->logprobs ? sp->top_logprobs : -1;
   }
   {
     std::lock_guard<std::mutex> lk(g.mu_);
@@ -1289,8 +1357,9 @@ static std::shared_ptr<Seq> find_req(Engine& g, uint64_t id) {
   return it == g.requests.end() ? nullptr : it->second;
 }
 
-int b200_poll(b200_engine* e, uint64_t req_id, int32_t* out_ids, int32_t cap, int32_t* n_out, int32_t* finished,
-              b200_usage* usage) {
+// b200_poll and b200_poll_logprobs: one drain cursor, so ids and their records never come apart
+static int poll_impl(b200_engine* e, uint64_t req_id, int32_t* out_ids, float* out_lp, int32_t* out_top_ids,
+                     float* out_top_lp, int32_t cap, int32_t* n_out, int32_t* finished, b200_usage* usage) {
   if (!e || !n_out) { set_error("b200_poll: bad arguments"); return B200_ERR_INVALID; }
   Engine& g = e->impl;
   std::shared_ptr<Seq> s;
@@ -1299,9 +1368,19 @@ int b200_poll(b200_engine* e, uint64_t req_id, int32_t* out_ids, int32_t cap, in
     s = find_req(g, req_id);
   }
   if (!s) { set_error("unknown request %llu", static_cast<unsigned long long>(req_id)); return B200_ERR_NOT_FOUND; }
+  const bool lp = out_lp != nullptr;
+  if (lp && s->top_logprobs < 0) { set_error("request %llu was submitted without logprobs", static_cast<unsigned long long>(req_id)); return B200_ERR_INVALID; }
+  if (lp && (!out_top_ids || !out_top_lp)) { set_error("b200_poll_logprobs: bad arguments"); return B200_ERR_INVALID; }
   std::lock_guard<std::mutex> lk(s->m);
   int n = static_cast<int>(std::min<size_t>(s->out.size() - s->drained, cap > 0 && out_ids ? cap : 0));
   if (n > 0) memcpy(out_ids, s->out.data() + s->drained, static_cast<size_t>(n) * 4);
+  if (lp)
+    for (int k = 0; k < n; ++k) {
+      const LogprobRecord& r = s->lp_out[s->drained + k];
+      out_lp[k] = r.lp;
+      memcpy(out_top_ids + static_cast<size_t>(k) * kMaxLogprobs, r.top_ids, s->top_logprobs * sizeof(int32_t));
+      memcpy(out_top_lp + static_cast<size_t>(k) * kMaxLogprobs, r.top_lp, s->top_logprobs * sizeof(float));
+    }
   s->drained += n;
   *n_out = n;
   if (finished) *finished = (s->drained == s->out.size()) ? s->finished : 0;
@@ -1312,6 +1391,17 @@ int b200_poll(b200_engine* e, uint64_t req_id, int32_t* out_ids, int32_t cap, in
     usage->completion_tokens = static_cast<int>(s->out.size());
   }
   return 0;
+}
+
+int b200_poll(b200_engine* e, uint64_t req_id, int32_t* out_ids, int32_t cap, int32_t* n_out, int32_t* finished,
+              b200_usage* usage) {
+  return poll_impl(e, req_id, out_ids, nullptr, nullptr, nullptr, cap, n_out, finished, usage);
+}
+
+int b200_poll_logprobs(b200_engine* e, uint64_t req_id, int32_t* out_ids, float* out_logprob, int32_t* out_top_ids,
+                       float* out_top_logprob, int32_t cap, int32_t* n_out, int32_t* finished, b200_usage* usage) {
+  if (!out_logprob) { set_error("b200_poll_logprobs: bad arguments"); return B200_ERR_INVALID; }
+  return poll_impl(e, req_id, out_ids, out_logprob, out_top_ids, out_top_logprob, cap, n_out, finished, usage);
 }
 
 int b200_wait(b200_engine* e, uint64_t req_id, int64_t timeout_us) {

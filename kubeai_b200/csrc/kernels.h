@@ -40,6 +40,14 @@ struct SampleRow {
 // out[s] = the token sampled from bf16 logits row s ([S, ld], ld % 8 == 0) under rows[s] (device memory)
 int sample_rows(const void* logits, int ld, const SampleRow* rows, int S, int V, int* out, cudaStream_t st);
 
+// Log-probabilities (sampling.cu; vLLM's raw_logprobs) of n rows of bf16 logits ([., ld], ld % 8 == 0): row i is
+// r = rows ? rows[i] : i, its N = clamp(top_n[i], 0, min(V, kMaxLogprobs)).  lp[i * lp_ld] gets the log-probability of
+// tokens[r]; top_lp[i * top_lp_ld + j] and top_ids[i * kMaxLogprobs + j], j < N, the N most likely tokens (by logit,
+// lowest id on ties).  Entries past N are not written.  Every pointer is device memory.
+constexpr int kMaxLogprobs = 20;
+int logprobs_rows(const void* logits, int ld, int V, const int* rows, const int* top_n, int n, const int* tokens, float* lp,
+                  int lp_ld, float* top_lp, int top_lp_ld, int* top_ids, cudaStream_t st);
+
 // One unit of attention work: q_count query tokens of one sequence starting at row q_tok0 of the
 // step's token batch; the first of them sits at absolute position q_pos0 in the sequence.
 struct AttnWork {

@@ -320,7 +320,181 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const uint16_t* __rest
   if (threadIdx.x == 0) out[s] = bi == 0x7fffffff ? 0 : bi;
 }
 
+// Log-probabilities of one row per CTA, vLLM V1's raw_logprobs (vllm/v1/sample/sampler.py compute_logprobs /
+// gather_logprobs) made deterministic: lp_v = (l_v - m) - log(sum_u exp(l_u - m)) in fp32, m = the row max.  Each thread
+// sums its tokens in visit order, then a fixed shuffle tree adds the 1024 partials, so the sum (and every lp) is a pure
+// function of the row.  The top N are chosen by 16-bit key (exact bf16 order; -0 and +0 are one key), lowest id on ties:
+//   1 row max   2 sum of exp + high-byte count histogram   3 low-byte count histogram of the bin of the N-th key
+//   4 collect the keys above the N-th key and the ties at it, then rank the <= 20 + kTieCap entries.
+// When more than kTieCap tokens tie at the N-th key they are taken in id order by a chunked ballot scan instead (slow, rare
+// on real logits).  Rows with N = 0 stop after pass 2 and the sampled token's gather.
+constexpr int kTieCap = 64;
+constexpr int kCntSmem = 256 * 32 * 4;   // 32 per-lane copies of a 256-bin count histogram: 32 KiB
+
+__global__ void __launch_bounds__(kThreads) logprobs_kernel(const uint16_t* __restrict__ logits, int ld, int V,
+                                                            const int* __restrict__ rows, const int* __restrict__ top_n,
+                                                            const int* __restrict__ tokens, float* __restrict__ out_lp,
+                                                            int lp_ld, float* __restrict__ out_top_lp, int top_lp_ld,
+                                                            int* __restrict__ out_top_ids) {
+  __shared__ uint32_t cnt_hi[256], cnt_lo[256];
+  __shared__ float sred[32];
+  __shared__ int swc[32];
+  __shared__ uint32_t s_kmax, s_thr, s_count, s_above, s_need, s_ties;
+  __shared__ float s_logz;
+  __shared__ uint32_t ent_key[kMaxLogprobs + kTieCap];
+  __shared__ int ent_id[kMaxLogprobs + kTieCap];
+  extern __shared__ __align__(16) uint32_t priv_cnt[];   // kCntSmem
+  griddep_enter();
+  const int i = blockIdx.x;
+  const int r = rows ? rows[i] : i;
+  const uint16_t* row = logits + static_cast<size_t>(r) * ld;
+  const int N = min(max(top_n[i], 0), min(V, kMaxLogprobs));
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+
+  // pass 1: row max, as a key
+  uint32_t km = 0;
+  visit_row(row, V, [&](int, uint32_t b) { km = max(km, key_of(b)); });
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) km = max(km, __shfl_xor_sync(0xffffffffu, km, o));
+  if (threadIdx.x == 0) s_kmax = 0;
+  if (N > 0)
+    for (int j = threadIdx.x; j < 256 * 32; j += kThreads) priv_cnt[j] = 0;
+  __syncthreads();
+  if (lane == 0) atomicMax(&s_kmax, km);
+  __syncthreads();
+  const float m = bf16_bits_to_f32(bits_of_key(s_kmax));
+
+  // pass 2: sum of exp (fixed order) and the high-byte histogram (per-lane copies: no bank collisions within a warp)
+  float acc = 0.f;
+  visit_row(row, V, [&](int, uint32_t b) {
+    acc = __fadd_rn(acc, expf(__fsub_rn(bf16_bits_to_f32(b), m)));
+    if (N > 0) atomicAdd(&priv_cnt[(key_of(b) >> 8) * 32 + lane], 1u);
+  });
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc = __fadd_rn(acc, __shfl_xor_sync(0xffffffffu, acc, o));
+  if (lane == 0) sred[warp] = acc;
+  __syncthreads();
+  if (warp == 0) {
+    float t = sred[lane];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) t = __fadd_rn(t, __shfl_xor_sync(0xffffffffu, t, o));
+    if (lane == 0) s_logz = logf(t);
+  }
+  __syncthreads();
+  const float logz = s_logz;
+  // the same arithmetic for every token of one key, so equal logits (and -0 / +0) get the same bits
+  auto lp_of_key = [&](uint32_t k) { return __fsub_rn(__fsub_rn(bf16_bits_to_f32(bits_of_key(k)), m), logz); };
+  if (threadIdx.x == 0) {
+    const int t = tokens[r];
+    out_lp[static_cast<size_t>(i) * lp_ld] = (t >= 0 && t < V) ? lp_of_key(key_of(row[t])) : __int_as_float(0x7fc00000);
+  }
+  if (N == 0) return;
+
+  auto reduce_hist = [&](uint32_t* c) {
+    __syncthreads();
+    for (int j = warp; j < 256; j += kThreads / 32) {
+      uint32_t cs = priv_cnt[j * 32 + lane];
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) cs += __shfl_xor_sync(0xffffffffu, cs, o);
+      if (lane == 0) c[j] = cs;
+    }
+    __syncthreads();
+  };
+  const unsigned long long need_n = static_cast<unsigned long long>(N);
+  auto reach = [&](unsigned long long c) { return c >= need_n; };
+  reduce_hist(cnt_hi);
+  int bk = 0;
+  unsigned long long cab = 0;
+  if (warp == 0) bk = warp_last_bin(cnt_hi, 0ull, reach, &cab);   // N <= V: always found
+  if (threadIdx.x == 0) {
+    s_thr = static_cast<uint32_t>(bk);
+    s_above = static_cast<uint32_t>(cab);
+  }
+  for (int j = threadIdx.x; j < 256 * 32; j += kThreads) priv_cnt[j] = 0;
+  __syncthreads();
+  bk = static_cast<int>(s_thr);
+
+  // pass 3: low-byte histogram inside the bin of the N-th key
+  visit_row(row, V, [&](int, uint32_t b) {
+    const uint32_t k = key_of(b);
+    if (static_cast<int>(k >> 8) == bk) atomicAdd(&priv_cnt[(k & 0xFFu) * 32 + lane], 1u);
+  });
+  reduce_hist(cnt_lo);
+  if (warp == 0) {
+    unsigned long long above_lo = 0;
+    const int lo = warp_last_bin(cnt_lo, static_cast<unsigned long long>(s_above), reach, &above_lo);
+    if (lane == 0) {
+      s_thr = (static_cast<uint32_t>(bk) << 8) | static_cast<uint32_t>(lo);
+      s_above += static_cast<uint32_t>(above_lo);   // tokens with a key above the N-th key: < N
+      s_need = static_cast<uint32_t>(N) - s_above;   // ties at it to keep, >= 1
+      s_ties = cnt_lo[lo];
+      s_count = 0;
+    }
+  }
+  __syncthreads();
+  const uint32_t thr = s_thr;
+  const bool few_ties = s_ties <= static_cast<uint32_t>(kTieCap);
+
+  // pass 4: every key above the threshold (< 20 of them) and, when they are few, every tie at it
+  visit_row(row, V, [&](int v, uint32_t b) {
+    const uint32_t k = key_of(b);
+    if (k > thr || (few_ties && k == thr)) {
+      const uint32_t slot = atomicAdd(&s_count, 1u);
+      ent_key[slot] = k;
+      ent_id[slot] = v;
+    }
+  });
+  __syncthreads();
+  int count = static_cast<int>(s_count);
+  if (!few_ties) {
+    // the lowest-id ties, 1024 ids at a time in id order (CTA-uniform loop)
+    int slot = count, need = static_cast<int>(s_need);
+    for (int c = 0; c < V && need > 0; c += kThreads) {
+      const int v = c + static_cast<int>(threadIdx.x);
+      const bool tie = v < V && key_of(row[v]) == thr;
+      const unsigned bal = __ballot_sync(0xffffffffu, tie);
+      if (lane == 0) swc[warp] = __popc(bal);
+      __syncthreads();
+      int before = 0, total = 0;
+      for (int w = 0; w < kThreads / 32; ++w) {
+        before += w < warp ? swc[w] : 0;
+        total += swc[w];
+      }
+      const int pos = before + __popc(bal & ((1u << lane) - 1u));
+      if (tie && pos < need) {
+        ent_key[slot + pos] = thr;
+        ent_id[slot + pos] = v;
+      }
+      const int take = min(total, need);
+      slot += take;
+      need -= take;
+      __syncthreads();
+    }
+    count = slot;
+  }
+  // rank = entries before this one (higher key, or the same key and a lower id); the first N go out in rank order
+  if (static_cast<int>(threadIdx.x) < count) {
+    const uint32_t k = ent_key[threadIdx.x];
+    const int v = ent_id[threadIdx.x];
+    int rank = 0;
+    for (int q = 0; q < count; ++q) rank += (ent_key[q] > k || (ent_key[q] == k && ent_id[q] < v)) ? 1 : 0;
+    if (rank < N) {
+      out_top_ids[static_cast<size_t>(i) * kMaxLogprobs + rank] = v;
+      out_top_lp[static_cast<size_t>(i) * top_lp_ld + rank] = lp_of_key(k);
+    }
+  }
+}
+
 }  // namespace
+
+int logprobs_rows(const void* logits, int ld, int V, const int* rows, const int* top_n, int n, const int* tokens, float* lp,
+                  int lp_ld, float* top_lp, int top_lp_ld, int* top_ids, cudaStream_t st) {
+  if (n <= 0) return 0;
+  if (V < 1 || ld < V || ld % 8 || (reinterpret_cast<uintptr_t>(logits) & 15)) return -1;
+  launch_pdl(logprobs_kernel, dim3(n), dim3(kThreads), kCntSmem, st, static_cast<const uint16_t*>(logits), ld, V, rows, top_n,
+             tokens, lp, lp_ld, top_lp, top_lp_ld, top_ids);
+  return cudaGetLastError() == cudaSuccess ? 0 : -2;
+}
 
 int sample_rows(const void* logits, int ld, const SampleRow* rows, int S, int V, int* out, cudaStream_t st) {
   if (S <= 0) return 0;

@@ -18,6 +18,7 @@
 #include <time.h>
 #include <unistd.h>
 
+#include <algorithm>
 #include <atomic>
 #include <cmath>
 #include <map>
@@ -48,6 +49,7 @@ struct Server {
   Tokenizer tok;
   int max_model_len = 2048;
   bool sampling = false;   // b200_server_config.enable_sampling: serve temperature >= 1e-5 (else greedy only)
+  bool logprobs = false;   // b200_server_config.enable_logprobs: serve logprobs / top_logprobs (else a 400)
   // optional real tokenizer (b200_server_set_tokenizer): a checkpoint's tokenizer.json instead of the synthetic byte/word ids
   const b200_tokenizer* real_tok = nullptr;
 
@@ -163,6 +165,7 @@ struct ParsedRequest {
   int top_k = 0;
   bool has_seed = false;
   int64_t seed = 0;
+  int logprobs = -1;   // -1: none; else the number of most likely tokens per position (chat top_logprobs, completions logprobs)
   std::vector<int32_t> stop_ids;
 };
 
@@ -281,6 +284,34 @@ int parse_request(Server& sv, const std::string& path, const std::string& ctype,
     *err = std::string("bad request: ") + bad_sampling;
     return 400;
   }
+  if (sv.logprobs) {
+    // chat: "logprobs": bool, "top_logprobs": 0..20 (> 0 needs logprobs, vLLM chat_completion/protocol.py); completions:
+    // "logprobs": 0..20.  null is absent; anything else that is not an integer in range is refused.
+    const char* bad_lp = nullptr;
+    auto count = [&](const JVal* v, const char* msg) {
+      if (!v || v->type == JVal::Null) return -1;
+      if (v->type != JVal::Num || !(v->num >= 0 && v->num <= B200_MAX_LOGPROBS && v->num == std::floor(v->num))) {
+        bad_lp = msg;
+        return -1;
+      }
+      return static_cast<int>(v->num);
+    };
+    const JVal* lp = root.get("logprobs");
+    if (pr->chat) {
+      bool on = false;
+      if (lp && lp->type == JVal::Bool) on = lp->b;
+      else if (lp && lp->type != JVal::Null) bad_lp = "logprobs must be a boolean";
+      const int n = count(root.get("top_logprobs"), "top_logprobs must be an integer in 0..20");
+      if (!bad_lp && n > 0 && !on) bad_lp = "top_logprobs needs \"logprobs\": true";
+      if (on) pr->logprobs = n > 0 ? n : 0;
+    } else {
+      pr->logprobs = count(lp, "logprobs must be an integer in 0..20");
+    }
+    if (bad_lp) {
+      *err = std::string("bad request: ") + bad_lp;
+      return 400;
+    }
+  }
   if (const JVal* v = root.get("stop_token_ids"); v && v->type == JVal::Arr)
     for (auto& e : v->arr)
       if (e.type == JVal::Num) pr->stop_ids.push_back(static_cast<int32_t>(e.num));
@@ -299,7 +330,9 @@ int parse_request(Server& sv, const std::string& path, const std::string& ctype,
   const char* bad = nullptr;
   if (num_of("n", 1) > 1) bad = "n > 1";
   else if (num_of("best_of", 1) > 1) bad = "best_of > 1";
-  else if (truthy("logprobs") || truthy("top_logprobs") || truthy("prompt_logprobs")) bad = "logprobs";
+  else if (!sv.logprobs && (truthy("logprobs") || truthy("top_logprobs") || truthy("prompt_logprobs"))) bad = "logprobs";
+  else if (truthy("prompt_logprobs")) bad = "prompt_logprobs";
+  else if (!pr->chat && truthy("top_logprobs")) bad = "top_logprobs on completions (use logprobs)";
   else if (nonempty("stop")) bad = "stop strings (use stop_token_ids)";
   else if (truthy("echo")) bad = "echo";
   else if (nonempty("suffix")) bad = "suffix";
@@ -328,6 +361,84 @@ std::string usage_json(const b200_usage& u) {
 }
 
 const char* finish_str(int code) { return code == B200_FINISH_STOP ? "stop" : code == B200_FINISH_LENGTH ? "length" : "abort"; }
+
+// ---- logprobs in vLLM 0.22's OpenAI format (vllm/v1/engine/logprobs.py, chat_completion/serving.py _create_chat_logprobs,
+// completion/serving.py _create_completion_logprobs)
+struct LpRecord {
+  int32_t id;
+  float lp;
+  std::vector<std::pair<int32_t, float>> top;   // the request's N most likely tokens
+};
+
+// the shortest decimal that reads back as the same fp32, after vLLM's clamp at -9999.0
+std::string lp_num(float v) {
+  v = std::max(v, -9999.0f);
+  char b[32];
+  for (int p = 6; p <= 9; ++p) {
+    snprintf(b, sizeof(b), "%.*g", p, static_cast<double>(v));
+    if (strtof(b, nullptr) == v) break;
+  }
+  return b;
+}
+
+// code points in valid UTF-8 (Python's len of the str)
+size_t utf8_len(const std::string& s) {
+  size_t n = 0;
+  for (unsigned char c : s) n += (c & 0xC0) != 0x80;
+  return n;
+}
+
+// vLLM's entries of one position: the sampled token first, then the top N without it
+std::vector<std::pair<int32_t, float>> lp_entries(const LpRecord& r) {
+  std::vector<std::pair<int32_t, float>> e{{r.id, r.lp}};
+  for (auto& t : r.top)
+    if (t.first != r.id) e.push_back(t);
+  return e;
+}
+
+std::string chat_lp_item(const std::string& tok, float lp, bool with_top) {
+  std::string o = "{\"token\":" + json_str(tok) + ",\"logprob\":" + lp_num(lp) + ",\"bytes\":[";
+  for (size_t i = 0; i < tok.size(); ++i) o += (i ? "," : "") + std::to_string(static_cast<unsigned char>(tok[i]));
+  o += "]";
+  if (!with_top) o += "}";
+  return o;
+}
+
+// one element of chat "logprobs.content": the token, then the first N entries
+template <class Str>
+std::string chat_lp_content(const LpRecord& r, const Str& token_str) {
+  const auto e = lp_entries(r);
+  std::string o = chat_lp_item(token_str(r.id), r.lp, true) + ",\"top_logprobs\":[";
+  for (size_t j = 0; j < r.top.size() && j < e.size(); ++j) o += (j ? "," : "") + chat_lp_item(token_str(e[j].first), e[j].second, false);
+  return o + "]}";
+}
+
+// completions "logprobs" of consecutive tokens, text_offset counted from `offset`: the first N + 1 entries of each position
+// as a {token string: logprob} object (a string that repeats keeps its first place and takes the later value, as a dict)
+template <class Str>
+std::string completion_lp(const std::vector<LpRecord>& rs, size_t offset, const Str& token_str) {
+  std::string off = "[", lps = "[", toks = "[", tops = "[";
+  for (size_t k = 0; k < rs.size(); ++k) {
+    const std::string s = token_str(rs[k].id);
+    const char* sep = k ? "," : "";
+    off += sep + std::to_string(offset);
+    offset += utf8_len(s);
+    lps += sep + lp_num(rs[k].lp);
+    toks += sep + json_str(s);
+    const auto e = lp_entries(rs[k]);
+    std::vector<std::pair<std::string, float>> d;
+    for (size_t j = 0; j <= rs[k].top.size() && j < e.size(); ++j) {
+      std::string key = token_str(e[j].first);
+      auto it = std::find_if(d.begin(), d.end(), [&](const std::pair<std::string, float>& x) { return x.first == key; });
+      if (it != d.end()) it->second = e[j].second;
+      else d.emplace_back(std::move(key), e[j].second);
+    }
+    tops += sep + std::string("{");
+    for (size_t j = 0; j < d.size(); ++j) tops += (j ? "," : "") + json_str(d[j].first) + ":" + lp_num(d[j].second);
+    tops += "}";
+  }
+  return "{\"text_offset\":" + off + "],\"token_logprobs\":" + lps + "],\"tokens\":" + toks + "],\"top_logprobs\":" + tops + "]}";
+}
 
 }  // namespace
 
@@ -435,6 +546,8 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
     sp.has_seed = pr.has_seed ? 1 : 0;
     sp.seed = static_cast<uint64_t>(pr.seed);
     sp.ignore_eos = pr.ignore_eos ? 1 : 0;
+    sp.logprobs = pr.logprobs >= 0 ? 1 : 0;
+    sp.top_logprobs = std::max(pr.logprobs, 0);
     std::vector<int32_t> stops = pr.stop_ids;
     if (sv.real_tok && !pr.ignore_eos) {   // the checkpoint's end-of-turn / end-of-text tokens end the generation
       for (const char* name : {"<|eot_id|>", "<|end_of_text|>"}) {
@@ -451,6 +564,11 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
     if (!failed && b200_submit(eng, ids.data(), static_cast<int>(ids.size()), &sp, &rid)) failed = true;
 
     std::vector<int32_t> all;
+    std::vector<LpRecord> all_lp;
+    const bool want_lp = pr.logprobs >= 0;
+    // a token's string in logprobs: the single-id lossy decode (vLLM's tokenizer.decode([id])), or the synthetic piece
+    auto token_str = [&](int32_t id) { return sv.real_tok ? tokenizer_token_text(sv.real_tok, id) : sv.tok.piece(id); };
+    size_t text_off = 0;   // completions stream: text_offset runs across chunks
     DetokStream detok;
     detok.tok = sv.real_tok;
     int fin = 0;
@@ -458,11 +576,27 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
     bool sent_any = false;
     if (!failed) {
       int32_t buf[256];
+      std::vector<float> lpv, top_lp;
+      std::vector<int32_t> top_ids;
+      if (want_lp) {
+        lpv.resize(256);
+        top_lp.resize(256 * B200_MAX_LOGPROBS);
+        top_ids.resize(256 * B200_MAX_LOGPROBS);
+      }
       while (!fin) {
         b200_wait(eng, rid, 200000);
         int n = 0;
-        if (b200_poll(eng, rid, buf, 256, &n, &fin, &usage)) { failed = true; break; }
+        const int prc = want_lp ? b200_poll_logprobs(eng, rid, buf, lpv.data(), top_ids.data(), top_lp.data(), 256, &n, &fin, &usage)
+                                : b200_poll(eng, rid, buf, 256, &n, &fin, &usage);
+        if (prc) { failed = true; break; }
         if (fin == B200_FINISH_ERROR && !sent_any) { failed = true; break; }
+        std::vector<LpRecord> recs;
+        for (int i = 0; want_lp && i < n; ++i) {
+          LpRecord r{buf[i], lpv[i], {}};
+          for (int j = 0; j < pr.logprobs; ++j)
+            r.top.emplace_back(top_ids[static_cast<size_t>(i) * B200_MAX_LOGPROBS + j], top_lp[static_cast<size_t>(i) * B200_MAX_LOGPROBS + j]);
+          recs.push_back(std::move(r));
+        }
         if (pr.stream && n > 0) {
           if (!sent_any) {
             w.begin(200, "text/event-stream; charset=utf-8");
@@ -475,15 +609,21 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
             const std::string fr = last ? std::string("\"") + finish_str(fin) + "\"" : "null";
             // one chunk per token; with a real tokenizer a chunk carries the text that token completed (possibly none: a
             // token may end inside a UTF-8 sequence), and the last chunk also what was still held
-            const std::string piece = json_str(sv.real_tok ? detok.push(buf[i]) + (last ? detok.flush() : std::string()) : sv.tok.piece(buf[i]));
+            const std::string text = sv.real_tok ? detok.push(buf[i]) + (last ? detok.flush() : std::string()) : sv.tok.piece(buf[i]);
+            const std::string piece = json_str(text);
+            std::string lpj = "null";
+            if (want_lp && pr.chat) lpj = "{\"content\":[" + chat_lp_content(recs[i], token_str) + "]}";
+            else if (want_lp) lpj = completion_lp({recs[i]}, text_off, token_str);
+            text_off += utf8_len(text);
             if (pr.chat)
-              w.write("data: " + head + ",\"choices\":[{\"index\":0,\"delta\":{\"content\":" + piece + "},\"logprobs\":null,\"finish_reason\":" + fr +
+              w.write("data: " + head + ",\"choices\":[{\"index\":0,\"delta\":{\"content\":" + piece + "},\"logprobs\":" + lpj + ",\"finish_reason\":" + fr +
                       (last ? ",\"stop_reason\":null" : "") + "}]}\n\n");
             else
-              w.write("data: " + head + ",\"choices\":[{\"index\":0,\"text\":" + piece + ",\"logprobs\":null,\"finish_reason\":" + fr + ",\"stop_reason\":null}],\"usage\":null}\n\n");
+              w.write("data: " + head + ",\"choices\":[{\"index\":0,\"text\":" + piece + ",\"logprobs\":" + lpj + ",\"finish_reason\":" + fr + ",\"stop_reason\":null}],\"usage\":null}\n\n");
           }
         }
         all.insert(all.end(), buf, buf + n);
+        all_lp.insert(all_lp.end(), recs.begin(), recs.end());
         if (w.gone) {  // client disconnected: abort the sequence and free its KV blocks
           b200_abort(eng, rid);
           break;
@@ -521,7 +661,15 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
                         "\",\"created\":" + std::to_string(created) + ",\"model\":" + json_str(pr.requested_model) + ",\"choices\":[{\"index\":0,";
       if (pr.chat) out += "\"message\":{\"role\":\"assistant\",\"content\":" + json_str(text) + "},";
       else out += "\"text\":" + json_str(text) + ",";
-      out += std::string("\"logprobs\":null,\"finish_reason\":\"") + finish_str(fin) + "\",\"stop_reason\":null}],\"usage\":" + usage_json(usage) + "}";
+      std::string lpj = "null";
+      if (want_lp && pr.chat) {
+        lpj = "{\"content\":[";
+        for (size_t k = 0; k < all_lp.size(); ++k) lpj += (k ? "," : "") + chat_lp_content(all_lp[k], token_str);
+        lpj += "]}";
+      } else if (want_lp) {
+        lpj = completion_lp(all_lp, 0, token_str);
+      }
+      out += "\"logprobs\":" + lpj + ",\"finish_reason\":\"" + finish_str(fin) + "\",\"stop_reason\":null}],\"usage\":" + usage_json(usage) + "}";
       w.begin(200, "application/json");
       w.write(out);
     }
@@ -758,6 +906,7 @@ int b200_server_create(const b200_server_config* cfg, b200_engine* const* replic
   sv.tok.vocab = cfg->vocab > 258 ? cfg->vocab : 128256;
   sv.max_model_len = cfg->max_model_len > 0 ? cfg->max_model_len : 2048;
   sv.sampling = cfg->enable_sampling != 0;
+  sv.logprobs = cfg->enable_logprobs != 0;
   if (b200_router_create(sv.replication, &sv.router)) { delete s; return B200_ERR_INVALID; }
   std::vector<std::string> names;
   std::string ad = cfg->adapters ? cfg->adapters : "";

@@ -319,6 +319,12 @@ size_t incomplete_tail(const std::string& b) {
 }
 }  // namespace
 
+std::string tokenizer_token_text(const b200_tokenizer* t, int32_t id) {
+  std::string b;
+  tokenizer_token_bytes(t, id, false, &b);
+  return sanitize_utf8(b.data(), b.size());
+}
+
 std::string DetokStream::push(int32_t id) {
   tokenizer_token_bytes(tok, id, skip_special, &pending);
   const size_t hold = incomplete_tail(pending);

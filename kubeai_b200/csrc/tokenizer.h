@@ -14,6 +14,8 @@ void tokenizer_token_bytes(const b200_tokenizer* t, int32_t id, bool skip_specia
 // ids of the Llama-3 control tokens (-1 if the vocabulary lacks one)
 int32_t tokenizer_bos(const b200_tokenizer* t);
 int32_t tokenizer_eot(const b200_tokenizer* t);
+// one id decoded on its own, special tokens kept, invalid UTF-8 replaced by U+FFFD (HF tokenizer.decode([id]))
+std::string tokenizer_token_text(const b200_tokenizer* t, int32_t id);
 
 // A token may end in the middle of a UTF-8 sequence (byte-level BPE): push() returns only text that is complete, holding an
 // unfinished tail until the next token completes it; bytes that can never become valid are replaced by U+FFFD, as a lossy

@@ -10,6 +10,8 @@ import numpy as np
 from ._lib import Config, Sampling, Stats, StepInfo, Usage, check, lib
 
 FINISH = {0: None, 1: "stop", 2: "length", 3: "aborted", 4: "error"}
+MAX_LOGPROBS = 20   # B200_MAX_LOGPROBS
+_PI32 = C.POINTER(C.c_int32)
 
 
 def default_config(**kw) -> Config:
@@ -53,6 +55,13 @@ class PollResult:
     usage: tuple
 
 
+@dataclass
+class LogprobsPollResult(PollResult):
+    lp: np.ndarray        # float32 [n]: each token's own log-probability
+    top_ids: np.ndarray   # int32 [n, N]
+    top_lp: np.ndarray    # float32 [n, N]
+
+
 class Engine:
     def __init__(self, cfg: Config):
         self._l = lib()
@@ -78,15 +87,18 @@ class Engine:
             pass
 
     def submit(self, prompt_ids, max_tokens=16, ignore_eos=True, stop_ids=(), temperature=0.0, top_p=1.0, top_k=0,
-               seed=None) -> int:
-        """temperature < 1e-5 is greedy; top_k 0 / -1 and top_p 1 are off; seed None = one drawn by the engine."""
+               seed=None, logprobs=False, top_logprobs=0) -> int:
+        """temperature < 1e-5 is greedy; top_k 0 / -1 and top_p 1 are off; seed None = one drawn by the engine.
+        logprobs: keep each generated token's log-probability and its top_logprobs (0..20) most likely tokens, read with
+        poll_logprobs."""
         ids = np.ascontiguousarray(prompt_ids, dtype=np.int32)
         stops = np.ascontiguousarray(stop_ids, dtype=np.int32)
         sp = Sampling(max_tokens=max_tokens, temperature=temperature, ignore_eos=1 if ignore_eos else 0,
                       num_stop_ids=len(stops),
                       stop_ids=stops.ctypes.data_as(C.POINTER(C.c_int32)) if len(stops) else None,
                       top_p=top_p, top_k=top_k, has_seed=0 if seed is None else 1,
-                      seed=0 if seed is None else seed & 0xFFFFFFFFFFFFFFFF)
+                      seed=0 if seed is None else seed & 0xFFFFFFFFFFFFFFFF,
+                      logprobs=1 if logprobs else 0, top_logprobs=top_logprobs)
         rid = C.c_uint64()
         check(self._l.b200_submit(self._h, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), C.byref(sp),
                                   C.byref(rid)))
@@ -98,6 +110,21 @@ class Engine:
         check(self._l.b200_poll(self._h, rid, buf, cap, C.byref(n), C.byref(fin), C.byref(u)))
         return PollResult(list(buf[: n.value]), FINISH[fin.value],
                           (u.prompt_tokens, u.cached_tokens, u.completion_tokens))
+
+    def poll_logprobs(self, rid: int, top_logprobs: int, cap: int = 4096) -> LogprobsPollResult:
+        """poll() with the records of the drained tokens: lp float32 [n], top_ids int32 [n, top_logprobs] and
+        top_lp float32 [n, top_logprobs] (top_logprobs = the request's)."""
+        ids = (C.c_int32 * cap)()
+        lp = np.zeros(cap, dtype=np.float32)
+        tid = np.zeros((cap, MAX_LOGPROBS), dtype=np.int32)
+        tlp = np.zeros((cap, MAX_LOGPROBS), dtype=np.float32)
+        n, fin, u = C.c_int32(), C.c_int32(), Usage()
+        check(self._l.b200_poll_logprobs(self._h, rid, ids, lp.ctypes.data_as(C.c_void_p), tid.ctypes.data_as(_PI32),
+                                         tlp.ctypes.data_as(C.c_void_p), cap, C.byref(n), C.byref(fin), C.byref(u)))
+        k = n.value
+        return LogprobsPollResult(list(ids[:k]), FINISH[fin.value],
+                                  (u.prompt_tokens, u.cached_tokens, u.completion_tokens), lp[:k].copy(),
+                                  tid[:k, :top_logprobs].copy(), tlp[:k, :top_logprobs].copy())
 
     def wait(self, rid: int, timeout_s: float = -1.0) -> bool:
         rc = self._l.b200_wait(self._h, rid, int(timeout_s * 1e6) if timeout_s >= 0 else -1)

@@ -148,6 +148,23 @@ def sample(logits, temperature, top_k=0, top_p=1.0, seed=0, n=0):
     return out
 
 
+def logprobs(logits, tokens, top_n):
+    """Log-probabilities of bf16 logits [S, V] (b200_op_logprobs): returns (lp float32 [S] of tokens[s], top_ids int32
+    [S, 20], top_lp float32 [S, 20]); row s's first top_n[s] entries (scalar or per row, 0..20) are its most likely tokens,
+    the rest stay zero."""
+    _chk(logits)
+    S, V = logits.shape
+    dev = logits.device
+    tok = torch.as_tensor(np.broadcast_to(np.asarray(tokens, dtype=np.int32), (S,)).copy()).to(dev)
+    n = torch.as_tensor(np.broadcast_to(np.asarray(top_n, dtype=np.int32), (S,)).copy()).to(dev)
+    lp = torch.zeros(S, dtype=torch.float32, device=dev)
+    top_ids = torch.zeros(S, 20, dtype=torch.int32, device=dev)
+    top_lp = torch.zeros(S, 20, dtype=torch.float32, device=dev)
+    check(lib().b200_op_logprobs(_p(logits), logits.stride(0), S, V, _p(tok), _p(n), _p(lp), _p(top_ids), _p(top_lp),
+                                 _stream()))
+    return lp, top_ids, top_lp
+
+
 def paged_attn(qkv, kv_layer, block_tables, work, q_heads, kv_heads, decode: bool, out=None, split: int = 0):
     """qkv: [T, (Hq+2Hkv)*128] (q read from it), work: int32 [n, 4] = (q_tok0, q_count, q_pos0, seq).
     split >= 1 (decode only): split-KV form with that many CTAs per (work item, KV head)."""
