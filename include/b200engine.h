@@ -83,9 +83,24 @@ typedef struct {
    * temperature / top-k / top-p; the sampled tokens do not change), read with b200_poll_logprobs. */
   int32_t logprobs;           /* 0 = off */
   int32_t top_logprobs;       /* 0..B200_MAX_LOGPROBS most likely tokens per position; > 0 needs logprobs */
+  /* Logits edits (vLLM's logits processors and penalties, csrc/penalties.cu), applied in fp32 to the raw bf16 row in this
+   * order and rounded back to bf16 before the token is chosen; logprobs still read the raw row:
+   *   logit_bias: l += bias (clamped to [-100, 100]);  min_tokens: the stop ids and EOS (even with ignore_eos, as vLLM's
+   *   all_stop_token_ids) are -inf while fewer than min_tokens tokens exist;  repetition_penalty r for tokens in the prompt
+   *   or the output: l *= (l > 0 ? 1/r : r);  l -= frequency_penalty * count;  l -= presence_penalty * (count > 0).
+   * min_p (sampled rows only) keeps the tokens with p >= min_p * p_max, after temperature and before top-k / top-p. */
+  float presence_penalty;     /* [-2, 2] */
+  float frequency_penalty;    /* [-2, 2] */
+  float repetition_penalty;   /* >= 0; 0 = off (read as 1) */
+  float min_p;                /* [0, 1] */
+  int32_t min_tokens;         /* 0..max_tokens */
+  int32_t num_logit_bias;     /* 0..B200_MAX_LOGIT_BIAS; ids in [0, vocab), finite values; a repeated id keeps its last */
+  const int32_t* logit_bias_ids;
+  const float* logit_bias_values;
 } b200_sampling;
 
-#define B200_MAX_LOGPROBS 20  /* vLLM's default max_logprobs */
+#define B200_MAX_LOGPROBS 20     /* vLLM's default max_logprobs */
+#define B200_MAX_LOGIT_BIAS 1024 /* logit_bias entries per request; also the stop ids of a request with min_tokens */
 
 typedef struct {
   int32_t prompt_tokens;
@@ -186,7 +201,7 @@ int b200_engine_forward_logits(b200_engine* e, const int32_t* ids, int32_t n, vo
 /* Parity hook for decode steps (manual_step mode): with keep != 0 the lm_head of every later step leaves the complete
  * bf16 logits of its sampled rows in HBM (the serving path only keeps what the argmax needs); read_logits copies the
  * first `rows` rows [rows, vocab] of the last step, in the order the step sampled them (scheduling order).  For a step
- * with a row at temperature >= 1e-5 these are the exact rows the sampler read. */
+ * with a row at temperature >= 1e-5 these are the raw rows, before the sparse edits. */
 int b200_engine_set_keep_logits(b200_engine* e, int32_t keep);
 int b200_engine_read_logits(b200_engine* e, void* host_logits_bf16, int32_t rows);
 
@@ -258,6 +273,9 @@ typedef struct {
   /* 1: serve logprobs (chat: "logprobs": true + "top_logprobs" 0..20; completions: "logprobs" 0..20) in vLLM's response
    * format; 0: they get a 400, as before logprobs existed (a zero-initialised config keeps that) */
   int32_t enable_logprobs;
+  /* 1: serve presence_penalty, frequency_penalty, repetition_penalty, min_p, min_tokens and logit_bias (see b200_sampling);
+   * 0: they get a 400, as before logits edits existed (a zero-initialised config keeps that) */
+  int32_t enable_logits_processors;
 } b200_server_config;
 int b200_server_create(const b200_server_config* cfg, b200_engine* const* replicas, int32_t n, b200_server** out);
 void b200_server_destroy(b200_server* s);
@@ -416,6 +434,7 @@ typedef struct {
   float top_p;
   uint32_t seed_lo, seed_hi;
   int32_t n;
+  float min_p;                /* 0 = off: keep the tokens with p >= min_p * p_max (a fixed predicate on z_v - z_max) */
 } b200_sample_row;
 /* out[s] = the token sampled from bf16 logits row s ([S, ld], ld % 8 == 0, V <= ld) under rows[s]; rows and out are device
  * memory.  Greedy rows give the same token as b200_op_argmax. */
@@ -426,6 +445,25 @@ int b200_op_sample(const void* logits, int32_t ld, const b200_sample_row* rows, 
  * pointer is device memory. */
 int b200_op_logprobs(const void* logits, int32_t ld, int32_t S, int32_t V, const int32_t* tokens, const int32_t* top_n,
                      float* out_logprob, int32_t* out_top_ids, float* out_top_logprob, void* stream);
+/* The logits edits of b200_sampling on explicit inputs, with the engine's device code: rows[s] (host memory) edits bf16
+ * logits row s ([S, ld], device, in place) as a request with those parameters, prompt and output tokens would see it when
+ * generating its num_output-th token (min_tokens counts the output; stop_ids are its stops, EOS included by the caller).
+ * edited (device [S, ld], optional): gets the edited rows, and `logits` is restored to its raw values, as the engine does
+ * after the token selection. */
+typedef struct {
+  float presence_penalty, frequency_penalty, repetition_penalty;   /* repetition 0 = off */
+  int32_t min_tokens;
+  int32_t num_prompt;
+  const int32_t* prompt;
+  int32_t num_output;
+  const int32_t* output;
+  int32_t num_logit_bias;
+  const int32_t* logit_bias_ids;
+  const float* logit_bias_values;
+  int32_t num_stop_ids;
+  const int32_t* stop_ids;
+} b200_penalty_row;
+int b200_op_penalize(void* logits, int32_t ld, int32_t S, int32_t V, const b200_penalty_row* rows, void* edited, void* stream);
 /* work: int32[num_work][4] = {q_tok0, q_count, q_pos0, seq}; kv_layer: [block][2][kv_heads][16][128] */
 int b200_op_paged_attn(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                        const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,

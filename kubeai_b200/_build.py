@@ -23,6 +23,7 @@ SOURCES = [
     "attention_wgmma.cu",
     "elementwise.cu",
     "sampling.cu",
+    "penalties.cu",
     "abi_ops.cu",
     "engine.cu",
     "router.cc",

@@ -45,12 +45,23 @@ class Sampling(C.Structure):
     _fields_ = [("max_tokens", C.c_int32), ("temperature", C.c_float), ("ignore_eos", C.c_int32),
                 ("num_stop_ids", C.c_int32), ("stop_ids", C.POINTER(C.c_int32)),
                 ("top_p", C.c_float), ("top_k", C.c_int32), ("has_seed", C.c_int32), ("seed", C.c_uint64),
-                ("logprobs", C.c_int32), ("top_logprobs", C.c_int32)]
+                ("logprobs", C.c_int32), ("top_logprobs", C.c_int32),
+                ("presence_penalty", C.c_float), ("frequency_penalty", C.c_float), ("repetition_penalty", C.c_float),
+                ("min_p", C.c_float), ("min_tokens", C.c_int32), ("num_logit_bias", C.c_int32),
+                ("logit_bias_ids", C.POINTER(C.c_int32)), ("logit_bias_values", C.POINTER(C.c_float))]
 
 
 class SampleRow(C.Structure):
     _fields_ = [("temperature", C.c_float), ("top_k", C.c_int32), ("top_p", C.c_float),
-                ("seed_lo", C.c_uint32), ("seed_hi", C.c_uint32), ("n", C.c_int32)]
+                ("seed_lo", C.c_uint32), ("seed_hi", C.c_uint32), ("n", C.c_int32), ("min_p", C.c_float)]
+
+
+class PenaltyRow(C.Structure):
+    _fields_ = [("presence_penalty", C.c_float), ("frequency_penalty", C.c_float), ("repetition_penalty", C.c_float),
+                ("min_tokens", C.c_int32), ("num_prompt", C.c_int32), ("prompt", C.POINTER(C.c_int32)),
+                ("num_output", C.c_int32), ("output", C.POINTER(C.c_int32)), ("num_logit_bias", C.c_int32),
+                ("logit_bias_ids", C.POINTER(C.c_int32)), ("logit_bias_values", C.POINTER(C.c_float)),
+                ("num_stop_ids", C.c_int32), ("stop_ids", C.POINTER(C.c_int32))]
 
 
 class Usage(C.Structure):
@@ -83,7 +94,8 @@ class ServerConfig(C.Structure):
     _fields_ = [("model", C.c_char_p), ("adapters", C.c_char_p), ("strategy", C.c_int32),
                 ("mean_load_pct", C.c_int32), ("replication", C.c_int32), ("prefix_char_length", C.c_int32),
                 ("max_retries", C.c_int32), ("default_max_tokens", C.c_int32), ("vocab", C.c_int32),
-                ("max_model_len", C.c_int32), ("enable_sampling", C.c_int32), ("enable_logprobs", C.c_int32)]
+                ("max_model_len", C.c_int32), ("enable_sampling", C.c_int32), ("enable_logprobs", C.c_int32),
+                ("enable_logits_processors", C.c_int32)]
 
 
 class HarnessConfig(C.Structure):
@@ -186,6 +198,7 @@ SYMBOLS = {
     "b200_op_silu_mul": (C.c_int, [_vp, _vp, _i32, _i32, _vp]),
     "b200_op_argmax": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _vp]),
     "b200_op_sample": (C.c_int, [_vp, _i32, _vp, _i32, _i32, _vp, _vp]),
+    "b200_op_penalize": (C.c_int, [_vp, _i32, _i32, _i32, C.POINTER(PenaltyRow), _vp, _vp]),
     "b200_op_logprobs": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "b200_op_paged_attn": (C.c_int, [_vp, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _f, _i32, _vp]),
     "b200_server_set_tokenizer": (C.c_int, [C.c_void_p, C.c_void_p]),

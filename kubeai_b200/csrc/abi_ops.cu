@@ -245,8 +245,70 @@ int b200_op_sample(const void* logits, int32_t ld, const b200_sample_row* rows, 
     set_error("b200_op_sample: bad arguments (S=%d V=%d ld=%d; ld %% 8 == 0 and V <= ld required)", S, V, ld);
     return B200_ERR_INVALID;
   }
-  int rc = sample_rows(logits, ld, reinterpret_cast<const SampleRow*>(rows), S, V, out, static_cast<cudaStream_t>(stream));
+  int rc = sample_rows(logits, ld, rows, 7, S, V, out, static_cast<cudaStream_t>(stream));
   return rc ? cuda_fail("sample_rows", rc) : 0;
+}
+
+int b200_op_penalize(void* logits, int32_t ld, int32_t S, int32_t V, const b200_penalty_row* rows, void* edited, void* stream) {
+  if (int rc = require_device()) return rc;
+  if (!logits || (S > 0 && !rows) || S < 0 || V < 1 || ld < V) {
+    set_error("b200_op_penalize: bad arguments (S=%d V=%d ld=%d)", S, V, ld);
+    return B200_ERR_INVALID;
+  }
+  if (S == 0) return 0;
+  // the engine's lists, one slot per row, built by the engine's host code
+  std::vector<std::vector<PenaltyRec>> lists(S);
+  std::vector<PenaltyRow> prow(S);
+  int cap = 1;
+  for (int s = 0; s < S; ++s) {
+    const b200_penalty_row& r = rows[s];
+    auto ids_ok = [&](const int32_t* p, int n) {
+      if (n < 0 || (n > 0 && !p)) return false;
+      for (int i = 0; i < n; ++i) if (p[i] < 0 || p[i] >= V) return false;
+      return true;
+    };
+    if (!ids_ok(r.prompt, r.num_prompt) || !ids_ok(r.output, r.num_output) || !ids_ok(r.logit_bias_ids, r.num_logit_bias) ||
+        !ids_ok(r.stop_ids, r.num_stop_ids) || (r.num_logit_bias > 0 && !r.logit_bias_values) || !(r.repetition_penalty >= 0.f)) {
+      set_error("b200_op_penalize: row %d has a token id outside [0, %d) or a bad list", s, V);
+      return B200_ERR_INVALID;
+    }
+    const float rp = r.repetition_penalty > 0.f ? r.repetition_penalty : 1.f;
+    prow[s] = PenaltyRow{s, s, r.presence_penalty, r.frequency_penalty, rp, r.num_output, r.min_tokens, 0};
+    const bool history = r.presence_penalty != 0.f || r.frequency_penalty != 0.f || rp != 1.f;
+    penalty_records(r.prompt, r.num_prompt, r.output, r.num_output, history, r.logit_bias_ids, r.logit_bias_values,
+                    r.num_logit_bias, r.stop_ids, r.num_output < r.min_tokens ? r.num_stop_ids : 0, &lists[s]);
+    cap = std::max(cap, static_cast<int>(lists[s].size()));
+  }
+  std::vector<PenaltyRec> recs(static_cast<size_t>(S) * cap);
+  std::vector<int> lens(S);
+  for (int s = 0; s < S; ++s) {
+    std::copy(lists[s].begin(), lists[s].end(), recs.begin() + static_cast<size_t>(s) * cap);
+    lens[s] = static_cast<int>(lists[s].size());
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  PenaltyRec* d_recs = nullptr;
+  PenaltyRow* d_rows = nullptr;
+  int* d_lens = nullptr;
+  uint16_t* d_save = nullptr;
+  cudaError_t ce = cudaMalloc(&d_recs, recs.size() * sizeof(PenaltyRec));
+  if (ce == cudaSuccess) ce = cudaMalloc(&d_rows, prow.size() * sizeof(PenaltyRow));
+  if (ce == cudaSuccess) ce = cudaMalloc(&d_lens, lens.size() * sizeof(int));
+  if (ce == cudaSuccess) ce = cudaMalloc(&d_save, static_cast<size_t>(S) * cap * sizeof(uint16_t));
+  if (ce == cudaSuccess) ce = cudaMemcpyAsync(d_recs, recs.data(), recs.size() * sizeof(PenaltyRec), cudaMemcpyHostToDevice, st);
+  if (ce == cudaSuccess) ce = cudaMemcpyAsync(d_rows, prow.data(), prow.size() * sizeof(PenaltyRow), cudaMemcpyHostToDevice, st);
+  if (ce == cudaSuccess) ce = cudaMemcpyAsync(d_lens, lens.data(), lens.size() * sizeof(int), cudaMemcpyHostToDevice, st);
+  int rc = ce == cudaSuccess ? 0 : -2;
+  if (!rc) rc = penalize_rows(logits, ld, d_rows, S, d_recs, d_lens, cap, d_save, st);
+  if (!rc && edited) {
+    ce = cudaMemcpyAsync(edited, logits, static_cast<size_t>(S) * ld * 2, cudaMemcpyDeviceToDevice, st);
+    rc = ce == cudaSuccess ? penalize_restore(logits, ld, d_rows, S, d_recs, d_lens, cap, d_save, st) : -2;
+  }
+  if (cudaStreamSynchronize(st) != cudaSuccess) rc = -2;   // before the host lists and the scratch go away
+  cudaFree(d_recs);
+  cudaFree(d_rows);
+  cudaFree(d_lens);
+  cudaFree(d_save);
+  return rc ? cuda_fail("penalize_rows", rc) : 0;
 }
 
 int b200_op_logprobs(const void* logits, int32_t ld, int32_t S, int32_t V, const int32_t* tokens, const int32_t* top_n,

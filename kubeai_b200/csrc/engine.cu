@@ -186,6 +186,14 @@ struct Seq {
   int top_k = 0;
   uint64_t seed = 0;
   int top_logprobs = -1;   // -1: no logprobs; else the N of every generated token's record
+  // logits edits (penalties.cu): off when every field is at its default; pen_slot = the device record list while admitted
+  float min_p = 0.f, presence = 0.f, frequency = 0.f, repetition = 1.f;
+  int min_tokens = 0;
+  std::vector<int32_t> bias_ids;
+  std::vector<float> bias_values;
+  int pen_slot = -1;
+  bool pen_history() const { return presence != 0.f || frequency != 0.f || repetition != 1.f; }
+  bool edits() const { return pen_history() || min_tokens > 0 || !bias_ids.empty(); }
   int n_generated = 0;
   std::atomic<int> n_cached{-1};  // prefix-hit tokens at first admission
   bool admitted = false;
@@ -224,6 +232,10 @@ struct StepMeta {
   int T = 0, nd = 0, np = 0, S = 0, nseq = 0;
   int off_ids = 0, off_pos = 0, off_slots = 0, off_rows = 0, off_dwork = 0, off_pwork = 0, off_btab = 0;
   int off_samp = -1;   // SampleRow per sampled row, packed only when one of them has temperature >= 1e-5
+  int samp_words = 6;  // words per SampleRow: 7 when a sampled row has min_p, else 6 (min_p off)
+  int off_pen = -1;    // PenaltyRow per row with logits edits, packed only when n_pen > 0
+  int n_pen = 0;
+  bool pen_update = false;   // some edited row keeps a token history
   int off_lp = -1;     // logprobs rows: n_lp row indices into [0, S), then their n_lp N values; packed only when n_lp > 0
   int n_lp = 0;
   int words = 0;
@@ -289,6 +301,15 @@ struct Engine {
   size_t kv_layer_elems = 0;
   BlockPool pool;
 
+  // logits edits (penalties.cu): max_num_seqs record lists of pen_cap records (pen_lens[slot] in use), the raw values a
+  // step's edit pass overwrote [Scap][pen_cap], and the free slots
+  PenaltyRec* pen_recs = nullptr;
+  int* pen_lens = nullptr;
+  uint16_t* pen_save = nullptr;
+  int pen_cap = 0;
+  std::vector<int> pen_free;
+  std::vector<PenaltyRec> pen_tmp_;
+
   // step input staging
   int step_words_cap = 0;
   int32_t* stage_host = nullptr;  // pinned, one per ring slot
@@ -353,6 +374,8 @@ struct Engine {
   std::vector<int> rows_;
   std::vector<SampleRow> samp_;          // parameters of the rows in rows_ order
   std::vector<int> lp_rows_, lp_n_;      // logprobs rows (indices into rows_) and their N
+  std::vector<PenaltyRow> pen_;          // rows with logits edits
+  int admit_edits(Seq& s);
   bool ensure_blocks(Seq& s, int upto);
   void release_blocks(Seq& s);
   void preempt(std::shared_ptr<Seq> s);
@@ -414,7 +437,7 @@ Engine::~Engine() {
   cudaSetDevice(cfg.device);
   if (stream) cudaStreamSynchronize(stream);
   void* frees[] = {weights_blob, res, x, normed, qkv, attn, gu, act, last_hidden, logits, sampled, gemm_ws,
-                   gemm_counters, kv, cand, attn_ws, lp_dev, lp_ids_dev};
+                   gemm_counters, kv, cand, attn_ws, lp_dev, lp_ids_dev, pen_recs, pen_lens, pen_save};
   for (void* p : frees)
     if (p) cudaFree(p);
   for (auto p : stage_dev)
@@ -623,10 +646,21 @@ int Engine::alloc_all() {
   CK(cudaMemsetAsync(kv, 0, kv_layer_elems * 2 * L, stream));
   pool.init(nblocks, cfg.enable_prefix_caching != 0);
 
+  // ---- logits-edit record lists, allocated after the KV pool is sized (they do not change num_kv_blocks).  A list holds
+  // one record per distinct id: at most max_model_len history ids, B200_MAX_LOGIT_BIAS bias ids, as many stop ids and EOS.
+  pen_cap = cfg.max_model_len + 2 * B200_MAX_LOGIT_BIAS + 1;
+  CK(cudaMalloc(&pen_recs, static_cast<size_t>(Scap) * pen_cap * sizeof(PenaltyRec)));
+  CK(cudaMalloc(&pen_lens, static_cast<size_t>(Scap) * sizeof(int)));
+  CK(cudaMalloc(&pen_save, static_cast<size_t>(Scap) * pen_cap * sizeof(uint16_t)));
+  CK(cudaMemsetAsync(pen_lens, 0, static_cast<size_t>(Scap) * sizeof(int), stream));
+  for (int i = Scap - 1; i >= 0; --i) pen_free.push_back(i);
+
   // ---- step input ring
   max_blocks_per_seq = (cfg.max_model_len + kPage - 1) / kPage;
-  step_words_cap = 3 * Tcap + Scap + 4 * Scap + 4 * (Tcap / 16 + Scap + 1) + Scap * max_blocks_per_seq + 6 * Scap + 2 * Scap + 64;
-  static_assert(sizeof(SampleRow) == 6 * sizeof(int32_t), "SampleRow is 6 words of the step input");
+  step_words_cap = 3 * Tcap + Scap + 4 * Scap + 4 * (Tcap / 16 + Scap + 1) + Scap * max_blocks_per_seq + 7 * Scap + 2 * Scap +
+                   8 * Scap + 64;
+  static_assert(sizeof(SampleRow) == 7 * sizeof(int32_t), "SampleRow is 7 words of the step input");
+  static_assert(sizeof(PenaltyRow) == 8 * sizeof(int32_t), "PenaltyRow is 8 words of the step input");
   ring_n = std::max(1, cfg.record_steps) + 1;  // last slot = scratch for unrecorded steps
   CK(cudaMallocHost(&stage_host, static_cast<size_t>(step_words_cap) * 4));
   stage_dev.assign(ring_n, nullptr);
@@ -765,19 +799,33 @@ int Engine::forward(const StepMeta& m, int32_t* dbuf, bool all_logits, bf16* log
     P(B200_K_NORM); norm(final_norm, last_hidden, rows, m.S); Q();
     // argmax candidates per 128-row slab in the lm_head epilogue (the candidate buffer holds 128 rows), or bf16 logits.
     // A step with a sampled row (temperature >= 1e-5) writes the logits and selects every row's token in one sample_rows
-    // launch, greedy rows included.  A step with a logprobs row writes the logits too, for logprobs_rows.
+    // launch, greedy rows included.  A step with a logprobs row writes the logits too, for logprobs_rows, and so does a
+    // step with logits edits: they are applied before the token selection and undone after it.
     const bool samp = m.off_samp >= 0;
-    const bool cand_ok = !samp && m.n_lp == 0 && fused && !keep_logits && m.S <= 128;
+    const bool cand_ok = !samp && m.n_lp == 0 && m.n_pen == 0 && fused && !keep_logits && m.S <= 128;
+    const PenaltyRow* pen_rows = m.n_pen > 0 ? reinterpret_cast<const PenaltyRow*>(dbuf + m.off_pen) : nullptr;
     Gemm3Params p = proj(p_lm, cand_ok ? GEMM3_EPI_ARGMAX : GEMM3_EPI_PLAIN);
     p.out = logits; p.ldo = V; p.cand = cand;
     P(B200_K_GEMM_LM); rc |= launch_proj(p, xm_last, m.S); Q();
     last_S = m.S;
+    if (m.n_pen > 0) {
+      P(B200_K_ARGMAX);
+      rc |= penalize_rows(logits, V, pen_rows, m.n_pen, pen_recs, pen_lens, pen_cap, pen_save, stream);
+      Q();
+      launched(1);
+    }
     P(B200_K_ARGMAX);
-    if (samp) rc |= sample_rows(logits, V, reinterpret_cast<const SampleRow*>(dbuf + m.off_samp), m.S, V, sampled, stream);
+    if (samp) rc |= sample_rows(logits, V, dbuf + m.off_samp, m.samp_words, m.S, V, sampled, stream);
     else if (cand_ok) rc |= argmax_candidates(cand, sampled, m.S, (V + 127) / 128, stream);
     else rc |= argmax_rows(logits, sampled, m.S, V, V, stream);
     Q();
     launched(1);
+    if (m.n_pen > 0) {   // logprobs and the kept logits read the raw rows
+      P(B200_K_ARGMAX);
+      rc |= penalize_restore(logits, V, pen_rows, m.n_pen, pen_recs, pen_lens, pen_cap, pen_save, stream);
+      Q();
+      launched(1);
+    }
     if (m.n_lp > 0) {   // after the token selection: it reads the sampled ids
       const int* lr = dbuf + m.off_lp;
       P(B200_K_ARGMAX);
@@ -804,6 +852,10 @@ void Engine::release_blocks(Seq& s) {
   // tail blocks go to the front of the LRU free queue order first (vLLM frees in reverse)
   for (auto it = s.blocks.rbegin(); it != s.blocks.rend(); ++it) pool.unref(*it);
   s.blocks.clear();
+  if (s.pen_slot >= 0) {   // the record list is a function of s.toks: the next admission rebuilds it
+    pen_free.push_back(s.pen_slot);
+    s.pen_slot = -1;
+  }
   s.n_computed = 0;
   s.n_published = 0;
   s.chain_uid = 0;
@@ -859,6 +911,29 @@ void Engine::admit_prefix(Seq& s) {
     stats.cached_prompt_tokens += s.n_computed;
     stats.prompt_tokens += s.n_prompt;
   }
+}
+
+// Build the request's record list from its prompt and generated tokens and upload it, once per admission (the first and
+// each one after a preemption); from then on only the device changes it.  The stream is idle here (the previous step has
+// completed), so waiting for the copy costs its own time only.
+int Engine::admit_edits(Seq& s) {
+  s.pen_slot = pen_free.back();
+  pen_free.pop_back();
+  std::vector<int32_t> stops;
+  if (s.n_generated < s.min_tokens) {   // vLLM's all_stop_token_ids: the stop ids and EOS, ignore_eos or not
+    for (int32_t t : s.stop_ids) if (t >= 0 && t < V) stops.push_back(t);
+    if (cfg.eos_token_id >= 0 && cfg.eos_token_id < V) stops.push_back(cfg.eos_token_id);
+  }
+  const int np = s.n_prompt, no = static_cast<int>(s.toks.size()) - s.n_prompt;
+  penalty_records(s.toks.data(), np, s.toks.data() + np, no, s.pen_history(), s.bias_ids.data(), s.bias_values.data(),
+                  static_cast<int>(s.bias_ids.size()), stops.data(), static_cast<int>(stops.size()), &pen_tmp_);
+  const int n = static_cast<int>(pen_tmp_.size());
+  if (n > pen_cap) { set_error("record list of %d entries exceeds %d", n, pen_cap); return B200_ERR_INVALID; }
+  CK(cudaMemcpyAsync(pen_recs + static_cast<size_t>(s.pen_slot) * pen_cap, pen_tmp_.data(), static_cast<size_t>(n) * sizeof(PenaltyRec),
+                     cudaMemcpyHostToDevice, stream));
+  CK(cudaMemcpyAsync(pen_lens + s.pen_slot, &n, sizeof(int), cudaMemcpyHostToDevice, stream));
+  CK(cudaStreamSynchronize(stream));
+  return 0;
 }
 
 // ------------------------------------------------------------------ one scheduler iteration + forward
@@ -942,6 +1017,8 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
     s->admitted = true;
     waiting.pop_front();
     running.push_back(s);
+    if (s->edits())
+      if (int rc = admit_edits(*s)) return rc;
     sched.push_back({s, n});
     budget -= n;
   }
@@ -963,7 +1040,8 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
   samp_.clear();
   lp_rows_.clear();
   lp_n_.clear();
-  bool any_sampled = false;
+  pen_.clear();
+  bool any_sampled = false, any_minp = false;
   int32_t* h = stage_host;
   m.off_ids = 0; m.off_pos = m.T; m.off_slots = 2 * m.T;
   int tok = 0;
@@ -991,8 +1069,14 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
       rows_.push_back(tok + n - 1);
       // n = the index of the token this row generates: a request recomputed after preemption draws the same noise
       samp_.push_back({s.temperature, s.top_k, s.top_p, static_cast<uint32_t>(s.seed), static_cast<uint32_t>(s.seed >> 32),
-                       s.n_generated});
+                       s.n_generated, s.min_p});
       any_sampled |= s.temperature >= 1e-5f;
+      any_minp |= s.temperature >= 1e-5f && s.min_p > 0.f;
+      if (s.pen_slot >= 0) {
+        pen_.push_back({static_cast<int>(rows_.size()) - 1, s.pen_slot, s.presence, s.frequency, s.repetition, s.n_generated,
+                        s.min_tokens, s.pen_history() ? 1 : 0});
+        m.pen_update |= s.pen_history();
+      }
       if (s.top_logprobs >= 0) {
         lp_rows_.push_back(static_cast<int>(rows_.size()) - 1);
         lp_n_.push_back(s.top_logprobs);
@@ -1023,8 +1107,15 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
   w += m.nseq * max_blocks_per_seq;
   if (any_sampled) {   // greedy-only steps carry no sampling section: the same words as without one
     m.off_samp = w;
-    memcpy(h + w, samp_.data(), samp_.size() * sizeof(SampleRow));
-    w += 6 * m.S;
+    m.samp_words = any_minp ? 7 : 6;   // likewise min_p takes a word per row only in steps that have it
+    for (int i = 0; i < m.S; ++i) memcpy(h + w + i * m.samp_words, &samp_[i], m.samp_words * sizeof(int32_t));
+    w += m.samp_words * m.S;
+  }
+  m.n_pen = static_cast<int>(pen_.size());
+  if (m.n_pen > 0) {   // and logits edits
+    m.off_pen = w;
+    memcpy(h + w, pen_.data(), pen_.size() * sizeof(PenaltyRow));
+    w += 8 * m.n_pen;
   }
   m.n_lp = static_cast<int>(lp_rows_.size());
   if (m.n_lp > 0) {   // likewise steps without a logprobs row carry no logprobs section
@@ -1054,7 +1145,12 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
   nvtxRangePushA(nv);
   CK(cudaMemcpyAsync(dbuf, h, static_cast<size_t>(w) * 4, cudaMemcpyHostToDevice, stream));
   CK(cudaEventRecord(ev0, stream));
-  const int frc = forward(m, dbuf, false, nullptr);
+  int frc = forward(m, dbuf, false, nullptr);
+  if (!frc && m.pen_update) {   // here, not in forward(): a replay must not change any history
+    ++stats.kernel_launches;
+    if (penalize_update(reinterpret_cast<const PenaltyRow*>(dbuf + m.off_pen), m.n_pen, sampled, pen_recs, pen_lens, pen_cap, stream))
+      frc = cuda_fail("penalize_update", -2);
+  }
   nvtxRangePop();
   if (frc) return frc;
   CK(cudaEventRecord(ev1, stream));
@@ -1307,6 +1403,21 @@ int b200_submit(b200_engine* e, const int32_t* prompt_ids, int32_t n, const b200
   if (sp && (sp->top_logprobs < 0 || sp->top_logprobs > B200_MAX_LOGPROBS)) { set_error("top_logprobs must be in 0..%d", B200_MAX_LOGPROBS); return B200_ERR_INVALID; }
   if (sp && sp->top_logprobs > 0 && !sp->logprobs) { set_error("top_logprobs needs logprobs"); return B200_ERR_INVALID; }
   for (int i = 0; i < n; ++i) if (prompt_ids[i] < 0 || prompt_ids[i] >= g.V) { set_error("token id out of range"); return B200_ERR_INVALID; }
+  // logits edits: vLLM's SamplingParams._verify_args ranges (repetition_penalty 0 is "off" at this ABI)
+  if (sp) {
+    if (!(sp->presence_penalty >= -2.f && sp->presence_penalty <= 2.f)) { set_error("presence_penalty must be in [-2, 2]"); return B200_ERR_INVALID; }
+    if (!(sp->frequency_penalty >= -2.f && sp->frequency_penalty <= 2.f)) { set_error("frequency_penalty must be in [-2, 2]"); return B200_ERR_INVALID; }
+    if (!(sp->repetition_penalty >= 0.f && std::isfinite(sp->repetition_penalty))) { set_error("repetition_penalty must be finite and >= 0"); return B200_ERR_INVALID; }
+    if (!(sp->min_p >= 0.f && sp->min_p <= 1.f)) { set_error("min_p must be in [0, 1]"); return B200_ERR_INVALID; }
+    if (sp->min_tokens < 0 || sp->min_tokens > max_tokens) { set_error("min_tokens must be in 0..max_tokens (%d)", max_tokens); return B200_ERR_INVALID; }
+    if (sp->min_tokens > 0 && sp->num_stop_ids > B200_MAX_LOGIT_BIAS) { set_error("min_tokens takes at most %d stop ids", B200_MAX_LOGIT_BIAS); return B200_ERR_INVALID; }
+    if (sp->num_logit_bias < 0 || sp->num_logit_bias > B200_MAX_LOGIT_BIAS) { set_error("logit_bias takes at most %d entries", B200_MAX_LOGIT_BIAS); return B200_ERR_INVALID; }
+    if (sp->num_logit_bias > 0 && (!sp->logit_bias_ids || !sp->logit_bias_values)) { set_error("logit_bias: null arrays"); return B200_ERR_INVALID; }
+    for (int i = 0; i < sp->num_logit_bias; ++i) {
+      if (sp->logit_bias_ids[i] < 0 || sp->logit_bias_ids[i] >= g.V) { set_error("logit_bias id %d out of range [0, %d)", sp->logit_bias_ids[i], g.V); return B200_ERR_INVALID; }
+      if (!std::isfinite(sp->logit_bias_values[i])) { set_error("logit_bias values must be finite"); return B200_ERR_INVALID; }
+    }
+  }
   auto s = std::make_shared<Seq>();
   s->toks.assign(prompt_ids, prompt_ids + n);
   s->n_prompt = n;
@@ -1319,6 +1430,15 @@ int b200_submit(b200_engine* e, const int32_t* prompt_ids, int32_t n, const b200
     s->top_p = sp->top_p > 0.f ? sp->top_p : 1.f;   // 0 = off at this ABI
     s->top_k = sp->top_k > 0 ? sp->top_k : 0;
     s->top_logprobs = sp->logprobs ? sp->top_logprobs : -1;
+    s->min_p = sp->temperature >= 1e-5f ? sp->min_p : 0.f;   // greedy rows ignore min_p, as in vLLM
+    s->presence = sp->presence_penalty;
+    s->frequency = sp->frequency_penalty;
+    s->repetition = sp->repetition_penalty > 0.f ? sp->repetition_penalty : 1.f;
+    s->min_tokens = sp->min_tokens;
+    if (sp->num_logit_bias > 0) {
+      s->bias_ids.assign(sp->logit_bias_ids, sp->logit_bias_ids + sp->num_logit_bias);
+      s->bias_values.assign(sp->logit_bias_values, sp->logit_bias_values + sp->num_logit_bias);
+    }
   }
   {
     std::lock_guard<std::mutex> lk(g.mu_);

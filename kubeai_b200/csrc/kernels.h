@@ -5,6 +5,8 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <vector>
+
 #include "partials.cuh"
 
 namespace b200 {
@@ -27,18 +29,51 @@ int permute_gate_up(void* dst, const void* src, int I, int H, int to_physical, c
 int argmax_rows(const void* logits, int* out, int S, int V, int ld, cudaStream_t st, PartialView pv = no_partials());
 int init_uniform(void* p, size_t n, uint32_t seed, float scale, float offset, cudaStream_t st);
 
-// Per-row sampling parameters (sampling.cu; b200_sample_row at the ABI): temperature < 1e-5 is greedy, top_k <= 0 or >= V
-// and top_p <= 0 or >= 1 are off; the noise of the row is Philox4x32-10 keyed by the seed and counted by n, the index of
-// the token being generated.
+// Per-row sampling parameters (sampling.cu; b200_sample_row at the ABI): temperature < 1e-5 is greedy, top_k <= 0 or >= V,
+// top_p <= 0 or >= 1 and min_p <= 0 are off; the noise of the row is Philox4x32-10 keyed by the seed and counted by n, the
+// index of the token being generated.
 struct SampleRow {
   float temperature;
   int top_k;
   float top_p;
   uint32_t seed_lo, seed_hi;
   int n;
+  float min_p;
 };
-// out[s] = the token sampled from bf16 logits row s ([S, ld], ld % 8 == 0) under rows[s] (device memory)
-int sample_rows(const void* logits, int ld, const SampleRow* rows, int S, int V, int* out, cudaStream_t st);
+// out[s] = the token sampled from bf16 logits row s ([S, ld], ld % 8 == 0) under row s of `rows` (device memory): rows of
+// row_words = 7 words (a SampleRow) or 6 (the same without min_p, which is then off)
+int sample_rows(const void* logits, int ld, const void* rows, int row_words, int S, int V, int* out, cudaStream_t st);
+
+// Sparse logits edits (penalties.cu): logit_bias, min_tokens and the repetition / frequency / presence penalties of vLLM V1,
+// applied in fp32 to the entries a request's record list names and written back rounded to bf16.  A list holds one record
+// per distinct token id, sorted by id: its count in the output, whether it is in the prompt, whether it is a stop id (EOS
+// included unless ignore_eos) banned until min_tokens tokens exist, and its bias.
+enum { kPenPrompt = 1, kPenStop = 2, kPenBias = 4 };
+struct PenaltyRec {
+  int id;
+  int count;       // occurrences in the generated tokens
+  float bias;      // with kPenBias
+  uint32_t flags;  // kPen*
+};
+// One edited row of a step: logits row `row`, record list `slot`; repetition 1 = off.  history: the list counts the
+// generated tokens (some penalty is on), so penalize_update adds each sampled token to it.
+struct PenaltyRow {
+  int row, slot;
+  float presence, frequency, repetition;
+  int n_generated, min_tokens, history;
+};
+// Record list of one request from host token lists (the prompt and output only when `history`; stops only when they apply)
+void penalty_records(const int32_t* prompt, int n_prompt, const int32_t* output, int n_output, bool history,
+                     const int32_t* bias_ids, const float* bias_values, int n_bias, const int32_t* stops, int n_stops,
+                     std::vector<PenaltyRec>* out);
+// Record lists live in recs[slot * cap ...], their lengths in lens[slot].  penalize_rows edits the n rows in place and
+// saves the raw bf16 entries it overwrites in save [n][cap]; penalize_restore writes them back; penalize_update adds
+// sampled[row] of every history row to its list (count + 1, or a new record in id order).  Device pointers throughout.
+int penalize_rows(void* logits, int ld, const PenaltyRow* rows, int n, const PenaltyRec* recs, const int* lens, int cap,
+                  uint16_t* save, cudaStream_t st);
+int penalize_restore(void* logits, int ld, const PenaltyRow* rows, int n, const PenaltyRec* recs, const int* lens, int cap,
+                     const uint16_t* save, cudaStream_t st);
+int penalize_update(const PenaltyRow* rows, int n, const int* sampled, PenaltyRec* recs, int* lens, int cap, cudaStream_t st);
 
 // Log-probabilities (sampling.cu; vLLM's raw_logprobs) of n rows of bf16 logits ([., ld], ld % 8 == 0): row i is
 // r = rows ? rows[i] : i, its N = clamp(top_n[i], 0, min(V, kMaxLogprobs)).  lp[i * lp_ld] gets the log-probability of

@@ -3,9 +3,11 @@
 // deterministic:
 //   - temperature < 1e-5: argmax, lowest index on ties (the same token as argmax_kernel in elementwise.cu);
 //   - z_v = float(l_v) / temperature (fp32);
+//   - min_p keeps every token with fp32 (z_v - z_max) >= log(min_p) (compared in double): vLLM's p_v >= min_p * p_max as a
+//     fixed predicate, monotone in z, so it is one more key threshold;
 //   - top-k keeps every token whose z is >= the k-th largest z (ties at the k-th value are kept);
-//   - top-p keeps token v iff the softmax mass of the top-k-kept tokens with z strictly greater than z_v is < p, so tie
-//     groups are kept or dropped whole;
+//   - top-p keeps token v iff the softmax mass of the min_p- and top-k-kept tokens with z strictly greater than z_v is < p,
+//     so tie groups are kept or dropped whole;
 //   - the token is the argmax over the kept tokens of z_v - log(E_v), E_v = -log(u_v) ~ Exp(1) (the probs / q race of
 //     vLLM's random_sample), lowest index on ties.  u_v = ((x >> 9) + 0.5) * 2^-23 is exact in fp32 and strictly inside
 //     (0, 1); x is word v & 3 of Philox4x32-10 with counter (v >> 2, n, 0, 0) and key (seed_lo, seed_hi).
@@ -18,8 +20,9 @@
 // floor(exp(z_v - z_max) * 2^40); both are summed with integer shared-memory atomics, whose result does not depend on
 // arrival order (2^40 * 2^17 tokens fits in 64 bits).  The passes re-read the row (250 KB at Llama-3's vocabulary), which
 // is still in L2 right after the lm_head:
-//   1 row max (top-p only)   2 high-byte histogram   3 low-byte histogram of the top-k bin   4 the same for the top-p bin
-//   (skipped when it is the top-k bin)   5 the race over the tokens at or above the threshold.
+//   1 row max (top-p, min_p)   2 high-byte histogram   3 low-byte histogram of the top-k bin   3b the same for the min_p
+//   bin, when min_p cuts deeper than top-k under top-p   4 the same for the top-p bin (skipped when pass 3 / 3b holds it)
+//   5 the race over the tokens at or above the threshold.  min_p's key is found by a binary search over the 65536 keys.
 // Rows with temperature only run pass 5 alone.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -150,19 +153,23 @@ __device__ __forceinline__ int warp_last_bin(const T* h, unsigned long long abov
 }
 
 __global__ void __launch_bounds__(kThreads) sample_kernel(const uint16_t* __restrict__ logits, int ld,
-                                                          const SampleRow* __restrict__ rows, int V, int* __restrict__ out) {
+                                                          const int32_t* __restrict__ rows, int row_words, int V,
+                                                          int* __restrict__ out) {
   __shared__ uint32_t cnt_hi[256], cnt_lo[256];
   __shared__ unsigned long long mass_hi[256], mass_lo[256];
   __shared__ float sb[32];
   __shared__ int si[32];
-  __shared__ uint32_t s_kmax, s_thr;
+  __shared__ uint32_t s_kmax, s_thr, s_tm;
   extern __shared__ __align__(16) unsigned char dyn_smem[];   // kPrivSmem: per-lane histogram copies
   unsigned long long* priv_mass = reinterpret_cast<unsigned long long*>(dyn_smem);
   uint32_t* priv_cnt = reinterpret_cast<uint32_t*>(dyn_smem + 256 * 32 * sizeof(unsigned long long));
   griddep_enter();
   const int s = blockIdx.x;
   const uint16_t* row = logits + static_cast<size_t>(s) * ld;
-  const SampleRow P = rows[s];
+  // rows of 6 words carry no min_p (steps without a min_p row keep their size)
+  SampleRow P;
+  memcpy(&P, rows + static_cast<size_t>(s) * row_words, 6 * sizeof(int32_t));
+  P.min_p = row_words > 6 ? __int_as_float(rows[static_cast<size_t>(s) * row_words + 6]) : 0.f;
 
   if (!(P.temperature >= kSamplingEps)) {
     // greedy: argmax_kernel's comparisons, so the same token
@@ -183,21 +190,40 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const uint16_t* __rest
   const float T = P.temperature;
   const bool topk_on = P.top_k > 0 && P.top_k < V;
   const bool topp_on = P.top_p > 0.f && P.top_p < 1.f;
+  const bool minp_on = P.min_p > 0.f;
   uint32_t thr = 0;   // the race runs over the tokens with key >= thr
-  if (topk_on || topp_on) {
-    float zmax = 0.f;
-    if (topp_on) {
-      // pass 1: row max, as a key (an integer max does not depend on order)
-      uint32_t km = 0;
-      visit_row(row, V, [&](int, uint32_t b) { km = max(km, key_of(b)); });
+  float zmax = 0.f;
+  uint32_t tm = 0;    // min_p: the smallest kept key
+  if (topp_on || minp_on) {
+    // pass 1: row max, as a key (an integer max does not depend on order)
+    uint32_t km = 0;
+    visit_row(row, V, [&](int, uint32_t b) { km = max(km, key_of(b)); });
 #pragma unroll
-      for (int o = 16; o > 0; o >>= 1) km = max(km, __shfl_xor_sync(0xffffffffu, km, o));
-      if (threadIdx.x == 0) s_kmax = 0;
+    for (int o = 16; o > 0; o >>= 1) km = max(km, __shfl_xor_sync(0xffffffffu, km, o));
+    if (threadIdx.x == 0) s_kmax = 0;
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) atomicMax(&s_kmax, km);
+    __syncthreads();
+    zmax = __fdiv_rn(bf16_bits_to_f32(bits_of_key(s_kmax)), T);
+    if (minp_on) {
+      // the smallest key t with (z(t) - z_max) >= log(min_p): the row max satisfies it (min_p <= 1), and NaN keys sit below
+      // -inf and fail it, so the predicate is false then true along the keys
+      if (threadIdx.x == 0) {
+        const double lm = log(static_cast<double>(P.min_p));
+        uint32_t lo = 0, hi = s_kmax;
+        while (lo < hi) {
+          const uint32_t mid = (lo + hi) >> 1;
+          const float d = __fsub_rn(__fdiv_rn(bf16_bits_to_f32(bits_of_key(mid)), T), zmax);
+          if (static_cast<double>(d) >= lm) hi = mid;
+          else lo = mid + 1;
+        }
+        s_tm = lo;
+      }
       __syncthreads();
-      if ((threadIdx.x & 31) == 0) atomicMax(&s_kmax, km);
-      __syncthreads();
-      zmax = __fdiv_rn(bf16_bits_to_f32(bits_of_key(s_kmax)), T);
+      tm = s_tm;
     }
+  }
+  if (topk_on || topp_on) {
     auto fixed_mass = [&](uint32_t b) {
       const float m = expf(__fsub_rn(__fdiv_rn(bf16_bits_to_f32(b), T), zmax));   // in [0, 1]
       return __float2ull_rz(__fmul_rn(m, kMassScale));
@@ -269,6 +295,22 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const uint16_t* __rest
       for (int o = 16; o > 0; o >>= 1) m += __shfl_xor_sync(0xffffffffu, m, o);
       z = m;
     }
+    int lo_bin = topk_on ? bk : -1;   // the high-byte bin whose low-byte histograms cnt_lo / mass_lo hold
+    if (topp_on && minp_on) {
+      // top-p runs over the mass of the tokens at or above max(tk, tm): when min_p cuts deeper, that is the bins above
+      // tm's and the keys >= tm inside it
+      const int bm = static_cast<int>(tm >> 8);
+      if (bm != lo_bin) histogram(bm, cnt_lo, mass_lo);   // pass 3b
+      lo_bin = bm;
+      if (lead && tm > tk) {
+        unsigned long long m = 0;
+        for (int i = threadIdx.x; i < 256; i += 32)
+          m += (i > bm ? mass_hi[i] : 0ull) + (i >= static_cast<int>(tm & 0xFFu) ? mass_lo[i] : 0ull);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) m += __shfl_xor_sync(0xffffffffu, m, o);
+        z = m;
+      }
+    }
     uint32_t tp = 0;
     if (topp_on) {
       // top-p: keep v iff mass(kept, key > key_v) < p * z, i.e. key_v >= the largest key t with mass(kept, key >= t) >=
@@ -282,16 +324,18 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const uint16_t* __rest
       if (threadIdx.x == 0) s_thr = static_cast<uint32_t>(bp);
       __syncthreads();
       bp = static_cast<int>(s_thr);
-      if (bp != bk) histogram(bp, cnt_lo, mass_lo);   // pass 4 (pass 3 already holds bin bk)
+      if (bp != lo_bin) histogram(bp, cnt_lo, mass_lo);   // pass 4 (pass 3 / 3b already holds bin lo_bin)
       if (lead) {
         const int lo = warp_last_bin(mass_lo, mab, reach, &unused);
         tp = (static_cast<uint32_t>(bp) << 8) | static_cast<uint32_t>(lo);
       }
     }
     __syncthreads();   // every reader of s_thr is past it
-    if (threadIdx.x == 0) s_thr = max(tk, tp);
+    if (threadIdx.x == 0) s_thr = max(max(tk, tp), tm);
     __syncthreads();
     thr = s_thr;
+  } else {
+    thr = tm;
   }
 
   // pass 5: the exponential race over the tokens with key >= thr
@@ -496,12 +540,13 @@ int logprobs_rows(const void* logits, int ld, int V, const int* rows, const int*
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 
-int sample_rows(const void* logits, int ld, const SampleRow* rows, int S, int V, int* out, cudaStream_t st) {
+int sample_rows(const void* logits, int ld, const void* rows, int row_words, int S, int V, int* out, cudaStream_t st) {
   if (S <= 0) return 0;
-  if (V < 1 || ld < V || ld % 8 || (reinterpret_cast<uintptr_t>(logits) & 15)) return -1;
+  if (V < 1 || ld < V || ld % 8 || (reinterpret_cast<uintptr_t>(logits) & 15) || (row_words != 6 && row_words != 7)) return -1;
   static std::atomic<unsigned long long> smem_set{0};
   if (!ensure_dynamic_smem(sample_kernel, kPrivSmem, &smem_set)) return -2;
-  launch_pdl(sample_kernel, dim3(S), dim3(kThreads), kPrivSmem, st, static_cast<const uint16_t*>(logits), ld, rows, V, out);
+  launch_pdl(sample_kernel, dim3(S), dim3(kThreads), kPrivSmem, st, static_cast<const uint16_t*>(logits), ld,
+             static_cast<const int32_t*>(rows), row_words, V, out);
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 

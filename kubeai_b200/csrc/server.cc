@@ -50,6 +50,7 @@ struct Server {
   int max_model_len = 2048;
   bool sampling = false;   // b200_server_config.enable_sampling: serve temperature >= 1e-5 (else greedy only)
   bool logprobs = false;   // b200_server_config.enable_logprobs: serve logprobs / top_logprobs (else a 400)
+  bool edits = false;      // b200_server_config.enable_logits_processors: serve penalties, min_p, min_tokens, logit_bias
   // optional real tokenizer (b200_server_set_tokenizer): a checkpoint's tokenizer.json instead of the synthetic byte/word ids
   const b200_tokenizer* real_tok = nullptr;
 
@@ -167,6 +168,11 @@ struct ParsedRequest {
   int64_t seed = 0;
   int logprobs = -1;   // -1: none; else the number of most likely tokens per position (chat top_logprobs, completions logprobs)
   std::vector<int32_t> stop_ids;
+  // logits edits (b200_sampling): read only when the server serves them
+  double presence = 0.0, frequency = 0.0, repetition = 1.0, min_p = 0.0;
+  int min_tokens = 0;
+  std::vector<int32_t> bias_ids;
+  std::vector<float> bias_values;
 };
 
 std::string content_text(const JVal& c) {
@@ -312,6 +318,56 @@ int parse_request(Server& sv, const std::string& path, const std::string& ctype,
       return 400;
     }
   }
+  if (sv.edits) {
+    // vLLM's SamplingParams ranges (sampling_params.py _verify_args, _validate_logit_bias); null is absent
+    std::string bad_ed;
+    auto number = [&](const char* k, double* dst, double lo, double hi, bool lo_open) {
+      const JVal* v = root.get(k);
+      if (!v || v->type == JVal::Null || !bad_ed.empty()) return;
+      if (v->type != JVal::Num) { bad_ed = std::string(k) + " must be a number"; return; }
+      char b[160];
+      if (!((lo_open ? v->num > lo : v->num >= lo) && v->num <= hi)) {
+        if (hi > 1e30) snprintf(b, sizeof(b), "%s must be greater than zero, got %g.", k, v->num);
+        else snprintf(b, sizeof(b), "%s must be in [%g, %g], got %g.", k, lo, hi, v->num);
+        bad_ed = b;
+        return;
+      }
+      *dst = v->num;
+    };
+    number("presence_penalty", &pr->presence, -2.0, 2.0, false);
+    number("frequency_penalty", &pr->frequency, -2.0, 2.0, false);
+    number("repetition_penalty", &pr->repetition, 0.0, 3.0e38, true);
+    number("min_p", &pr->min_p, 0.0, 1.0, false);
+    if (const JVal* v = root.get("min_tokens"); bad_ed.empty() && v && v->type != JVal::Null) {
+      if (v->type != JVal::Num || !(v->num >= 0 && v->num == std::floor(v->num) && v->num <= 2147483647.0))
+        bad_ed = "min_tokens must be an integer >= 0";
+      else pr->min_tokens = static_cast<int>(v->num);
+    }
+    if (const JVal* v = root.get("logit_bias"); bad_ed.empty() && v && v->type != JVal::Null) {
+      if (v->type != JVal::Obj) bad_ed = "logit_bias must be an object of token ids to numbers";
+      else if (v->obj.size() > B200_MAX_LOGIT_BIAS) bad_ed = "logit_bias takes at most " + std::to_string(B200_MAX_LOGIT_BIAS) + " entries";
+      std::string oov;
+      for (auto& kv : v->obj) {
+        if (!bad_ed.empty()) break;
+        const std::string& key = kv.first;
+        size_t i = (!key.empty() && (key[0] == '-' || key[0] == '+')) ? 1 : 0;
+        bool digits = i < key.size() && key.size() - i <= 9;
+        for (size_t j = i; j < key.size() && digits; ++j) digits = key[j] >= '0' && key[j] <= '9';
+        if (!digits) { bad_ed = "logit_bias keys must be integer token ids, got \"" + key + "\""; break; }
+        if (kv.second.type != JVal::Num) { bad_ed = "logit_bias values must be numbers"; break; }
+        const long id = strtol(key.c_str(), nullptr, 10);
+        if (id < 0 || id >= sv.tok.vocab) { oov += (oov.empty() ? "" : ", ") + std::to_string(id); continue; }
+        pr->bias_ids.push_back(static_cast<int32_t>(id));
+        pr->bias_values.push_back(static_cast<float>(std::min(100.0, std::max(-100.0, kv.second.num))));   // OpenAI's clamp
+      }
+      if (bad_ed.empty() && !oov.empty())
+        bad_ed = "token_id(s) [" + oov + "] in logit_bias contain out-of-vocab token ids. Vocabulary size: " + std::to_string(sv.tok.vocab);
+    }
+    if (!bad_ed.empty()) {
+      *err = "bad request: " + bad_ed;
+      return 400;
+    }
+  }
   if (const JVal* v = root.get("stop_token_ids"); v && v->type == JVal::Arr)
     for (auto& e : v->arr)
       if (e.type == JVal::Num) pr->stop_ids.push_back(static_cast<int32_t>(e.num));
@@ -336,11 +392,11 @@ int parse_request(Server& sv, const std::string& path, const std::string& ctype,
   else if (nonempty("stop")) bad = "stop strings (use stop_token_ids)";
   else if (truthy("echo")) bad = "echo";
   else if (nonempty("suffix")) bad = "suffix";
-  else if (num_of("presence_penalty", 0) != 0 || num_of("frequency_penalty", 0) != 0 || num_of("repetition_penalty", 1) != 1) bad = "sampling penalties";
-  else if (nonempty("logit_bias")) bad = "logit_bias";
+  else if (!sv.edits && (num_of("presence_penalty", 0) != 0 || num_of("frequency_penalty", 0) != 0 || num_of("repetition_penalty", 1) != 1)) bad = "sampling penalties";
+  else if (!sv.edits && nonempty("logit_bias")) bad = "logit_bias";
   else if (nonempty("tools") || nonempty("functions")) bad = "tool calling";
-  else if (truthy("min_tokens")) bad = "min_tokens";
-  else if (num_of("min_p", 0) > 0 && pr->temperature >= 1e-5) bad = "min_p";   // harmless under greedy decoding only
+  else if (!sv.edits && truthy("min_tokens")) bad = "min_tokens";
+  else if (!sv.edits && num_of("min_p", 0) > 0 && pr->temperature >= 1e-5) bad = "min_p";   // harmless under greedy decoding only
   else if (const JVal* rf = root.get("response_format"); rf && rf->type == JVal::Obj) {
     const JVal* ty = rf->get("type");
     if (ty && ty->type == JVal::Str && ty->str != "text") bad = "response_format other than text";
@@ -497,6 +553,9 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
   if (static_cast<int>(ids.size()) + 1 > sv.max_model_len)
     return send_error(w, 400, "bad request: prompt is longer than the model's context length");
   max_tokens = std::min(max_tokens, sv.max_model_len - static_cast<int>(ids.size()));
+  if (pr.min_tokens > max_tokens)
+    return send_error(w, 400, "bad request: min_tokens must be less than or equal to max_tokens=" + std::to_string(max_tokens) +
+                                  ", got " + std::to_string(pr.min_tokens) + ".");
 
   // metrics.InferenceRequestsActive +1 / defer -1 (handler.go:76-81)
   {
@@ -548,6 +607,14 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
     sp.ignore_eos = pr.ignore_eos ? 1 : 0;
     sp.logprobs = pr.logprobs >= 0 ? 1 : 0;
     sp.top_logprobs = std::max(pr.logprobs, 0);
+    sp.presence_penalty = static_cast<float>(pr.presence);
+    sp.frequency_penalty = static_cast<float>(pr.frequency);
+    sp.repetition_penalty = static_cast<float>(pr.repetition);
+    sp.min_p = static_cast<float>(pr.min_p);
+    sp.min_tokens = pr.min_tokens;
+    sp.num_logit_bias = static_cast<int>(pr.bias_ids.size());
+    sp.logit_bias_ids = pr.bias_ids.empty() ? nullptr : pr.bias_ids.data();
+    sp.logit_bias_values = pr.bias_values.empty() ? nullptr : pr.bias_values.data();
     std::vector<int32_t> stops = pr.stop_ids;
     if (sv.real_tok && !pr.ignore_eos) {   // the checkpoint's end-of-turn / end-of-text tokens end the generation
       for (const char* name : {"<|eot_id|>", "<|end_of_text|>"}) {
@@ -907,6 +974,7 @@ int b200_server_create(const b200_server_config* cfg, b200_engine* const* replic
   sv.max_model_len = cfg->max_model_len > 0 ? cfg->max_model_len : 2048;
   sv.sampling = cfg->enable_sampling != 0;
   sv.logprobs = cfg->enable_logprobs != 0;
+  sv.edits = cfg->enable_logits_processors != 0;
   if (b200_router_create(sv.replication, &sv.router)) { delete s; return B200_ERR_INVALID; }
   std::vector<std::string> names;
   std::string ad = cfg->adapters ? cfg->adapters : "";

@@ -87,18 +87,27 @@ class Engine:
             pass
 
     def submit(self, prompt_ids, max_tokens=16, ignore_eos=True, stop_ids=(), temperature=0.0, top_p=1.0, top_k=0,
-               seed=None, logprobs=False, top_logprobs=0) -> int:
+               seed=None, logprobs=False, top_logprobs=0, min_p=0.0, presence_penalty=0.0, frequency_penalty=0.0,
+               repetition_penalty=1.0, min_tokens=0, logit_bias=None) -> int:
         """temperature < 1e-5 is greedy; top_k 0 / -1 and top_p 1 are off; seed None = one drawn by the engine.
         logprobs: keep each generated token's log-probability and its top_logprobs (0..20) most likely tokens, read with
-        poll_logprobs."""
+        poll_logprobs.  min_p 0, the penalties 0 (repetition 1), min_tokens 0 and logit_bias None ({id: bias}) are off."""
         ids = np.ascontiguousarray(prompt_ids, dtype=np.int32)
         stops = np.ascontiguousarray(stop_ids, dtype=np.int32)
+        bias = dict(logit_bias or {})
+        bias_ids = np.ascontiguousarray(list(bias.keys()), dtype=np.int32)
+        bias_vals = np.ascontiguousarray(list(bias.values()), dtype=np.float32)
         sp = Sampling(max_tokens=max_tokens, temperature=temperature, ignore_eos=1 if ignore_eos else 0,
                       num_stop_ids=len(stops),
                       stop_ids=stops.ctypes.data_as(C.POINTER(C.c_int32)) if len(stops) else None,
                       top_p=top_p, top_k=top_k, has_seed=0 if seed is None else 1,
                       seed=0 if seed is None else seed & 0xFFFFFFFFFFFFFFFF,
-                      logprobs=1 if logprobs else 0, top_logprobs=top_logprobs)
+                      logprobs=1 if logprobs else 0, top_logprobs=top_logprobs,
+                      presence_penalty=presence_penalty, frequency_penalty=frequency_penalty,
+                      repetition_penalty=repetition_penalty, min_p=min_p, min_tokens=min_tokens,
+                      num_logit_bias=len(bias_ids),
+                      logit_bias_ids=bias_ids.ctypes.data_as(C.POINTER(C.c_int32)) if len(bias_ids) else None,
+                      logit_bias_values=bias_vals.ctypes.data_as(C.POINTER(C.c_float)) if len(bias_ids) else None)
         rid = C.c_uint64()
         check(self._l.b200_submit(self._h, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), C.byref(sp),
                                   C.byref(rid)))

@@ -127,14 +127,14 @@ def argmax(logits):
     return out
 
 
-def sample(logits, temperature, top_k=0, top_p=1.0, seed=0, n=0):
+def sample(logits, temperature, top_k=0, top_p=1.0, seed=0, n=0, min_p=0.0):
     """Token per row of bf16 logits [S, V] (b200_op_sample).  Each parameter is a scalar or one value per row:
-    temperature < 1e-5 = greedy; top_k 0 / -1 / >= V and top_p 1 = off; seed (uint64) keys the row's Philox stream and
-    n (the index of the token being generated) counts it."""
+    temperature < 1e-5 = greedy; top_k 0 / -1 / >= V, top_p 1 and min_p 0 = off; seed (uint64) keys the row's Philox
+    stream and n (the index of the token being generated) counts it."""
     _chk(logits)
     S = logits.shape[0]
     rows = np.empty(S, dtype=[("temperature", "<f4"), ("top_k", "<i4"), ("top_p", "<f4"), ("seed_lo", "<u4"),
-                              ("seed_hi", "<u4"), ("n", "<i4")])
+                              ("seed_hi", "<u4"), ("n", "<i4"), ("min_p", "<f4")])
     seed = np.broadcast_to(np.asarray(seed, dtype=object), (S,))
     rows["temperature"] = np.broadcast_to(np.asarray(temperature, dtype=np.float32), (S,))
     rows["top_k"] = np.broadcast_to(np.asarray(top_k, dtype=np.int32), (S,))
@@ -142,10 +142,41 @@ def sample(logits, temperature, top_k=0, top_p=1.0, seed=0, n=0):
     rows["seed_lo"] = [int(s) & 0xFFFFFFFF for s in seed]
     rows["seed_hi"] = [(int(s) >> 32) & 0xFFFFFFFF for s in seed]
     rows["n"] = np.broadcast_to(np.asarray(n, dtype=np.int32), (S,))
-    rows_dev = torch.from_numpy(rows.view(np.int32).reshape(S, 6).copy()).to(logits.device)
+    rows["min_p"] = np.broadcast_to(np.asarray(min_p, dtype=np.float32), (S,))
+    rows_dev = torch.from_numpy(rows.view(np.int32).reshape(S, 7).copy()).to(logits.device)
     out = torch.empty(S, dtype=torch.int32, device=logits.device)
     check(lib().b200_op_sample(_p(logits), logits.stride(0), _p(rows_dev), S, logits.shape[1], _p(out), _stream()))
     return out
+
+
+def penalize(logits, rows, restore=True):
+    """The engine's logits edits on bf16 logits [S, V] (b200_op_penalize), one dict per row with any of presence_penalty,
+    frequency_penalty, repetition_penalty (1 or 0 = off), min_tokens, prompt, output, logit_bias ({id: bias}) and stop_ids.
+    restore=True: returns the edited rows and puts the raw values back into `logits`; False: edits `logits` in place and
+    returns it."""
+    from ._lib import PenaltyRow
+    _chk(logits)
+    S, V = logits.shape
+    keep, arr = [], (PenaltyRow * max(S, 1))()
+
+    def ptr(a, ct):
+        keep.append(a)
+        return a.ctypes.data_as(C.POINTER(ct)) if len(a) else None
+    for s, r in enumerate(rows):
+        prompt = np.ascontiguousarray(r.get("prompt", ()), dtype=np.int32)
+        output = np.ascontiguousarray(r.get("output", ()), dtype=np.int32)
+        stops = np.ascontiguousarray(r.get("stop_ids", ()), dtype=np.int32)
+        bias = dict(r.get("logit_bias") or {})
+        bid = np.ascontiguousarray(list(bias.keys()), dtype=np.int32)
+        bval = np.ascontiguousarray(list(bias.values()), dtype=np.float32)
+        arr[s] = PenaltyRow(presence_penalty=r.get("presence_penalty", 0.0), frequency_penalty=r.get("frequency_penalty", 0.0),
+                            repetition_penalty=r.get("repetition_penalty", 1.0), min_tokens=r.get("min_tokens", 0),
+                            num_prompt=len(prompt), prompt=ptr(prompt, C.c_int32), num_output=len(output),
+                            output=ptr(output, C.c_int32), num_logit_bias=len(bid), logit_bias_ids=ptr(bid, C.c_int32),
+                            logit_bias_values=ptr(bval, C.c_float), num_stop_ids=len(stops), stop_ids=ptr(stops, C.c_int32))
+    edited = torch.empty_like(logits) if restore else None
+    check(lib().b200_op_penalize(_p(logits), logits.stride(0), S, V, arr, _p(edited), _stream()))
+    return edited if restore else logits
 
 
 def logprobs(logits, tokens, top_n):
