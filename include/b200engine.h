@@ -97,6 +97,11 @@ typedef struct {
   int32_t num_logit_bias;     /* 0..B200_MAX_LOGIT_BIAS; ids in [0, vocab), finite values; a repeated id keeps its last */
   const int32_t* logit_bias_ids;
   const float* logit_bias_values;
+  /* Prompt log-probabilities (vLLM's prompt_logprobs), read with b200_poll_prompt_logprobs: for prompt positions k = 1..n-1,
+   * the raw log-probability of prompt token k from the row at position k-1, its rank and that row's top_prompt_logprobs
+   * most likely tokens.  Such a request does not read the prefix cache (vLLM's skip_reading_prefix_cache). */
+  int32_t prompt_logprobs;      /* 0 = off */
+  int32_t top_prompt_logprobs;  /* 0..B200_MAX_LOGPROBS */
 } b200_sampling;
 
 #define B200_MAX_LOGPROBS 20     /* vLLM's default max_logprobs */
@@ -144,6 +149,12 @@ int b200_poll(b200_engine* e, uint64_t req_id, int32_t* out_ids, int32_t cap, in
  * (lowest id on equal logits); the rest of each row is left as it was. */
 int b200_poll_logprobs(b200_engine* e, uint64_t req_id, int32_t* out_ids, float* out_logprob, int32_t* out_top_ids,
                        float* out_top_logprob, int32_t cap, int32_t* n_out, int32_t* finished, b200_usage* usage);
+/* The prompt log-probabilities of a request submitted with prompt_logprobs (else B200_ERR_INVALID).  *n_out = 0 until every
+ * record exists (no later than the first generated token is polled), then n_prompt - 1: record k is prompt token k + 1's
+ * out_logprob[k] and out_rank[k], and out_top_ids / out_top_logprob[k * B200_MAX_LOGPROBS + j], j < top_prompt_logprobs,
+ * the most likely tokens at that position.  cap < n_prompt - 1 is B200_ERR_INVALID.  The token cursor does not move. */
+int b200_poll_prompt_logprobs(b200_engine* e, uint64_t req_id, float* out_logprob, int32_t* out_rank, int32_t* out_top_ids,
+                              float* out_top_logprob, int32_t cap, int32_t* n_out);
 /* Block until the request has undrained tokens or is finished (B200_ERR_TIMEOUT otherwise). */
 int b200_wait(b200_engine* e, uint64_t req_id, int64_t timeout_us);
 int b200_abort(b200_engine* e, uint64_t req_id);
@@ -276,6 +287,9 @@ typedef struct {
   /* 1: serve presence_penalty, frequency_penalty, repetition_penalty, min_p, min_tokens and logit_bias (see b200_sampling);
    * 0: they get a 400, as before logits edits existed (a zero-initialised config keeps that) */
   int32_t enable_logits_processors;
+  /* 1: serve prompt_logprobs (both routes) and echo (completions) in vLLM's response format; 0: they get a 400, as before
+   * prompt logprobs existed (a zero-initialised config keeps that) */
+  int32_t enable_prompt_logprobs;
 } b200_server_config;
 int b200_server_create(const b200_server_config* cfg, b200_engine* const* replicas, int32_t n, b200_server** out);
 void b200_server_destroy(b200_server* s);
@@ -445,6 +459,10 @@ int b200_op_sample(const void* logits, int32_t ld, const b200_sample_row* rows, 
  * pointer is device memory. */
 int b200_op_logprobs(const void* logits, int32_t ld, int32_t S, int32_t V, const int32_t* tokens, const int32_t* top_n,
                      float* out_logprob, int32_t* out_top_ids, float* out_top_logprob, void* stream);
+/* b200_op_logprobs plus out_rank[s] (device): the number of tokens whose logit is >= that of tokens[s] (vLLM's prompt-logprob
+ * rank; equal logits share a rank).  The other outputs are bit-identical to b200_op_logprobs. */
+int b200_op_logprobs_rank(const void* logits, int32_t ld, int32_t S, int32_t V, const int32_t* tokens, const int32_t* top_n,
+                          float* out_logprob, int32_t* out_rank, int32_t* out_top_ids, float* out_top_logprob, void* stream);
 /* The logits edits of b200_sampling on explicit inputs, with the engine's device code: rows[s] (host memory) edits bf16
  * logits row s ([S, ld], device, in place) as a request with those parameters, prompt and output tokens would see it when
  * generating its num_output-th token (min_tokens counts the output; stop_ids are its stops, EOS included by the caller).

@@ -48,7 +48,8 @@ class Sampling(C.Structure):
                 ("logprobs", C.c_int32), ("top_logprobs", C.c_int32),
                 ("presence_penalty", C.c_float), ("frequency_penalty", C.c_float), ("repetition_penalty", C.c_float),
                 ("min_p", C.c_float), ("min_tokens", C.c_int32), ("num_logit_bias", C.c_int32),
-                ("logit_bias_ids", C.POINTER(C.c_int32)), ("logit_bias_values", C.POINTER(C.c_float))]
+                ("logit_bias_ids", C.POINTER(C.c_int32)), ("logit_bias_values", C.POINTER(C.c_float)),
+                ("prompt_logprobs", C.c_int32), ("top_prompt_logprobs", C.c_int32)]
 
 
 class SampleRow(C.Structure):
@@ -95,7 +96,7 @@ class ServerConfig(C.Structure):
                 ("mean_load_pct", C.c_int32), ("replication", C.c_int32), ("prefix_char_length", C.c_int32),
                 ("max_retries", C.c_int32), ("default_max_tokens", C.c_int32), ("vocab", C.c_int32),
                 ("max_model_len", C.c_int32), ("enable_sampling", C.c_int32), ("enable_logprobs", C.c_int32),
-                ("enable_logits_processors", C.c_int32)]
+                ("enable_logits_processors", C.c_int32), ("enable_prompt_logprobs", C.c_int32)]
 
 
 class HarnessConfig(C.Structure):
@@ -134,6 +135,7 @@ SYMBOLS = {
     "b200_submit": (C.c_int, [_vp, _pi32, _i32, C.POINTER(Sampling), C.POINTER(_u64)]),
     "b200_poll": (C.c_int, [_vp, _u64, _pi32, _i32, _pi32, _pi32, C.POINTER(Usage)]),
     "b200_poll_logprobs": (C.c_int, [_vp, _u64, _pi32, _vp, _pi32, _vp, _i32, _pi32, _pi32, C.POINTER(Usage)]),
+    "b200_poll_prompt_logprobs": (C.c_int, [_vp, _u64, _vp, _pi32, _pi32, _vp, _i32, _pi32]),
     "b200_wait": (C.c_int, [_vp, _u64, _i64]),
     "b200_abort": (C.c_int, [_vp, _u64]),
     "b200_release": (C.c_int, [_vp, _u64]),
@@ -200,6 +202,7 @@ SYMBOLS = {
     "b200_op_sample": (C.c_int, [_vp, _i32, _vp, _i32, _i32, _vp, _vp]),
     "b200_op_penalize": (C.c_int, [_vp, _i32, _i32, _i32, C.POINTER(PenaltyRow), _vp, _vp]),
     "b200_op_logprobs": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "b200_op_logprobs_rank": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "b200_op_paged_attn": (C.c_int, [_vp, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _f, _i32, _vp]),
     "b200_server_set_tokenizer": (C.c_int, [C.c_void_p, C.c_void_p]),
     "b200_server_render_prompt": (C.c_int64, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_size_t, _vp, C.c_size_t]),

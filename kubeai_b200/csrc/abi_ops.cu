@@ -324,6 +324,19 @@ int b200_op_logprobs(const void* logits, int32_t ld, int32_t S, int32_t V, const
   return rc ? cuda_fail("logprobs_rows", rc) : 0;
 }
 
+int b200_op_logprobs_rank(const void* logits, int32_t ld, int32_t S, int32_t V, const int32_t* tokens, const int32_t* top_n,
+                          float* out_logprob, int32_t* out_rank, int32_t* out_top_ids, float* out_top_logprob, void* stream) {
+  if (int rc = require_device()) return rc;
+  if (!logits || !tokens || !top_n || !out_logprob || !out_rank || !out_top_ids || !out_top_logprob || S < 0 || V < 1 ||
+      ld < V || ld % 8) {
+    set_error("b200_op_logprobs_rank: bad arguments (S=%d V=%d ld=%d; ld %% 8 == 0 and V <= ld required)", S, V, ld);
+    return B200_ERR_INVALID;
+  }
+  int rc = logprobs_rows(logits, ld, V, nullptr, top_n, S, tokens, out_logprob, 1, out_top_logprob, kMaxLogprobs, out_top_ids,
+                         static_cast<cudaStream_t>(stream), out_rank);
+  return rc ? cuda_fail("logprobs_rows", rc) : 0;
+}
+
 int b200_op_paged_attn(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                        const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
                        int32_t q_heads, int32_t kv_heads, float scale, int32_t decode, void* stream) {

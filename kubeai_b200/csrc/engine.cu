@@ -169,6 +169,11 @@ struct LogprobRecord {
   float top_lp[kMaxLogprobs];
   int32_t top_ids[kMaxLogprobs];
 };
+// one prompt position's record: the next prompt token's log-probability and rank, then the position's top N
+struct PromptLogprobRecord {
+  LogprobRecord r;
+  int32_t rank;
+};
 
 struct Seq {
   uint64_t id = 0;
@@ -186,6 +191,10 @@ struct Seq {
   int top_k = 0;
   uint64_t seed = 0;
   int top_logprobs = -1;   // -1: no logprobs; else the N of every generated token's record
+  // -1: no prompt logprobs; else the N of every prompt position's record.  plp_done = prompt positions whose record a
+  // launched step produces (engine thread): a prompt recomputed after a preemption does not produce them again
+  int prompt_logprobs = -1;
+  int plp_done = 0;
   // logits edits (penalties.cu): off when every field is at its default; pen_slot = the device record list while admitted
   float min_p = 0.f, presence = 0.f, frequency = 0.f, repetition = 1.f;
   int min_tokens = 0;
@@ -203,6 +212,7 @@ struct Seq {
   std::condition_variable cv;
   std::vector<int32_t> out;
   std::vector<LogprobRecord> lp_out;   // one per token of `out` when top_logprobs >= 0
+  std::vector<PromptLogprobRecord> plp_out;   // one per prompt position 0..n_prompt-2 when prompt_logprobs >= 0
   size_t drained = 0;
   int finished = 0;
   uint64_t arrival_key = 0;   // xxh64 of the prompt: admission order among requests that arrive between two steps
@@ -212,6 +222,7 @@ struct Seq {
 struct Sched {
   std::shared_ptr<Seq> s;
   int n;
+  int n_plp = 0;   // prompt-logprob rows this chunk produces
 };
 // a launched, not yet completed step
 struct InFlight {
@@ -226,6 +237,7 @@ struct Pub {
   bool has_tok;
   int code;
   int lp = -1;   // index of the token's record in Engine::pending_lp
+  int plp0 = 0, n_plp = 0;   // prompt records pending_plp[plp0, plp0 + n_plp), published before the token
 };
 
 struct StepMeta {
@@ -238,6 +250,10 @@ struct StepMeta {
   bool pen_update = false;   // some edited row keeps a token history
   int off_lp = -1;     // logprobs rows: n_lp row indices into [0, S), then their n_lp N values; packed only when n_lp > 0
   int n_lp = 0;
+  // prompt-logprob rows: n_plp step token indices, their target ids (the next prompt token), their N; packed only when
+  // n_plp > 0.  Records go to the plp buffers in this order.
+  int off_plp = -1;
+  int n_plp = 0;
   int words = 0;
   int64_t kv_tokens = 0;
   int out_tokens = 0;  // sampled rows that produce a generated token
@@ -310,6 +326,20 @@ struct Engine {
   std::vector<int> pen_free;
   std::vector<PenaltyRec> pen_tmp_;
 
+  // prompt logprobs: a step's rows go through the final norm, the lm_head and logprobs_rows in groups of plp_G, each
+  // group's hidden rows in prompt_hidden [plp_G, H] and its logits in prompt_logits [plp_G, V]; the records of the step's
+  // rows in step order: plp_f [Tcap][1 + kMaxLogprobs] floats (lp, then the top N), plp_ids [Tcap][kMaxLogprobs],
+  // plp_rank [Tcap]; device and pinned host copies
+  int plp_G = 0;
+  bf16 *prompt_hidden = nullptr, *prompt_logits = nullptr;
+  XMaps xm_phid;
+  float* plp_f_dev = nullptr;
+  int* plp_ids_dev = nullptr;
+  int* plp_rank_dev = nullptr;
+  float* plp_f_host = nullptr;
+  int32_t* plp_ids_host = nullptr;
+  int32_t* plp_rank_host = nullptr;
+
   // step input staging
   int step_words_cap = 0;
   int32_t* stage_host = nullptr;  // pinned, one per ring slot
@@ -369,9 +399,11 @@ struct Engine {
   void loop();
   std::vector<Pub> pending_pub;
   std::vector<LogprobRecord> pending_lp;   // records of pending_pub entries (Pub::lp)
+  std::vector<PromptLogprobRecord> pending_plp;   // prompt records of pending_pub entries (Pub::plp0, n_plp)
   InFlight inflight_;
   std::vector<AttnWork> dwork_, pwork_;  // packing scratch (kept across steps: no per-step allocation)
   std::vector<int> rows_;
+  std::vector<int> plp_tok_, plp_tgt_, plp_n_;   // prompt-logprob rows: step token index, target id, N
   std::vector<SampleRow> samp_;          // parameters of the rows in rows_ order
   std::vector<int> lp_rows_, lp_n_;      // logprobs rows (indices into rows_) and their N
   std::vector<PenaltyRow> pen_;          // rows with logits edits
@@ -437,15 +469,15 @@ Engine::~Engine() {
   cudaSetDevice(cfg.device);
   if (stream) cudaStreamSynchronize(stream);
   void* frees[] = {weights_blob, res, x, normed, qkv, attn, gu, act, last_hidden, logits, sampled, gemm_ws,
-                   gemm_counters, kv, cand, attn_ws, lp_dev, lp_ids_dev, pen_recs, pen_lens, pen_save};
+                   gemm_counters, kv, cand, attn_ws, lp_dev, lp_ids_dev, pen_recs, pen_lens, pen_save, prompt_hidden,
+                   prompt_logits, plp_f_dev, plp_ids_dev, plp_rank_dev};
   for (void* p : frees)
     if (p) cudaFree(p);
   for (auto p : stage_dev)
     if (p) cudaFree(p);
-  if (stage_host) cudaFreeHost(stage_host);
-  if (sampled_host) cudaFreeHost(sampled_host);
-  if (lp_host) cudaFreeHost(lp_host);
-  if (lp_ids_host) cudaFreeHost(lp_ids_host);
+  void* host_frees[] = {stage_host, sampled_host, lp_host, lp_ids_host, plp_f_host, plp_ids_host, plp_rank_host};
+  for (void* p : host_frees)
+    if (p) cudaFreeHost(p);
   if (ev0) cudaEventDestroy(ev0);
   if (ev1) cudaEventDestroy(ev1);
   if (stream) cudaStreamDestroy(stream);
@@ -655,10 +687,27 @@ int Engine::alloc_all() {
   CK(cudaMemsetAsync(pen_lens, 0, static_cast<size_t>(Scap) * sizeof(int), stream));
   for (int i = Scap - 1; i >= 0; --i) pen_free.push_back(i);
 
+  // ---- prompt-logprob scratch and records, likewise after the KV pool.  A group of 512 rows reads the lm_head once for
+  // 512 rows (compute-bound) and keeps the scratch at 512 * V bf16 (131 MB at Llama-3's vocabulary).
+  plp_G = std::min(Tcap, 512);
+  CK(cudaMalloc(&prompt_hidden, static_cast<size_t>(plp_G) * H * 2));
+  CK(cudaMalloc(&prompt_logits, static_cast<size_t>(plp_G) * V * 2));
+  CK(cudaMemset(prompt_hidden, 0, static_cast<size_t>(plp_G) * H * 2));
+  CK(cudaMalloc(&plp_f_dev, static_cast<size_t>(Tcap) * (1 + kMaxLogprobs) * sizeof(float)));
+  CK(cudaMalloc(&plp_ids_dev, static_cast<size_t>(Tcap) * kMaxLogprobs * sizeof(int)));
+  CK(cudaMalloc(&plp_rank_dev, static_cast<size_t>(Tcap) * sizeof(int)));
+  CK(cudaMallocHost(&plp_f_host, static_cast<size_t>(Tcap) * (1 + kMaxLogprobs) * sizeof(float)));
+  CK(cudaMallocHost(&plp_ids_host, static_cast<size_t>(Tcap) * kMaxLogprobs * sizeof(int32_t)));
+  CK(cudaMallocHost(&plp_rank_host, static_cast<size_t>(Tcap) * sizeof(int32_t)));
+  // bf16 logits [plp_G, V] of the last group of prompt-logprob rows of the last step
+  tensors["step.prompt_logits"] = {prompt_logits, static_cast<size_t>(plp_G) * V * 2};
+  for (int i = 0; i < kGemmNumBlockN; ++i)
+    if (gemm_make_x_map(&xm_phid.m[i], prompt_hidden, plp_G, H, H, bns[i])) return cuda_fail("gemm_make_x_map", -2);
+
   // ---- step input ring
   max_blocks_per_seq = (cfg.max_model_len + kPage - 1) / kPage;
   step_words_cap = 3 * Tcap + Scap + 4 * Scap + 4 * (Tcap / 16 + Scap + 1) + Scap * max_blocks_per_seq + 7 * Scap + 2 * Scap +
-                   8 * Scap + 64;
+                   8 * Scap + 3 * Tcap + 64;
   static_assert(sizeof(SampleRow) == 7 * sizeof(int32_t), "SampleRow is 7 words of the step input");
   static_assert(sizeof(PenaltyRow) == 8 * sizeof(int32_t), "PenaltyRow is 8 words of the step input");
   ring_n = std::max(1, cfg.record_steps) + 1;  // last slot = scratch for unrecorded steps
@@ -835,6 +884,28 @@ int Engine::forward(const StepMeta& m, int32_t* dbuf, bool all_logits, bf16* log
       launched(1);
     }
   }
+  // prompt-logprob rows, plp_G at a time: gathered final norm (the residual is not written back, so the rows can be read
+  // again), plain lm_head into the scratch, then the ranked log-softmax into the step's records.  Only scratch is
+  // written, so a replay changes nothing a later step reads.
+  if (!all_logits && m.n_plp > 0) {
+    const int* ptok = dbuf + m.off_plp;
+    const int* ptgt = ptok + m.n_plp;
+    const int* pn = ptgt + m.n_plp;
+    for (int g0 = 0; g0 < m.n_plp && !rc; g0 += plp_G) {
+      const int n = std::min(plp_G, m.n_plp - g0);
+      P(B200_K_NORM); norm(final_norm, prompt_hidden, ptok + g0, n); Q();
+      Gemm3Params p = proj(p_lm, GEMM3_EPI_PLAIN);
+      p.out = prompt_logits; p.ldo = V;
+      P(B200_K_GEMM_LM); rc |= launch_proj(p, xm_phid, n); Q();
+      P(B200_K_ARGMAX);
+      rc |= logprobs_rows(prompt_logits, V, V, nullptr, pn + g0, n, ptgt + g0,
+                          plp_f_dev + static_cast<size_t>(g0) * (1 + kMaxLogprobs), 1 + kMaxLogprobs,
+                          plp_f_dev + static_cast<size_t>(g0) * (1 + kMaxLogprobs) + 1, 1 + kMaxLogprobs,
+                          plp_ids_dev + static_cast<size_t>(g0) * kMaxLogprobs, stream, plp_rank_dev + g0);
+      Q();
+      launched(1);
+    }
+  }
   if (rc) return cuda_fail("forward(head)", -2);
   return 0;
 }
@@ -879,6 +950,7 @@ void Engine::publish() {
   for (auto& p : pending_pub) {
     {
       std::lock_guard<std::mutex> lk(p.s->m);
+      p.s->plp_out.insert(p.s->plp_out.end(), pending_plp.begin() + p.plp0, pending_plp.begin() + p.plp0 + p.n_plp);
       if (p.has_tok) p.s->out.push_back(p.tok);
       if (p.lp >= 0) p.s->lp_out.push_back(pending_lp[p.lp]);
       if (p.code) p.s->finished = p.code;
@@ -887,12 +959,15 @@ void Engine::publish() {
   }
   pending_pub.clear();
   pending_lp.clear();
+  pending_plp.clear();
 }
 
 void Engine::admit_prefix(Seq& s) {
-  // hash-chained full-block lookup; a hit may cover at most len-1 tokens (kv_cache_manager.py:210-222)
+  // hash-chained full-block lookup; a hit may cover at most len-1 tokens (kv_cache_manager.py:210-222).  A request with
+  // prompt logprobs needs the logits of every prompt position, so it reads no cached block (vLLM's
+  // skip_reading_prefix_cache); it still publishes its own blocks.
   const int len = static_cast<int>(s.toks.size());
-  const int nfull = (len - 1) / kPage;
+  const int nfull = s.prompt_logprobs >= 0 ? 0 : (len - 1) / kPage;
   uint64_t parent = 0;
   int hit = 0;
   for (int b = 0; b < nfull; ++b) {
@@ -1041,6 +1116,9 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
   lp_rows_.clear();
   lp_n_.clear();
   pen_.clear();
+  plp_tok_.clear();
+  plp_tgt_.clear();
+  plp_n_.clear();
   bool any_sampled = false, any_minp = false;
   int32_t* h = stage_host;
   m.off_ids = 0; m.off_pos = m.T; m.off_slots = 2 * m.T;
@@ -1054,6 +1132,20 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
       h[m.off_ids + tok + j] = s.toks[p];
       h[m.off_pos + tok + j] = p;
       h[m.off_slots + tok + j] = s.blocks[p / kPage] * kPage + (p % kPage);
+    }
+    if (s.prompt_logprobs >= 0) {
+      // positions p in [p0, p0 + n) that still need a record: the row at p gives prompt token p + 1's.  The last prompt
+      // position is the sampled row, whose record (if asked for) is the first generated token's.
+      const int lo = std::max(p0, s.plp_done), hi = std::min(p0 + n, s.n_prompt - 1);
+      for (int p = lo; p < hi; ++p) {
+        plp_tok_.push_back(tok + p - p0);
+        plp_tgt_.push_back(s.toks[p + 1]);
+        plp_n_.push_back(s.prompt_logprobs);
+      }
+      if (hi > lo) {
+        sched[si].n_plp = hi - lo;
+        s.plp_done = hi;
+      }
     }
     if (n == 1) {
       dwork_.push_back({tok, 1, p0, si});
@@ -1124,6 +1216,14 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
     memcpy(h + w + m.n_lp, lp_n_.data(), lp_n_.size() * 4);
     w += 2 * m.n_lp;
   }
+  m.n_plp = static_cast<int>(plp_tok_.size());
+  if (m.n_plp > 0) {   // and prompt logprobs
+    m.off_plp = w;
+    memcpy(h + w, plp_tok_.data(), plp_tok_.size() * 4);
+    memcpy(h + w + m.n_plp, plp_tgt_.data(), plp_tgt_.size() * 4);
+    memcpy(h + w + 2 * m.n_plp, plp_n_.data(), plp_n_.size() * 4);
+    w += 3 * m.n_plp;
+  }
   m.words = w;
   if (w > step_words_cap) {
     set_error("step staging overflow (%d > %d words)", w, step_words_cap);
@@ -1159,6 +1259,11 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
     CK(cudaMemcpyAsync(lp_host, lp_dev, static_cast<size_t>(m.n_lp) * (1 + kMaxLogprobs) * sizeof(float), cudaMemcpyDeviceToHost, stream));
     CK(cudaMemcpyAsync(lp_ids_host, lp_ids_dev, static_cast<size_t>(m.n_lp) * kMaxLogprobs * sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
   }
+  if (m.n_plp) {
+    CK(cudaMemcpyAsync(plp_f_host, plp_f_dev, static_cast<size_t>(m.n_plp) * (1 + kMaxLogprobs) * sizeof(float), cudaMemcpyDeviceToHost, stream));
+    CK(cudaMemcpyAsync(plp_ids_host, plp_ids_dev, static_cast<size_t>(m.n_plp) * kMaxLogprobs * sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
+    CK(cudaMemcpyAsync(plp_rank_host, plp_rank_dev, static_cast<size_t>(m.n_plp) * sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
+  }
   f->t_launched = timing ? now_s() : 0.0;
   f->words = w;
   *mp = m;
@@ -1174,7 +1279,7 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
   float ms = 0.f;
   cudaEventElapsedTime(&ms, ev0, ev1);
 
-  int ri = 0, li = 0;
+  int ri = 0, li = 0, pi = 0;
   int64_t gen = 0;
   bool any_done = false;
   for (int si = 0; si < m.nseq; ++si) {
@@ -1189,7 +1294,21 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
       s.chain_uid = pool.publish(s.blocks[b], s.chain_uid, &s.toks[static_cast<size_t>(b) * kPage]);
       ++s.n_published;
     }
-    if (!samples) continue;
+    // prompt records come back in step order; they are published with (or before) the first generated token
+    const int plp0 = static_cast<int>(pending_plp.size()), n_plp = f.sched[si].n_plp;
+    for (int k = 0; k < n_plp; ++k, ++pi) {
+      PromptLogprobRecord r;
+      const float* src = plp_f_host + static_cast<size_t>(pi) * (1 + kMaxLogprobs);
+      r.r.lp = src[0];
+      memcpy(r.r.top_lp, src + 1, sizeof(r.r.top_lp));
+      memcpy(r.r.top_ids, plp_ids_host + static_cast<size_t>(pi) * kMaxLogprobs, sizeof(r.r.top_ids));
+      r.rank = plp_rank_host[pi];
+      pending_plp.push_back(r);
+    }
+    if (!samples) {
+      if (n_plp > 0) pending_pub.push_back({sp, 0, false, 0, -1, plp0, n_plp});
+      continue;
+    }
     const int32_t t = sampled_host[ri++];
     s.toks.push_back(t);
     ++s.n_generated;
@@ -1210,7 +1329,7 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
       lp = static_cast<int>(pending_lp.size());
       pending_lp.push_back(r);
     }
-    pending_pub.push_back({sp, t, true, code, lp});
+    pending_pub.push_back({sp, t, true, code, lp, plp0, n_plp});
     if (code) {
       release_blocks(s);
       s.leaving = true;
@@ -1231,7 +1350,8 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
     stats.total_device_us += ms * 1000.0;
     stats.last_step_tokens = m.T;
     stats.h2d_bytes += static_cast<int64_t>(f.words) * 4;
-    stats.d2h_bytes += static_cast<int64_t>(m.S) * 4 + static_cast<int64_t>(m.n_lp) * (1 + 2 * kMaxLogprobs) * 4;
+    stats.d2h_bytes += static_cast<int64_t>(m.S) * 4 + static_cast<int64_t>(m.n_lp) * (1 + 2 * kMaxLogprobs) * 4 +
+                       static_cast<int64_t>(m.n_plp) * (2 + 2 * kMaxLogprobs) * 4;
     stats.running = static_cast<int>(running.size());
     stats.waiting = static_cast<int>(waiting.size());
     stats.kv_blocks_free = pool.free_count();
@@ -1314,6 +1434,7 @@ void Engine::fail_all() {
   }
   pending_pub.clear();
   pending_lp.clear();
+  pending_plp.clear();
   for (auto& s : all) {
     { std::lock_guard<std::mutex> lk(s->m); s->finished = B200_FINISH_ERROR; }
     s->cv.notify_all();
@@ -1402,6 +1523,8 @@ int b200_submit(b200_engine* e, const int32_t* prompt_ids, int32_t n, const b200
   if (sp && sp->top_k < -1) { set_error("top_k must be >= -1"); return B200_ERR_INVALID; }
   if (sp && (sp->top_logprobs < 0 || sp->top_logprobs > B200_MAX_LOGPROBS)) { set_error("top_logprobs must be in 0..%d", B200_MAX_LOGPROBS); return B200_ERR_INVALID; }
   if (sp && sp->top_logprobs > 0 && !sp->logprobs) { set_error("top_logprobs needs logprobs"); return B200_ERR_INVALID; }
+  if (sp && (sp->top_prompt_logprobs < 0 || sp->top_prompt_logprobs > B200_MAX_LOGPROBS)) { set_error("top_prompt_logprobs must be in 0..%d", B200_MAX_LOGPROBS); return B200_ERR_INVALID; }
+  if (sp && sp->top_prompt_logprobs > 0 && !sp->prompt_logprobs) { set_error("top_prompt_logprobs needs prompt_logprobs"); return B200_ERR_INVALID; }
   for (int i = 0; i < n; ++i) if (prompt_ids[i] < 0 || prompt_ids[i] >= g.V) { set_error("token id out of range"); return B200_ERR_INVALID; }
   // logits edits: vLLM's SamplingParams._verify_args ranges (repetition_penalty 0 is "off" at this ABI)
   if (sp) {
@@ -1430,6 +1553,7 @@ int b200_submit(b200_engine* e, const int32_t* prompt_ids, int32_t n, const b200
     s->top_p = sp->top_p > 0.f ? sp->top_p : 1.f;   // 0 = off at this ABI
     s->top_k = sp->top_k > 0 ? sp->top_k : 0;
     s->top_logprobs = sp->logprobs ? sp->top_logprobs : -1;
+    s->prompt_logprobs = sp->prompt_logprobs ? sp->top_prompt_logprobs : -1;
     s->min_p = sp->temperature >= 1e-5f ? sp->min_p : 0.f;   // greedy rows ignore min_p, as in vLLM
     s->presence = sp->presence_penalty;
     s->frequency = sp->frequency_penalty;
@@ -1522,6 +1646,32 @@ int b200_poll_logprobs(b200_engine* e, uint64_t req_id, int32_t* out_ids, float*
                        float* out_top_logprob, int32_t cap, int32_t* n_out, int32_t* finished, b200_usage* usage) {
   if (!out_logprob) { set_error("b200_poll_logprobs: bad arguments"); return B200_ERR_INVALID; }
   return poll_impl(e, req_id, out_ids, out_logprob, out_top_ids, out_top_logprob, cap, n_out, finished, usage);
+}
+
+int b200_poll_prompt_logprobs(b200_engine* e, uint64_t req_id, float* out_logprob, int32_t* out_rank, int32_t* out_top_ids,
+                              float* out_top_logprob, int32_t cap, int32_t* n_out) {
+  if (!e || !out_logprob || !out_rank || !out_top_ids || !out_top_logprob || !n_out) { set_error("b200_poll_prompt_logprobs: bad arguments"); return B200_ERR_INVALID; }
+  Engine& g = e->impl;
+  std::shared_ptr<Seq> s;
+  {
+    std::lock_guard<std::mutex> lk(g.mu_);
+    s = find_req(g, req_id);
+  }
+  if (!s) { set_error("unknown request %llu", static_cast<unsigned long long>(req_id)); return B200_ERR_NOT_FOUND; }
+  if (s->prompt_logprobs < 0) { set_error("request %llu was submitted without prompt_logprobs", static_cast<unsigned long long>(req_id)); return B200_ERR_INVALID; }
+  const int want = s->n_prompt - 1;
+  if (cap < want) { set_error("b200_poll_prompt_logprobs: cap %d < %d records", cap, want); return B200_ERR_INVALID; }
+  std::lock_guard<std::mutex> lk(s->m);
+  const int n = static_cast<int>(s->plp_out.size()) == want ? want : 0;
+  for (int k = 0; k < n; ++k) {
+    const PromptLogprobRecord& r = s->plp_out[k];
+    out_logprob[k] = r.r.lp;
+    out_rank[k] = r.rank;
+    memcpy(out_top_ids + static_cast<size_t>(k) * kMaxLogprobs, r.r.top_ids, s->prompt_logprobs * sizeof(int32_t));
+    memcpy(out_top_logprob + static_cast<size_t>(k) * kMaxLogprobs, r.r.top_lp, s->prompt_logprobs * sizeof(float));
+  }
+  *n_out = n;
+  return 0;
 }
 
 int b200_wait(b200_engine* e, uint64_t req_id, int64_t timeout_us) {

@@ -78,10 +78,11 @@ int penalize_update(const PenaltyRow* rows, int n, const int* sampled, PenaltyRe
 // Log-probabilities (sampling.cu; vLLM's raw_logprobs) of n rows of bf16 logits ([., ld], ld % 8 == 0): row i is
 // r = rows ? rows[i] : i, its N = clamp(top_n[i], 0, min(V, kMaxLogprobs)).  lp[i * lp_ld] gets the log-probability of
 // tokens[r]; top_lp[i * top_lp_ld + j] and top_ids[i * kMaxLogprobs + j], j < N, the N most likely tokens (by logit,
-// lowest id on ties).  Entries past N are not written.  Every pointer is device memory.
+// lowest id on ties).  Entries past N are not written.  rank (optional): rank[i] = the number of tokens whose logit is >=
+// that of tokens[r] (vLLM's prompt-logprob rank).  Every pointer is device memory.
 constexpr int kMaxLogprobs = 20;
 int logprobs_rows(const void* logits, int ld, int V, const int* rows, const int* top_n, int n, const int* tokens, float* lp,
-                  int lp_ld, float* top_lp, int top_lp_ld, int* top_ids, cudaStream_t st);
+                  int lp_ld, float* top_lp, int top_lp_ld, int* top_ids, cudaStream_t st, int* rank = nullptr);
 
 // One unit of attention work: q_count query tokens of one sequence starting at row q_tok0 of the
 // step's token batch; the first of them sits at absolute position q_pos0 in the sequence.

@@ -372,18 +372,23 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const uint16_t* __rest
 //   4 collect the keys above the N-th key and the ties at it, then rank the <= 20 + kTieCap entries.
 // When more than kTieCap tokens tie at the N-th key they are taken in id order by a chunked ballot scan instead (slow, rare
 // on real logits).  Rows with N = 0 stop after pass 2 and the sampled token's gather.
+// kRank adds the token's rank, vLLM's batched_count_greater_than: the number of tokens whose key is >= the token's key
+// (so equal logits share a rank, and -0 / +0 are one key).  It is counted exactly in pass 2, with integer adds whose sum
+// does not depend on order, so no extra pass reads the row; N = 0 rows get it too.  Without kRank the kernel is the same
+// code as before ranks existed.
 constexpr int kTieCap = 64;
 constexpr int kCntSmem = 256 * 32 * 4;   // 32 per-lane copies of a 256-bin count histogram: 32 KiB
 
+template <bool kRank>
 __global__ void __launch_bounds__(kThreads) logprobs_kernel(const uint16_t* __restrict__ logits, int ld, int V,
                                                             const int* __restrict__ rows, const int* __restrict__ top_n,
                                                             const int* __restrict__ tokens, float* __restrict__ out_lp,
                                                             int lp_ld, float* __restrict__ out_top_lp, int top_lp_ld,
-                                                            int* __restrict__ out_top_ids) {
+                                                            int* __restrict__ out_top_ids, int* __restrict__ out_rank) {
   __shared__ uint32_t cnt_hi[256], cnt_lo[256];
   __shared__ float sred[32];
   __shared__ int swc[32];
-  __shared__ uint32_t s_kmax, s_thr, s_count, s_above, s_need, s_ties;
+  __shared__ uint32_t s_kmax, s_thr, s_count, s_above, s_need, s_ties, s_rank;
   __shared__ float s_logz;
   __shared__ uint32_t ent_key[kMaxLogprobs + kTieCap];
   __shared__ int ent_id[kMaxLogprobs + kTieCap];
@@ -394,6 +399,11 @@ __global__ void __launch_bounds__(kThreads) logprobs_kernel(const uint16_t* __re
   const uint16_t* row = logits + static_cast<size_t>(r) * ld;
   const int N = min(max(top_n[i], 0), min(V, kMaxLogprobs));
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  uint32_t kt = 0;   // kRank: the token's key (above every key when the id is out of range: rank 0)
+  if (kRank) {
+    const int t = tokens[r];
+    kt = (t >= 0 && t < V) ? key_of(row[t]) : 0x10000u;
+  }
 
   // pass 1: row max, as a key
   uint32_t km = 0;
@@ -401,6 +411,7 @@ __global__ void __launch_bounds__(kThreads) logprobs_kernel(const uint16_t* __re
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) km = max(km, __shfl_xor_sync(0xffffffffu, km, o));
   if (threadIdx.x == 0) s_kmax = 0;
+  if (kRank && threadIdx.x == 0) s_rank = 0;
   if (N > 0)
     for (int j = threadIdx.x; j < 256 * 32; j += kThreads) priv_cnt[j] = 0;
   __syncthreads();
@@ -410,10 +421,17 @@ __global__ void __launch_bounds__(kThreads) logprobs_kernel(const uint16_t* __re
 
   // pass 2: sum of exp (fixed order) and the high-byte histogram (per-lane copies: no bank collisions within a warp)
   float acc = 0.f;
+  uint32_t ge = 0;   // kRank: tokens with key >= kt
   visit_row(row, V, [&](int, uint32_t b) {
     acc = __fadd_rn(acc, expf(__fsub_rn(bf16_bits_to_f32(b), m)));
     if (N > 0) atomicAdd(&priv_cnt[(key_of(b) >> 8) * 32 + lane], 1u);
+    if (kRank) ge += key_of(b) >= kt ? 1u : 0u;
   });
+  if (kRank) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) ge += __shfl_xor_sync(0xffffffffu, ge, o);
+    if (lane == 0) atomicAdd(&s_rank, ge);
+  }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) acc = __fadd_rn(acc, __shfl_xor_sync(0xffffffffu, acc, o));
   if (lane == 0) sred[warp] = acc;
@@ -431,6 +449,7 @@ __global__ void __launch_bounds__(kThreads) logprobs_kernel(const uint16_t* __re
   if (threadIdx.x == 0) {
     const int t = tokens[r];
     out_lp[static_cast<size_t>(i) * lp_ld] = (t >= 0 && t < V) ? lp_of_key(key_of(row[t])) : __int_as_float(0x7fc00000);
+    if (kRank) out_rank[i] = static_cast<int>(s_rank);
   }
   if (N == 0) return;
 
@@ -532,11 +551,15 @@ __global__ void __launch_bounds__(kThreads) logprobs_kernel(const uint16_t* __re
 }  // namespace
 
 int logprobs_rows(const void* logits, int ld, int V, const int* rows, const int* top_n, int n, const int* tokens, float* lp,
-                  int lp_ld, float* top_lp, int top_lp_ld, int* top_ids, cudaStream_t st) {
+                  int lp_ld, float* top_lp, int top_lp_ld, int* top_ids, cudaStream_t st, int* rank) {
   if (n <= 0) return 0;
   if (V < 1 || ld < V || ld % 8 || (reinterpret_cast<uintptr_t>(logits) & 15)) return -1;
-  launch_pdl(logprobs_kernel, dim3(n), dim3(kThreads), kCntSmem, st, static_cast<const uint16_t*>(logits), ld, V, rows, top_n,
-             tokens, lp, lp_ld, top_lp, top_lp_ld, top_ids);
+  if (rank)
+    launch_pdl(logprobs_kernel<true>, dim3(n), dim3(kThreads), kCntSmem, st, static_cast<const uint16_t*>(logits), ld, V, rows,
+               top_n, tokens, lp, lp_ld, top_lp, top_lp_ld, top_ids, rank);
+  else
+    launch_pdl(logprobs_kernel<false>, dim3(n), dim3(kThreads), kCntSmem, st, static_cast<const uint16_t*>(logits), ld, V, rows,
+               top_n, tokens, lp, lp_ld, top_lp, top_lp_ld, top_ids, rank);
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 

@@ -51,6 +51,7 @@ struct Server {
   bool sampling = false;   // b200_server_config.enable_sampling: serve temperature >= 1e-5 (else greedy only)
   bool logprobs = false;   // b200_server_config.enable_logprobs: serve logprobs / top_logprobs (else a 400)
   bool edits = false;      // b200_server_config.enable_logits_processors: serve penalties, min_p, min_tokens, logit_bias
+  bool prompt_lp = false;  // b200_server_config.enable_prompt_logprobs: serve prompt_logprobs and completions echo
   // optional real tokenizer (b200_server_set_tokenizer): a checkpoint's tokenizer.json instead of the synthetic byte/word ids
   const b200_tokenizer* real_tok = nullptr;
 
@@ -167,6 +168,9 @@ struct ParsedRequest {
   bool has_seed = false;
   int64_t seed = 0;
   int logprobs = -1;   // -1: none; else the number of most likely tokens per position (chat top_logprobs, completions logprobs)
+  // read only when the server serves them: prompt_logprobs (-1: absent) and completions echo
+  int prompt_logprobs = -1;
+  bool echo = false;
   std::vector<int32_t> stop_ids;
   // logits edits (b200_sampling): read only when the server serves them
   double presence = 0.0, frequency = 0.0, repetition = 1.0, min_p = 0.0;
@@ -318,6 +322,29 @@ int parse_request(Server& sv, const std::string& path, const std::string& ctype,
       return 400;
     }
   }
+  if (sv.prompt_lp) {
+    // vLLM's checks, in its order (CompletionRequest / ChatCompletionRequest check_logprobs, then SamplingParams
+    // _validate_logprobs at max_logprobs 20); null is absent.  Chat echo keeps its 400 below: it means something else there.
+    std::string bad_plp;
+    if (const JVal* v = root.get("prompt_logprobs"); v && v->type != JVal::Null) {
+      if (v->type != JVal::Num || v->num != std::floor(v->num) || std::fabs(v->num) > 2147483647.0) {
+        bad_plp = "prompt_logprobs must be an integer";
+      } else {
+        const int n = static_cast<int>(v->num);
+        if (pr->stream && (n > 0 || n == -1)) bad_plp = "`prompt_logprobs` are not available when `stream=True`.";
+        else if (n < 0 && n != -1) bad_plp = "`prompt_logprobs` must be a positive value or -1.";
+        else if (n == -1 || n > B200_MAX_LOGPROBS)
+          bad_plp = "Requested prompt logprobs of " + std::to_string(n == -1 ? sv.tok.vocab : n) + ", which is greater than max allowed: " +
+                    std::to_string(B200_MAX_LOGPROBS);
+        else pr->prompt_logprobs = n;
+      }
+    }
+    if (const JVal* v = root.get("echo"); !pr->chat && v && v->type == JVal::Bool) pr->echo = v->b;
+    if (!bad_plp.empty()) {
+      *err = "bad request: " + bad_plp;
+      return 400;
+    }
+  }
   if (sv.edits) {
     // vLLM's SamplingParams ranges (sampling_params.py _verify_args, _validate_logit_bias); null is absent
     std::string bad_ed;
@@ -386,11 +413,11 @@ int parse_request(Server& sv, const std::string& path, const std::string& ctype,
   const char* bad = nullptr;
   if (num_of("n", 1) > 1) bad = "n > 1";
   else if (num_of("best_of", 1) > 1) bad = "best_of > 1";
-  else if (!sv.logprobs && (truthy("logprobs") || truthy("top_logprobs") || truthy("prompt_logprobs"))) bad = "logprobs";
-  else if (truthy("prompt_logprobs")) bad = "prompt_logprobs";
+  else if (!sv.logprobs && (truthy("logprobs") || truthy("top_logprobs") || (!sv.prompt_lp && truthy("prompt_logprobs")))) bad = "logprobs";
+  else if (!sv.prompt_lp && truthy("prompt_logprobs")) bad = "prompt_logprobs";
   else if (!pr->chat && truthy("top_logprobs")) bad = "top_logprobs on completions (use logprobs)";
   else if (nonempty("stop")) bad = "stop strings (use stop_token_ids)";
-  else if (truthy("echo")) bad = "echo";
+  else if ((pr->chat || !sv.prompt_lp) && truthy("echo")) bad = "echo";
   else if (nonempty("suffix")) bad = "suffix";
   else if (!sv.edits && (num_of("presence_penalty", 0) != 0 || num_of("frequency_penalty", 0) != 0 || num_of("repetition_penalty", 1) != 1)) bad = "sampling penalties";
   else if (!sv.edits && nonempty("logit_bias")) bad = "logit_bias";
@@ -424,6 +451,8 @@ struct LpRecord {
   int32_t id;
   float lp;
   std::vector<std::pair<int32_t, float>> top;   // the request's N most likely tokens
+  bool none = false;   // the first prompt position of an echo: no record (null entries)
+  int32_t rank = 0;    // prompt records: the token's rank
 };
 
 // the shortest decimal that reads back as the same fp32, after vLLM's clamp at -9999.0
@@ -470,20 +499,26 @@ std::string chat_lp_content(const LpRecord& r, const Str& token_str) {
 }
 
 // completions "logprobs" of consecutive tokens, text_offset counted from `offset`: the first N + 1 entries of each position
-// as a {token string: logprob} object (a string that repeats keeps its first place and takes the later value, as a dict)
+// as a {token string: logprob} object (a string that repeats keeps its first place and takes the later value, as a dict).
+// An echoed prompt's first position has null entries.
 template <class Str>
-std::string completion_lp(const std::vector<LpRecord>& rs, size_t offset, const Str& token_str) {
+std::string completion_lp(const std::vector<LpRecord>& rs, size_t offset, const Str& token_str, int n) {
   std::string off = "[", lps = "[", toks = "[", tops = "[";
   for (size_t k = 0; k < rs.size(); ++k) {
     const std::string s = token_str(rs[k].id);
     const char* sep = k ? "," : "";
     off += sep + std::to_string(offset);
     offset += utf8_len(s);
-    lps += sep + lp_num(rs[k].lp);
     toks += sep + json_str(s);
+    if (rs[k].none) {
+      lps += sep + std::string("null");
+      tops += sep + std::string("null");
+      continue;
+    }
+    lps += sep + lp_num(rs[k].lp);
     const auto e = lp_entries(rs[k]);
     std::vector<std::pair<std::string, float>> d;
-    for (size_t j = 0; j <= rs[k].top.size() && j < e.size(); ++j) {
+    for (size_t j = 0; j <= static_cast<size_t>(n) && j < e.size(); ++j) {
       std::string key = token_str(e[j].first);
       auto it = std::find_if(d.begin(), d.end(), [&](const std::pair<std::string, float>& x) { return x.first == key; });
       if (it != d.end()) it->second = e[j].second;
@@ -494,6 +529,32 @@ std::string completion_lp(const std::vector<LpRecord>& rs, size_t offset, const 
     tops += "}";
   }
   return "{\"text_offset\":" + off + "],\"token_logprobs\":" + lps + "],\"tokens\":" + toks + "],\"top_logprobs\":" + tops + "]}";
+}
+
+// vLLM's "prompt_logprobs" list: null for the first prompt position, then per position a {"<id>": {logprob, rank,
+// decoded_token}} object built as vllm/logprobs.py append_logprobs_for_next_position does (the prompt token with its rank
+// first, then the top N with ranks 1..N, a repeated id keeping its first place and taking the later entry); -inf is -9999
+// (clamp_prompt_logprobs)
+template <class Str>
+std::string prompt_lp_json(const std::vector<LpRecord>& rs, const Str& token_str) {
+  auto num = [](float v) { return std::isinf(v) && v < 0 ? std::string("-9999.0") : lp_num(v); };
+  std::string o = "[null";
+  for (const LpRecord& r : rs) {
+    struct E { int32_t id; float lp; int32_t rank; };
+    std::vector<E> d{{r.id, r.lp, r.rank}};
+    for (size_t j = 0; j < r.top.size(); ++j) {
+      const E e{r.top[j].first, r.top[j].second, static_cast<int32_t>(j + 1)};
+      auto it = std::find_if(d.begin(), d.end(), [&](const E& x) { return x.id == e.id; });
+      if (it != d.end()) *it = e;
+      else d.push_back(e);
+    }
+    o += ",{";
+    for (size_t j = 0; j < d.size(); ++j)
+      o += (j ? ",\"" : "\"") + std::to_string(d[j].id) + "\":{\"logprob\":" + num(d[j].lp) + ",\"rank\":" + std::to_string(d[j].rank) +
+           ",\"decoded_token\":" + json_str(token_str(d[j].id)) + "}";
+    o += "}";
+  }
+  return o + "]";
 }
 
 }  // namespace
@@ -550,6 +611,10 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
   for (auto t : ids)
     if (t < 0 || t >= sv.tok.vocab) return send_error(w, 400, "bad request: prompt token id out of range");
   int max_tokens = pr.max_tokens > 0 ? pr.max_tokens : sv.default_max_tokens;
+  // echo with max_tokens 0 returns the prompt only; vLLM generates one token for it and drops it (completion/protocol.py
+  // to_sampling_params), and counts that token in the usage
+  const bool echo_only = pr.echo && pr.max_tokens == 0;
+  if (echo_only) max_tokens = 1;
   if (static_cast<int>(ids.size()) + 1 > sv.max_model_len)
     return send_error(w, 400, "bad request: prompt is longer than the model's context length");
   max_tokens = std::min(max_tokens, sv.max_model_len - static_cast<int>(ids.size()));
@@ -571,6 +636,21 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
       --s.active[m];
     }
   } dec{sv, pr.requested_model};
+
+  // prompt logprobs: asked for, or echo with logprobs (which then covers the prompt with the same N)
+  const int plp_n = pr.prompt_logprobs >= 0 ? pr.prompt_logprobs : (pr.echo && pr.logprobs >= 0 ? pr.logprobs : -1);
+  // the echoed prompt text: the request's own text, or the decoded ids of a token-id prompt
+  std::string echo_text;
+  if (pr.echo && !pr.prompt_is_ids) {
+    echo_text = pr.prompt_text;
+  } else if (pr.echo && sv.real_tok) {
+    DetokStream d;
+    d.tok = sv.real_tok;
+    for (auto t : ids) echo_text += d.push(t);
+    echo_text += d.flush();
+  } else if (pr.echo) {
+    for (auto t : ids) echo_text += sv.tok.piece(t);
+  }
 
   const std::string id = (pr.chat ? "chatcmpl-" : "cmpl-") + hex_id(32);
   const long created = static_cast<long>(time(nullptr));
@@ -615,6 +695,8 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
     sp.num_logit_bias = static_cast<int>(pr.bias_ids.size());
     sp.logit_bias_ids = pr.bias_ids.empty() ? nullptr : pr.bias_ids.data();
     sp.logit_bias_values = pr.bias_values.empty() ? nullptr : pr.bias_values.data();
+    sp.prompt_logprobs = plp_n >= 0 ? 1 : 0;
+    sp.top_prompt_logprobs = std::max(plp_n, 0);
     std::vector<int32_t> stops = pr.stop_ids;
     if (sv.real_tok && !pr.ignore_eos) {   // the checkpoint's end-of-turn / end-of-text tokens end the generation
       for (const char* name : {"<|eot_id|>", "<|end_of_text|>"}) {
@@ -632,6 +714,15 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
 
     std::vector<int32_t> all;
     std::vector<LpRecord> all_lp;
+    std::vector<LpRecord> prompt_lp;   // the prompt records (plp_n >= 0), read with the first token
+    bool have_plp = false, echoed = false;
+    // an echo's leading records: the first prompt token's null entry, then the prompt records
+    auto echo_recs = [&] {
+      std::vector<LpRecord> e{LpRecord{ids[0], 0.f, {}}};
+      e[0].none = true;
+      e.insert(e.end(), prompt_lp.begin(), prompt_lp.end());
+      return e;
+    };
     const bool want_lp = pr.logprobs >= 0;
     // a token's string in logprobs: the single-id lossy decode (vLLM's tokenizer.decode([id])), or the synthetic piece
     auto token_str = [&](int32_t id) { return sv.real_tok ? tokenizer_token_text(sv.real_tok, id) : sv.tok.piece(id); };
@@ -657,6 +748,21 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
                                 : b200_poll(eng, rid, buf, 256, &n, &fin, &usage);
         if (prc) { failed = true; break; }
         if (fin == B200_FINISH_ERROR && !sent_any) { failed = true; break; }
+        if (plp_n >= 0 && !have_plp && n > 0) {   // published no later than the first token
+          const int np = static_cast<int>(ids.size()) - 1;
+          std::vector<float> plv(std::max(np, 1)), ptl(static_cast<size_t>(std::max(np, 1)) * B200_MAX_LOGPROBS);
+          std::vector<int32_t> prk(std::max(np, 1)), pti(static_cast<size_t>(std::max(np, 1)) * B200_MAX_LOGPROBS);
+          int got = 0;
+          if (b200_poll_prompt_logprobs(eng, rid, plv.data(), prk.data(), pti.data(), ptl.data(), np, &got) || got != np) { failed = true; break; }
+          for (int k = 0; k < np; ++k) {
+            LpRecord r{ids[k + 1], plv[k], {}};
+            r.rank = prk[k];
+            for (int j = 0; j < plp_n; ++j)
+              r.top.emplace_back(pti[static_cast<size_t>(k) * B200_MAX_LOGPROBS + j], ptl[static_cast<size_t>(k) * B200_MAX_LOGPROBS + j]);
+            prompt_lp.push_back(std::move(r));
+          }
+          have_plp = true;
+        }
         std::vector<LpRecord> recs;
         for (int i = 0; want_lp && i < n; ++i) {
           LpRecord r{buf[i], lpv[i], {}};
@@ -677,10 +783,21 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
             // one chunk per token; with a real tokenizer a chunk carries the text that token completed (possibly none: a
             // token may end inside a UTF-8 sequence), and the last chunk also what was still held
             const std::string text = sv.real_tok ? detok.push(buf[i]) + (last ? detok.flush() : std::string()) : sv.tok.piece(buf[i]);
-            const std::string piece = json_str(text);
+            std::string piece = json_str(text);
             std::string lpj = "null";
             if (want_lp && pr.chat) lpj = "{\"content\":[" + chat_lp_content(recs[i], token_str) + "]}";
-            else if (want_lp) lpj = completion_lp({recs[i]}, text_off, token_str);
+            else if (want_lp) lpj = completion_lp({recs[i]}, text_off, token_str, pr.logprobs);
+            if (pr.echo && !echoed) {
+              // vLLM's first echo chunk: the prompt and its records, then the first token's unless max_tokens was 0.  The
+              // offsets of later chunks count the generated text only, as in vLLM.
+              piece = json_str(echo_text + (echo_only ? std::string() : text));
+              if (want_lp) {
+                std::vector<LpRecord> e = echo_recs();
+                if (!echo_only) e.push_back(recs[i]);
+                lpj = completion_lp(e, 0, token_str, pr.logprobs);
+              }
+              echoed = true;
+            }
             text_off += utf8_len(text);
             if (pr.chat)
               w.write("data: " + head + ",\"choices\":[{\"index\":0,\"delta\":{\"content\":" + piece + "},\"logprobs\":" + lpj + ",\"finish_reason\":" + fr +
@@ -726,6 +843,7 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
       }
       std::string out = "{\"id\":\"" + id + "\",\"object\":\"" + (pr.chat ? "chat.completion" : "text_completion") +
                         "\",\"created\":" + std::to_string(created) + ",\"model\":" + json_str(pr.requested_model) + ",\"choices\":[{\"index\":0,";
+      if (pr.echo) text = echo_text + (echo_only ? std::string() : text);
       if (pr.chat) out += "\"message\":{\"role\":\"assistant\",\"content\":" + json_str(text) + "},";
       else out += "\"text\":" + json_str(text) + ",";
       std::string lpj = "null";
@@ -733,10 +851,17 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
         lpj = "{\"content\":[";
         for (size_t k = 0; k < all_lp.size(); ++k) lpj += (k ? "," : "") + chat_lp_content(all_lp[k], token_str);
         lpj += "]}";
+      } else if (want_lp && pr.echo) {
+        std::vector<LpRecord> e = echo_recs();
+        if (!echo_only) e.insert(e.end(), all_lp.begin(), all_lp.end());
+        lpj = completion_lp(e, 0, token_str, pr.logprobs);
       } else if (want_lp) {
-        lpj = completion_lp(all_lp, 0, token_str);
+        lpj = completion_lp(all_lp, 0, token_str, pr.logprobs);
       }
-      out += "\"logprobs\":" + lpj + ",\"finish_reason\":\"" + finish_str(fin) + "\",\"stop_reason\":null}],\"usage\":" + usage_json(usage) + "}";
+      // vLLM's prompt_logprobs: on the completions choice, at the top level of a chat response
+      const std::string plj = plp_n >= 0 ? ",\"prompt_logprobs\":" + prompt_lp_json(prompt_lp, token_str) : std::string();
+      out += "\"logprobs\":" + lpj + ",\"finish_reason\":\"" + finish_str(fin) + "\",\"stop_reason\":null" + (pr.chat ? "" : plj) +
+             "}],\"usage\":" + usage_json(usage) + (pr.chat ? plj : "") + "}";
       w.begin(200, "application/json");
       w.write(out);
     }
@@ -975,6 +1100,7 @@ int b200_server_create(const b200_server_config* cfg, b200_engine* const* replic
   sv.sampling = cfg->enable_sampling != 0;
   sv.logprobs = cfg->enable_logprobs != 0;
   sv.edits = cfg->enable_logits_processors != 0;
+  sv.prompt_lp = cfg->enable_prompt_logprobs != 0;
   if (b200_router_create(sv.replication, &sv.router)) { delete s; return B200_ERR_INVALID; }
   std::vector<std::string> names;
   std::string ad = cfg->adapters ? cfg->adapters : "";

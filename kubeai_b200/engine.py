@@ -88,10 +88,12 @@ class Engine:
 
     def submit(self, prompt_ids, max_tokens=16, ignore_eos=True, stop_ids=(), temperature=0.0, top_p=1.0, top_k=0,
                seed=None, logprobs=False, top_logprobs=0, min_p=0.0, presence_penalty=0.0, frequency_penalty=0.0,
-               repetition_penalty=1.0, min_tokens=0, logit_bias=None) -> int:
+               repetition_penalty=1.0, min_tokens=0, logit_bias=None, prompt_logprobs=None) -> int:
         """temperature < 1e-5 is greedy; top_k 0 / -1 and top_p 1 are off; seed None = one drawn by the engine.
         logprobs: keep each generated token's log-probability and its top_logprobs (0..20) most likely tokens, read with
-        poll_logprobs.  min_p 0, the penalties 0 (repetition 1), min_tokens 0 and logit_bias None ({id: bias}) are off."""
+        poll_logprobs.  min_p 0, the penalties 0 (repetition 1), min_tokens 0 and logit_bias None ({id: bias}) are off.
+        prompt_logprobs N (0..20): keep each prompt token's log-probability, rank and its position's top N, read with
+        poll_prompt_logprobs; None is off."""
         ids = np.ascontiguousarray(prompt_ids, dtype=np.int32)
         stops = np.ascontiguousarray(stop_ids, dtype=np.int32)
         bias = dict(logit_bias or {})
@@ -107,7 +109,9 @@ class Engine:
                       repetition_penalty=repetition_penalty, min_p=min_p, min_tokens=min_tokens,
                       num_logit_bias=len(bias_ids),
                       logit_bias_ids=bias_ids.ctypes.data_as(C.POINTER(C.c_int32)) if len(bias_ids) else None,
-                      logit_bias_values=bias_vals.ctypes.data_as(C.POINTER(C.c_float)) if len(bias_ids) else None)
+                      logit_bias_values=bias_vals.ctypes.data_as(C.POINTER(C.c_float)) if len(bias_ids) else None,
+                      prompt_logprobs=0 if prompt_logprobs is None else 1,
+                      top_prompt_logprobs=0 if prompt_logprobs is None else prompt_logprobs)
         rid = C.c_uint64()
         check(self._l.b200_submit(self._h, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), C.byref(sp),
                                   C.byref(rid)))
@@ -134,6 +138,23 @@ class Engine:
         return LogprobsPollResult(list(ids[:k]), FINISH[fin.value],
                                   (u.prompt_tokens, u.cached_tokens, u.completion_tokens), lp[:k].copy(),
                                   tid[:k, :top_logprobs].copy(), tlp[:k, :top_logprobs].copy())
+
+    def poll_prompt_logprobs(self, rid: int, n_prompt: int, top_n: int):
+        """The prompt records of a request submitted with prompt_logprobs=top_n, or None until they all exist: (lp
+        float32 [n_prompt - 1], rank int32 [n_prompt - 1], top_ids int32 [n_prompt - 1, top_n], top_lp float32
+        [n_prompt - 1, top_n]); record k is prompt token k + 1's.  Does not drain any token."""
+        cap = max(n_prompt - 1, 0)
+        lp = np.zeros(max(cap, 1), dtype=np.float32)
+        rank = np.zeros(max(cap, 1), dtype=np.int32)
+        tid = np.zeros((max(cap, 1), MAX_LOGPROBS), dtype=np.int32)
+        tlp = np.zeros((max(cap, 1), MAX_LOGPROBS), dtype=np.float32)
+        n = C.c_int32()
+        check(self._l.b200_poll_prompt_logprobs(self._h, rid, lp.ctypes.data_as(C.c_void_p), rank.ctypes.data_as(_PI32),
+                                                tid.ctypes.data_as(_PI32), tlp.ctypes.data_as(C.c_void_p), cap,
+                                                C.byref(n)))
+        if n.value != cap:
+            return None
+        return lp[:cap].copy(), rank[:cap].copy(), tid[:cap, :top_n].copy(), tlp[:cap, :top_n].copy()
 
     def wait(self, rid: int, timeout_s: float = -1.0) -> bool:
         rc = self._l.b200_wait(self._h, rid, int(timeout_s * 1e6) if timeout_s >= 0 else -1)

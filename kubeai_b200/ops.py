@@ -196,6 +196,23 @@ def logprobs(logits, tokens, top_n):
     return lp, top_ids, top_lp
 
 
+def logprobs_rank(logits, tokens, top_n):
+    """logprobs() plus the rank of tokens[s] (b200_op_logprobs_rank): returns (lp, rank int32 [S], top_ids, top_lp); the
+    rank is the number of tokens whose logit is >= tokens[s]'s."""
+    _chk(logits)
+    S, V = logits.shape
+    dev = logits.device
+    tok = torch.as_tensor(np.broadcast_to(np.asarray(tokens, dtype=np.int32), (S,)).copy()).to(dev)
+    n = torch.as_tensor(np.broadcast_to(np.asarray(top_n, dtype=np.int32), (S,)).copy()).to(dev)
+    lp = torch.zeros(S, dtype=torch.float32, device=dev)
+    rank = torch.zeros(S, dtype=torch.int32, device=dev)
+    top_ids = torch.zeros(S, 20, dtype=torch.int32, device=dev)
+    top_lp = torch.zeros(S, 20, dtype=torch.float32, device=dev)
+    check(lib().b200_op_logprobs_rank(_p(logits), logits.stride(0), S, V, _p(tok), _p(n), _p(lp), _p(rank), _p(top_ids),
+                                      _p(top_lp), _stream()))
+    return lp, rank, top_ids, top_lp
+
+
 def paged_attn(qkv, kv_layer, block_tables, work, q_heads, kv_heads, decode: bool, out=None, split: int = 0):
     """qkv: [T, (Hq+2Hkv)*128] (q read from it), work: int32 [n, 4] = (q_tok0, q_count, q_pos0, seq).
     split >= 1 (decode only): split-KV form with that many CTAs per (work item, KV head)."""

@@ -43,11 +43,14 @@ class Server:
     and the server decodes greedily only (the serving shell's behaviour before sampling existed).
     enable_logprobs: serve logprobs / top_logprobs in vLLM's response format; off, they get a 400.
     enable_logits_processors: serve presence / frequency / repetition penalties, min_p, min_tokens and logit_bias; off,
+    they get a 400.
+    enable_prompt_logprobs: serve prompt_logprobs (both routes) and echo (completions) in vLLM's response format; off,
     they get a 400."""
 
     def __init__(self, engines, model="llama-3-8b", adapters=None, strategy=LEAST_LOAD, mean_load_pct=125,
                  replication=256, prefix_char_length=100, max_retries=3, default_max_tokens=256, vocab=128256,
-                 max_model_len=2048, enable_sampling=False, enable_logprobs=False, enable_logits_processors=False):
+                 max_model_len=2048, enable_sampling=False, enable_logprobs=False, enable_logits_processors=False,
+                 enable_prompt_logprobs=False):
         self._l = lib()
         self._engines = list(engines)   # keep alive; entries may be None for parse-path-only tests
         n = len(self._engines)
@@ -58,7 +61,8 @@ class Server:
                            default_max_tokens=default_max_tokens, vocab=vocab, max_model_len=max_model_len,
                            enable_sampling=1 if enable_sampling else 0,
                            enable_logprobs=1 if enable_logprobs else 0,
-                           enable_logits_processors=1 if enable_logits_processors else 0)
+                           enable_logits_processors=1 if enable_logits_processors else 0,
+                           enable_prompt_logprobs=1 if enable_prompt_logprobs else 0)
         self._h = C.c_void_p()
         check(self._l.b200_server_create(C.byref(cfg), arr, n, C.byref(self._h)))
 

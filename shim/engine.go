@@ -87,7 +87,7 @@ func NewServer(model string, strategy int, engines []*Engine) (*Server, error) {
 	defer C.free(unsafe.Pointer(cm))
 	cfg := C.b200_server_config{model: cm, strategy: C.int32_t(strategy), mean_load_pct: 125, replication: 256,
 		prefix_char_length: 100, max_retries: 3, default_max_tokens: 256, vocab: 128256, max_model_len: 2048,
-		enable_sampling: 1, enable_logprobs: 1, enable_logits_processors: 1}
+		enable_sampling: 1, enable_logprobs: 1, enable_logits_processors: 1, enable_prompt_logprobs: 1}
 	hs := make([]*C.b200_engine, len(engines))
 	for i, e := range engines {
 		hs[i] = e.h
