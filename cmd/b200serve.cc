@@ -73,6 +73,7 @@ int main(int argc, char** argv) {
   sc.enable_logprobs = 1;
   sc.enable_logits_processors = 1;
   sc.enable_prompt_logprobs = 1;
+  sc.max_n = max_seqs;   // every choice of a request runs at once
   b200_server* srv = nullptr;
   if (b200_server_create(&sc, engines.data(), gpus, &srv)) { fprintf(stderr, "server: %s\n", b200_last_error()); return 1; }
   // the checkpoint's tokenizer + Llama-3 chat template when there is one; the synthetic tokenizer otherwise

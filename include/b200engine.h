@@ -140,6 +140,14 @@ int b200_engine_create(const b200_config* cfg, b200_engine** out);
 void b200_engine_destroy(b200_engine* e);
 
 int b200_submit(b200_engine* e, const int32_t* prompt_ids, int32_t n, const b200_sampling* sp, uint64_t* req_id);
+/* Parallel sampling (vLLM's n): n requests that share one prompt, prefilled once.  req_ids[0..n) receive n request ids, each
+ * usable with every per-request call below.  Member i samples with seed + i when sp has a seed (vLLM's
+ * ParentRequest._get_child_sampling_params), else with a seed of its own drawn by the engine; otherwise every member uses sp.
+ * When the prompt is computed, the members fork: they share its full KV pages by reference and each gets its own copy of
+ * the partly filled last page.  All n run at once, so 1 <= n <= max_num_seqs; n > 1 needs temperature >= 1e-5 (vLLM's
+ * "n must be 1 when using greedy sampling").  B200_ERR_INVALID otherwise.  n = 1 is b200_submit. */
+int b200_submit_n(b200_engine* e, const int32_t* prompt_ids, int32_t n_prompt, const b200_sampling* sp, int32_t n,
+                  uint64_t* req_ids);
 /* Drain newly generated token ids (at most cap).  *finished gets a B200_FINISH_* code or 0. */
 int b200_poll(b200_engine* e, uint64_t req_id, int32_t* out_ids, int32_t cap, int32_t* n_out, int32_t* finished,
               b200_usage* usage);
@@ -157,6 +165,9 @@ int b200_poll_prompt_logprobs(b200_engine* e, uint64_t req_id, float* out_logpro
                               float* out_top_logprob, int32_t cap, int32_t* n_out);
 /* Block until the request has undrained tokens or is finished (B200_ERR_TIMEOUT otherwise). */
 int b200_wait(b200_engine* e, uint64_t req_id, int64_t timeout_us);
+/* Block until any of ids[0..count) has undrained tokens or is finished (B200_ERR_TIMEOUT otherwise).  count 1 is b200_wait;
+ * with count > 1 the ids must be members of one b200_submit_n call (else B200_ERR_INVALID). */
+int b200_wait_any(b200_engine* e, const uint64_t* ids, int32_t count, int64_t timeout_us);
 int b200_abort(b200_engine* e, uint64_t req_id);
 /* Forget a finished request (frees its host-side record). */
 int b200_release(b200_engine* e, uint64_t req_id);
@@ -290,6 +301,9 @@ typedef struct {
   /* 1: serve prompt_logprobs (both routes) and echo (completions) in vLLM's response format; 0: they get a 400, as before
    * prompt logprobs existed (a zero-initialised config keeps that) */
   int32_t enable_prompt_logprobs;
+  /* k >= 2: serve "n" up to k on both routes (b200_submit_n; k at most the engines' max_num_seqs), with vLLM's checks;
+   * 0 or 1: n > 1 gets a 400, as before parallel sampling existed (a zero-initialised config keeps that) */
+  int32_t max_n;
 } b200_server_config;
 int b200_server_create(const b200_server_config* cfg, b200_engine* const* replicas, int32_t n, b200_server** out);
 void b200_server_destroy(b200_server* s);
@@ -497,6 +511,11 @@ int b200_op_paged_attn_prefill_tc(const void* qkv, int32_t q_rows, int32_t ldq, 
                                   const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
                                   int32_t q_heads, int32_t kv_heads, float scale, void* stream);
 int b200_op_init_uniform(void* p, uint64_t n, uint32_t seed, float scale, float offset, void* stream);
+/* The fork's page copy: for i < n_pairs and every layer l, the block_bytes at kv + l * layer_stride_bytes + src[i] * block_bytes
+ * are copied to dst[i]'s page (src / dst device int32 arrays; a src may repeat).  block_bytes and layer_stride_bytes are
+ * 16-byte multiples and kv is 16-byte aligned.  Bit-exact; nothing outside the dst pages is written. */
+int b200_op_kv_copy_blocks(void* kv, int32_t num_layers, int64_t layer_stride_bytes, int64_t block_bytes, const int32_t* src,
+                           const int32_t* dst, int32_t n_pairs, void* stream);
 
 #ifdef __cplusplus
 }

@@ -24,6 +24,7 @@ SOURCES = [
     "elementwise.cu",
     "sampling.cu",
     "penalties.cu",
+    "kv_fork.cu",
     "abi_ops.cu",
     "engine.cu",
     "router.cc",

@@ -96,7 +96,7 @@ class ServerConfig(C.Structure):
                 ("mean_load_pct", C.c_int32), ("replication", C.c_int32), ("prefix_char_length", C.c_int32),
                 ("max_retries", C.c_int32), ("default_max_tokens", C.c_int32), ("vocab", C.c_int32),
                 ("max_model_len", C.c_int32), ("enable_sampling", C.c_int32), ("enable_logprobs", C.c_int32),
-                ("enable_logits_processors", C.c_int32), ("enable_prompt_logprobs", C.c_int32)]
+                ("enable_logits_processors", C.c_int32), ("enable_prompt_logprobs", C.c_int32), ("max_n", C.c_int32)]
 
 
 class HarnessConfig(C.Structure):
@@ -136,7 +136,9 @@ SYMBOLS = {
     "b200_poll": (C.c_int, [_vp, _u64, _pi32, _i32, _pi32, _pi32, C.POINTER(Usage)]),
     "b200_poll_logprobs": (C.c_int, [_vp, _u64, _pi32, _vp, _pi32, _vp, _i32, _pi32, _pi32, C.POINTER(Usage)]),
     "b200_poll_prompt_logprobs": (C.c_int, [_vp, _u64, _vp, _pi32, _pi32, _vp, _i32, _pi32]),
+    "b200_submit_n": (C.c_int, [_vp, _pi32, _i32, C.POINTER(Sampling), _i32, C.POINTER(_u64)]),
     "b200_wait": (C.c_int, [_vp, _u64, _i64]),
+    "b200_wait_any": (C.c_int, [_vp, C.POINTER(_u64), _i32, _i64]),
     "b200_abort": (C.c_int, [_vp, _u64]),
     "b200_release": (C.c_int, [_vp, _u64]),
     "b200_stats_get": (C.c_int, [_vp, C.POINTER(Stats)]),
@@ -221,6 +223,7 @@ SYMBOLS = {
     "b200_op_paged_attn_decode_split": (C.c_int, [_vp, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _f, _i32, _vp]),
     "b200_op_paged_attn_prefill_tc": (C.c_int, [_vp, _i32, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _f, _vp]),
     "b200_op_init_uniform": (C.c_int, [_vp, _u64, C.c_uint32, _f, _f, _vp]),
+    "b200_op_kv_copy_blocks": (C.c_int, [_vp, _i32, _i64, _i64, _vp, _vp, _i32, _vp]),
 }
 
 

@@ -381,6 +381,19 @@ int b200_op_paged_attn_prefill_tc(const void* qkv, int32_t q_rows, int32_t ldq, 
   return rc ? cuda_fail("paged_attention_prefill_tc", rc) : 0;
 }
 
+int b200_op_kv_copy_blocks(void* kv, int32_t num_layers, int64_t layer_stride_bytes, int64_t block_bytes, const int32_t* src,
+                           const int32_t* dst, int32_t n_pairs, void* stream) {
+  if (int rc = require_device()) return rc;
+  int rc = kv_copy_blocks(kv, num_layers, layer_stride_bytes, block_bytes, src, dst, n_pairs, static_cast<cudaStream_t>(stream));
+  if (rc == -1) {
+    set_error("b200_op_kv_copy_blocks: bad arguments (n_pairs=%d num_layers=%d block_bytes=%lld layer_stride_bytes=%lld; "
+              "16-byte multiples and a 16-byte aligned kv required)", n_pairs, num_layers, static_cast<long long>(block_bytes),
+              static_cast<long long>(layer_stride_bytes));
+    return B200_ERR_INVALID;
+  }
+  return rc ? cuda_fail("kv_copy_blocks", rc) : 0;
+}
+
 int b200_op_init_uniform(void* p, uint64_t n, uint32_t seed, float scale, float offset, void* stream) {
   if (int rc = require_device()) return rc;
   int rc = init_uniform(p, n, seed, scale, offset, static_cast<cudaStream_t>(stream));

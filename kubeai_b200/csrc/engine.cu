@@ -175,6 +175,13 @@ struct PromptLogprobRecord {
   int32_t rank;
 };
 
+// the members of one b200_submit_n call: b200_wait_any sleeps here; every publish to a member bumps gen
+struct WaitGroup {
+  std::mutex m;
+  std::condition_variable cv;
+  uint64_t gen = 0;
+};
+
 struct Seq {
   uint64_t id = 0;
   std::vector<int32_t> toks;  // prompt + generated
@@ -207,6 +214,18 @@ struct Seq {
   std::atomic<int> n_cached{-1};  // prefix-hit tokens at first admission
   bool admitted = false;
   bool leaving = false;  // finished in the step being completed: swept out of the running list
+  // parallel sampling (b200_submit_n), engine thread: the leader (member 0) holds the members 1..n-1 until the step that
+  // completes its prompt forks them; they are registered and pollable but never queued before.  fork = the members that
+  // fork in the step being launched, fork_tails = their own copies of the prompt's partly filled last page (none when the
+  // prompt fills its pages).  group: b200_wait_any of the members.
+  std::vector<std::shared_ptr<Seq>> children, fork;
+  std::vector<int> fork_tails;
+  std::shared_ptr<WaitGroup> group;
+  void notify_group() {
+    if (!group) return;
+    { std::lock_guard<std::mutex> lk(group->m); ++group->gen; }
+    group->cv.notify_all();
+  }
   // shared with API threads: guarded by m (one lock per request, so a step's 128 wake-ups do not convoy on one mutex)
   std::mutex m;
   std::condition_variable cv;
@@ -254,6 +273,10 @@ struct StepMeta {
   // n_plp > 0.  Records go to the plp buffers in this order.
   int off_plp = -1;
   int n_plp = 0;
+  // parallel sampling's fork: n_fork source pages, then their n_fork destination pages (kv_copy_blocks after the forward);
+  // packed only when n_fork > 0
+  int off_fork = -1;
+  int n_fork = 0;
   int words = 0;
   int64_t kv_tokens = 0;
   int out_tokens = 0;  // sampled rows that produce a generated token
@@ -407,8 +430,11 @@ struct Engine {
   std::vector<SampleRow> samp_;          // parameters of the rows in rows_ order
   std::vector<int> lp_rows_, lp_n_;      // logprobs rows (indices into rows_) and their N
   std::vector<PenaltyRow> pen_;          // rows with logits edits
+  std::vector<int> fork_src_, fork_dst_; // the step's fork page copies
   int admit_edits(Seq& s);
-  bool ensure_blocks(Seq& s, int upto);
+  bool ensure_blocks(Seq& s, int upto, int tails = 0);
+  int plan_fork(Seq& s, int n);
+  void finish_group(std::shared_ptr<Seq> s, int code);
   void release_blocks(Seq& s);
   void preempt(std::shared_ptr<Seq> s);
   void finish(std::shared_ptr<Seq> s, int code);
@@ -456,6 +482,7 @@ Engine::~Engine() {
         if (!s->finished) s->finished = B200_FINISH_ABORTED;
       }
       s->cv.notify_all();
+      s->notify_group();
     }
   }
   if (step_timing[0] > 0) {
@@ -707,7 +734,7 @@ int Engine::alloc_all() {
   // ---- step input ring
   max_blocks_per_seq = (cfg.max_model_len + kPage - 1) / kPage;
   step_words_cap = 3 * Tcap + Scap + 4 * Scap + 4 * (Tcap / 16 + Scap + 1) + Scap * max_blocks_per_seq + 7 * Scap + 2 * Scap +
-                   8 * Scap + 3 * Tcap + 64;
+                   8 * Scap + 3 * Tcap + 2 * Scap + 64;
   static_assert(sizeof(SampleRow) == 7 * sizeof(int32_t), "SampleRow is 7 words of the step input");
   static_assert(sizeof(PenaltyRow) == 8 * sizeof(int32_t), "PenaltyRow is 8 words of the step input");
   ring_n = std::max(1, cfg.record_steps) + 1;  // last slot = scratch for unrecorded steps
@@ -911,18 +938,40 @@ int Engine::forward(const StepMeta& m, int32_t* dbuf, bool all_logits, bf16* log
 }
 
 // ------------------------------------------------------------------ scheduler helpers
-bool Engine::ensure_blocks(Seq& s, int upto) {
-  const int need = (upto + kPage - 1) / kPage - static_cast<int>(s.blocks.size());
-  if (need <= 0) return true;
-  if (pool.free_count() < need) return false;
+// Pages for s up to token `upto`, plus `tails` fresh pages for the members it forks in this step (all or nothing)
+bool Engine::ensure_blocks(Seq& s, int upto, int tails) {
+  const int need = std::max((upto + kPage - 1) / kPage - static_cast<int>(s.blocks.size()), 0);
+  if (need + tails == 0) return true;
+  if (pool.free_count() < need + tails) return false;
   for (int i = 0; i < need; ++i) s.blocks.push_back(pool.alloc());
+  for (int i = 0; i < tails; ++i) s.fork_tails.push_back(pool.alloc());
   return true;
+}
+
+// When a chunk of n tokens completes the prompt of a leader with members not forked yet, the members still live fork in
+// this step (s.fork); returns the tail pages they need: one each when the prompt ends inside a page
+int Engine::plan_fork(Seq& s, int n) {
+  s.fork.clear();
+  if (s.children.empty() || s.n_computed + n != static_cast<int>(s.toks.size())) return 0;
+  for (auto& c : s.children)
+    if (!c->abort_requested.load(std::memory_order_relaxed)) s.fork.push_back(c);
+  return s.n_prompt % kPage ? static_cast<int>(s.fork.size()) : 0;
+}
+
+// s and the members it has not forked yet
+void Engine::finish_group(std::shared_ptr<Seq> s, int code) {
+  for (auto& c : s->children) finish(c, code);
+  s->children.clear();
+  finish(std::move(s), code);
 }
 
 void Engine::release_blocks(Seq& s) {
   // tail blocks go to the front of the LRU free queue order first (vLLM frees in reverse)
   for (auto it = s.blocks.rbegin(); it != s.blocks.rend(); ++it) pool.unref(*it);
   s.blocks.clear();
+  for (int b : s.fork_tails) pool.unref(b);
+  s.fork_tails.clear();
+  s.fork.clear();
   if (s.pen_slot >= 0) {   // the record list is a function of s.toks: the next admission rebuilds it
     pen_free.push_back(s.pen_slot);
     s.pen_slot = -1;
@@ -956,6 +1005,7 @@ void Engine::publish() {
       if (p.code) p.s->finished = p.code;
     }
     p.s->cv.notify_all();
+    p.s->notify_group();
   }
   pending_pub.clear();
   pending_lp.clear();
@@ -1033,17 +1083,24 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
                        return a->arrival_key != b->arrival_key ? a->arrival_key < b->arrival_key : a->n_prompt < b->n_prompt;
                      });
   }
-  // aborted requests leave first
+  // aborted requests leave first.  A leader whose members have not forked yet stays while any of them is live: the
+  // prompt is computed for them, and it leaves at the fork.
   {
+    auto aborted = [](const Seq& s) {
+      if (!s.abort_requested.load(std::memory_order_relaxed)) return false;
+      for (auto& c : s.children)
+        if (!c->abort_requested.load(std::memory_order_relaxed)) return false;
+      return true;
+    };
     size_t k = 0;
     for (size_t i = 0; i < running.size(); ++i) {
-      if (running[i]->abort_requested.load(std::memory_order_relaxed)) finish(running[i], B200_FINISH_ABORTED);
+      if (aborted(*running[i])) finish_group(running[i], B200_FINISH_ABORTED);
       else running[k++] = running[i];
     }
     running.resize(k);
     for (auto it = waiting.begin(); it != waiting.end();) {
-      if ((*it)->abort_requested.load(std::memory_order_relaxed)) {
-        finish(*it, B200_FINISH_ABORTED);
+      if (aborted(**it)) {
+        finish_group(*it, B200_FINISH_ABORTED);
         it = waiting.erase(it);
       } else {
         ++it;
@@ -1061,7 +1118,7 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
     int n = std::min(static_cast<int>(s->toks.size()) - s->n_computed, budget);
     if (n <= 0) { ++i; continue; }
     bool ok = true;
-    while (!ensure_blocks(*s, s->n_computed + n)) {
+    while (!ensure_blocks(*s, s->n_computed + n, plan_fork(*s, n))) {
       auto victim = running.back();
       running.pop_back();
       preempt(victim);
@@ -1073,18 +1130,23 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
     budget -= n;
     ++i;
   }
-  // 2. admit waiting requests
-  while (!preempted && budget > 0 && !waiting.empty() && static_cast<int>(running.size()) < cfg.max_num_seqs) {
+  // 2. admit waiting requests.  A parallel-sampling group holds the running slots of its members from the admission of
+  // its leader, so the fork always finds a slot, a sampled row and a logits-edit list for each of them.
+  int reserved = 0;
+  for (auto& s : running) reserved += static_cast<int>(s->children.size());
+  while (!preempted && budget > 0 && !waiting.empty() && static_cast<int>(running.size()) + reserved < cfg.max_num_seqs) {
     auto s = waiting.front();
+    const int members = static_cast<int>(s->children.size());
+    if (static_cast<int>(running.size()) + reserved + 1 + members > cfg.max_num_seqs) break;
     if (!s->admitted) admit_prefix(*s);
     int n = std::min(static_cast<int>(s->toks.size()) - s->n_computed, budget);
-    if (!ensure_blocks(*s, s->n_computed + n)) {
+    if (!ensure_blocks(*s, s->n_computed + n, plan_fork(*s, n))) {
       release_blocks(*s);
       if (running.empty() && sched.empty()) {
         // nothing else holds pages and it still does not fit: it never will (cannot happen while the pool holds one
         // max_model_len sequence, which init() enforces) — fail it instead of blocking the queue behind it forever
         waiting.pop_front();
-        finish(s, B200_FINISH_ERROR);
+        finish_group(s, B200_FINISH_ERROR);
         continue;
       }
       break;
@@ -1092,6 +1154,7 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
     s->admitted = true;
     waiting.pop_front();
     running.push_back(s);
+    reserved += members;
     if (s->edits())
       if (int rc = admit_edits(*s)) return rc;
     sched.push_back({s, n});
@@ -1119,6 +1182,8 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
   plp_tok_.clear();
   plp_tgt_.clear();
   plp_n_.clear();
+  fork_src_.clear();
+  fork_dst_.clear();
   bool any_sampled = false, any_minp = false;
   int32_t* h = stage_host;
   m.off_ids = 0; m.off_pos = m.T; m.off_slots = 2 * m.T;
@@ -1173,6 +1238,35 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
         lp_rows_.push_back(static_cast<int>(rows_.size()) - 1);
         lp_n_.push_back(s.top_logprobs);
       }
+      if (!s.children.empty()) {
+        // the fork: the last prompt position is sampled once more for every member that forks, each row with the member's
+        // own seed, logits-edit list and logprobs (the gathered final norm reads a row index any number of times).  A
+        // member aborted before the fork leaves here.
+        for (auto& c : s.children)
+          if (std::find(s.fork.begin(), s.fork.end(), c) == s.fork.end()) finish(c, B200_FINISH_ABORTED);
+        s.children.clear();
+        for (size_t k = 0; k < s.fork.size(); ++k) {
+          Seq& c = *s.fork[k];
+          rows_.push_back(tok + n - 1);
+          samp_.push_back({c.temperature, c.top_k, c.top_p, static_cast<uint32_t>(c.seed), static_cast<uint32_t>(c.seed >> 32),
+                           0, c.min_p});
+          any_minp |= c.min_p > 0.f;
+          if (c.edits()) {
+            if (int rc = admit_edits(c)) return rc;
+            pen_.push_back({static_cast<int>(rows_.size()) - 1, c.pen_slot, c.presence, c.frequency, c.repetition, 0,
+                            c.min_tokens, c.pen_history() ? 1 : 0});
+            m.pen_update |= c.pen_history();
+          }
+          if (c.top_logprobs >= 0) {
+            lp_rows_.push_back(static_cast<int>(rows_.size()) - 1);
+            lp_n_.push_back(c.top_logprobs);
+          }
+          if (!s.fork_tails.empty()) {   // the prompt ends inside its last page: each member gets its own copy
+            fork_src_.push_back(s.blocks[s.n_prompt / kPage]);
+            fork_dst_.push_back(s.fork_tails[k]);
+          }
+        }
+      }
     }
     tok += n;
   }
@@ -1224,6 +1318,13 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
     memcpy(h + w + 2 * m.n_plp, plp_n_.data(), plp_n_.size() * 4);
     w += 3 * m.n_plp;
   }
+  m.n_fork = static_cast<int>(fork_src_.size());
+  if (m.n_fork > 0) {   // and fork page copies
+    m.off_fork = w;
+    memcpy(h + w, fork_src_.data(), fork_src_.size() * 4);
+    memcpy(h + w + m.n_fork, fork_dst_.data(), fork_dst_.size() * 4);
+    w += 2 * m.n_fork;
+  }
   m.words = w;
   if (w > step_words_cap) {
     set_error("step staging overflow (%d > %d words)", w, step_words_cap);
@@ -1250,6 +1351,13 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
     ++stats.kernel_launches;
     if (penalize_update(reinterpret_cast<const PenaltyRow*>(dbuf + m.off_pen), m.n_pen, sampled, pen_recs, pen_lens, pen_cap, stream))
       frc = cuda_fail("penalize_update", -2);
+  }
+  if (!frc && m.n_fork > 0) {   // likewise: after this step wrote the prompt's KV, before the next step writes past it
+    ++stats.kernel_launches;
+    const size_t block_bytes = static_cast<size_t>(2) * Hkv * kPage * kD * 2;
+    if (kv_copy_blocks(kv, L, static_cast<int64_t>(kv_layer_elems) * 2, static_cast<int64_t>(block_bytes), dbuf + m.off_fork,
+                       dbuf + m.off_fork + m.n_fork, m.n_fork, stream))
+      frc = cuda_fail("kv_copy_blocks", -2);
   }
   nvtxRangePop();
   if (frc) return frc;
@@ -1309,27 +1417,78 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
       if (n_plp > 0) pending_pub.push_back({sp, 0, false, 0, -1, plp0, n_plp});
       continue;
     }
-    const int32_t t = sampled_host[ri++];
-    s.toks.push_back(t);
-    ++s.n_generated;
-    ++gen;
-    int code = 0;
-    if (!s.ignore_eos && cfg.eos_token_id >= 0 && t == cfg.eos_token_id) code = B200_FINISH_STOP;
-    for (int sid : s.stop_ids) if (t == sid) code = B200_FINISH_STOP;
-    if (!code && s.n_generated >= s.max_tokens) code = B200_FINISH_LENGTH;
-    if (!code && static_cast<int>(s.toks.size()) >= cfg.max_model_len) code = B200_FINISH_LENGTH;
+    // the sampled token of `q` (the next row), its finish code and its logprobs record
+    auto take = [&](Seq& q, int32_t* t, int* lp) {
+      *t = sampled_host[ri++];
+      q.toks.push_back(*t);
+      ++q.n_generated;
+      ++gen;
+      int code = 0;
+      if (!q.ignore_eos && cfg.eos_token_id >= 0 && *t == cfg.eos_token_id) code = B200_FINISH_STOP;
+      for (int sid : q.stop_ids) if (*t == sid) code = B200_FINISH_STOP;
+      if (!code && q.n_generated >= q.max_tokens) code = B200_FINISH_LENGTH;
+      if (!code && static_cast<int>(q.toks.size()) >= cfg.max_model_len) code = B200_FINISH_LENGTH;
+      *lp = -1;
+      if (q.top_logprobs >= 0) {   // records come back in step order, as the ids do
+        LogprobRecord r;
+        const float* src = lp_host + static_cast<size_t>(li) * (1 + kMaxLogprobs);
+        r.lp = src[0];
+        memcpy(r.top_lp, src + 1, sizeof(r.top_lp));
+        memcpy(r.top_ids, lp_ids_host + static_cast<size_t>(li) * kMaxLogprobs, sizeof(r.top_ids));
+        ++li;
+        *lp = static_cast<int>(pending_lp.size());
+        pending_lp.push_back(r);
+      }
+      return code;
+    };
+    int32_t t = 0;
     int lp = -1;
-    if (s.top_logprobs >= 0) {   // records come back in step order, as the ids do
-      LogprobRecord r;
-      const float* src = lp_host + static_cast<size_t>(li) * (1 + kMaxLogprobs);
-      r.lp = src[0];
-      memcpy(r.top_lp, src + 1, sizeof(r.top_lp));
-      memcpy(r.top_ids, lp_ids_host + static_cast<size_t>(li) * kMaxLogprobs, sizeof(r.top_ids));
-      ++li;
-      lp = static_cast<int>(pending_lp.size());
-      pending_lp.push_back(r);
+    int code = take(s, &t, &lp);
+    const bool fork = !s.fork.empty();
+    // a leader aborted before its fork computed the prompt for its members only: it leaves with no token
+    const bool gone = fork && s.abort_requested.load(std::memory_order_relaxed);
+    if (gone) {
+      s.toks.pop_back();
+      --s.n_generated;
+      --gen;
+      code = B200_FINISH_ABORTED;
     }
-    pending_pub.push_back({sp, t, true, code, lp, plp0, n_plp});
+    pending_pub.push_back({sp, t, !gone, code, gone ? -1 : lp, plp0, n_plp});
+    if (fork) {
+      // members 1..n-1 become running sequences: the prompt's full pages by reference, their own copy of its partly
+      // filled last page, the leader's cache chain and prompt records, and the token their own row sampled
+      std::vector<PromptLogprobRecord> plp_all;
+      if (s.prompt_logprobs >= 0) {
+        { std::lock_guard<std::mutex> lk(s.m); plp_all = s.plp_out; }
+        plp_all.insert(plp_all.end(), pending_plp.begin() + plp0, pending_plp.begin() + plp0 + n_plp);
+      }
+      const int shared = s.n_prompt / kPage;   // with a full last page there are no tails: every page is shared
+      for (size_t k = 0; k < s.fork.size(); ++k) {
+        const std::shared_ptr<Seq>& cp = s.fork[k];
+        Seq& c = *cp;
+        for (int b = 0; b < shared; ++b) {
+          pool.ref(s.blocks[b]);
+          c.blocks.push_back(s.blocks[b]);
+        }
+        if (!s.fork_tails.empty()) c.blocks.push_back(s.fork_tails[k]);
+        c.n_computed = s.n_computed;
+        c.n_published = s.n_published;
+        c.chain_uid = s.chain_uid;
+        c.plp_done = s.plp_done;
+        c.n_cached = s.n_cached.load();
+        c.admitted = true;
+        int32_t tc = 0;
+        int lpc = -1;
+        const int cc = take(c, &tc, &lpc);
+        const int pc0 = static_cast<int>(pending_plp.size());
+        pending_plp.insert(pending_plp.end(), plp_all.begin(), plp_all.end());
+        pending_pub.push_back({cp, tc, true, cc, lpc, pc0, static_cast<int>(plp_all.size())});
+        if (cc) release_blocks(c);
+        else running.push_back(cp);
+      }
+      s.fork_tails.clear();   // owned by the members now
+      s.fork.clear();
+    }
     if (code) {
       release_blocks(s);
       s.leaving = true;
@@ -1435,9 +1594,15 @@ void Engine::fail_all() {
   pending_pub.clear();
   pending_lp.clear();
   pending_plp.clear();
+  const size_t n_queued = all.size();
+  for (size_t i = 0; i < n_queued; ++i) {   // and the members their leaders have not forked yet
+    all.insert(all.end(), all[i]->children.begin(), all[i]->children.end());
+    all.insert(all.end(), all[i]->fork.begin(), all[i]->fork.end());
+  }
   for (auto& s : all) {
     { std::lock_guard<std::mutex> lk(s->m); s->finished = B200_FINISH_ERROR; }
     s->cv.notify_all();
+    s->notify_group();
   }
 }
 
@@ -1513,9 +1678,15 @@ int b200_engine_create(const b200_config* cfg, b200_engine** out) {
 
 void b200_engine_destroy(b200_engine* e) { delete e; }
 
-int b200_submit(b200_engine* e, const int32_t* prompt_ids, int32_t n, const b200_sampling* sp, uint64_t* req_id) {
-  if (!e || !prompt_ids || n <= 0 || !req_id) { set_error("b200_submit: bad arguments"); return B200_ERR_INVALID; }
+// b200_submit (members 1) and b200_submit_n
+static int submit_impl(b200_engine* e, const int32_t* prompt_ids, int32_t n, const b200_sampling* sp, int32_t members,
+                       uint64_t* req_ids) {
+  if (!e || !prompt_ids || n <= 0 || !req_ids) { set_error("b200_submit: bad arguments"); return B200_ERR_INVALID; }
   Engine& g = e->impl;
+  // vLLM's SamplingParams._verify_args / _verify_greedy_sampling; every member runs at once, so max_num_seqs bounds n
+  if (members < 1) { set_error("n must be at least 1, got %d.", members); return B200_ERR_INVALID; }
+  if (members > g.cfg.max_num_seqs) { set_error("n (%d) exceeds max_num_seqs %d", members, g.cfg.max_num_seqs); return B200_ERR_INVALID; }
+  if (members > 1 && !(sp && sp->temperature >= 1e-5f)) { set_error("n must be 1 when using greedy sampling, got %d.", members); return B200_ERR_INVALID; }
   const int max_tokens = sp && sp->max_tokens > 0 ? sp->max_tokens : 16;
   if (n + 1 > g.cfg.max_model_len) { set_error("prompt (%d tokens) exceeds max_model_len %d", n, g.cfg.max_model_len); return B200_ERR_INVALID; }
   if (sp && !(std::isfinite(sp->temperature) && sp->temperature >= 0.f)) { set_error("temperature must be finite and >= 0"); return B200_ERR_INVALID; }
@@ -1541,40 +1712,62 @@ int b200_submit(b200_engine* e, const int32_t* prompt_ids, int32_t n, const b200
       if (!std::isfinite(sp->logit_bias_values[i])) { set_error("logit_bias values must be finite"); return B200_ERR_INVALID; }
     }
   }
-  auto s = std::make_shared<Seq>();
-  s->toks.assign(prompt_ids, prompt_ids + n);
-  s->n_prompt = n;
-  s->arrival_key = xxh64(prompt_ids, static_cast<size_t>(n) * sizeof(int32_t), 0);
-  s->max_tokens = max_tokens;
-  s->ignore_eos = sp && sp->ignore_eos;
-  if (sp && sp->num_stop_ids > 0 && sp->stop_ids) s->stop_ids.assign(sp->stop_ids, sp->stop_ids + sp->num_stop_ids);
-  if (sp) {
-    s->temperature = sp->temperature;
-    s->top_p = sp->top_p > 0.f ? sp->top_p : 1.f;   // 0 = off at this ABI
-    s->top_k = sp->top_k > 0 ? sp->top_k : 0;
-    s->top_logprobs = sp->logprobs ? sp->top_logprobs : -1;
-    s->prompt_logprobs = sp->prompt_logprobs ? sp->top_prompt_logprobs : -1;
-    s->min_p = sp->temperature >= 1e-5f ? sp->min_p : 0.f;   // greedy rows ignore min_p, as in vLLM
-    s->presence = sp->presence_penalty;
-    s->frequency = sp->frequency_penalty;
-    s->repetition = sp->repetition_penalty > 0.f ? sp->repetition_penalty : 1.f;
-    s->min_tokens = sp->min_tokens;
-    if (sp->num_logit_bias > 0) {
-      s->bias_ids.assign(sp->logit_bias_ids, sp->logit_bias_ids + sp->num_logit_bias);
-      s->bias_values.assign(sp->logit_bias_values, sp->logit_bias_values + sp->num_logit_bias);
+  auto make = [&] {
+    auto s = std::make_shared<Seq>();
+    s->toks.assign(prompt_ids, prompt_ids + n);
+    s->n_prompt = n;
+    s->arrival_key = xxh64(prompt_ids, static_cast<size_t>(n) * sizeof(int32_t), 0);
+    s->max_tokens = max_tokens;
+    s->ignore_eos = sp && sp->ignore_eos;
+    if (sp && sp->num_stop_ids > 0 && sp->stop_ids) s->stop_ids.assign(sp->stop_ids, sp->stop_ids + sp->num_stop_ids);
+    if (sp) {
+      s->temperature = sp->temperature;
+      s->top_p = sp->top_p > 0.f ? sp->top_p : 1.f;   // 0 = off at this ABI
+      s->top_k = sp->top_k > 0 ? sp->top_k : 0;
+      s->top_logprobs = sp->logprobs ? sp->top_logprobs : -1;
+      s->prompt_logprobs = sp->prompt_logprobs ? sp->top_prompt_logprobs : -1;
+      s->min_p = sp->temperature >= 1e-5f ? sp->min_p : 0.f;   // greedy rows ignore min_p, as in vLLM
+      s->presence = sp->presence_penalty;
+      s->frequency = sp->frequency_penalty;
+      s->repetition = sp->repetition_penalty > 0.f ? sp->repetition_penalty : 1.f;
+      s->min_tokens = sp->min_tokens;
+      if (sp->num_logit_bias > 0) {
+        s->bias_ids.assign(sp->logit_bias_ids, sp->logit_bias_ids + sp->num_logit_bias);
+        s->bias_values.assign(sp->logit_bias_values, sp->logit_bias_values + sp->num_logit_bias);
+      }
     }
+    return s;
+  };
+  std::vector<std::shared_ptr<Seq>> group;
+  for (int i = 0; i < members; ++i) group.push_back(make());
+  if (members > 1) {
+    auto wg = std::make_shared<WaitGroup>();
+    for (auto& s : group) s->group = wg;
+    group[0]->children.assign(group.begin() + 1, group.end());
   }
   {
     std::lock_guard<std::mutex> lk(g.mu_);
     if (g.fatal) { set_error("engine is in a failed state"); return B200_ERR_CUDA; }
-    s->seed = sp && sp->has_seed ? sp->seed : splitmix64(&g.seed_state);
-    s->id = g.next_id++;
-    g.requests[s->id] = s;
-    g.incoming.push_back(s);
-    *req_id = s->id;
+    for (int i = 0; i < members; ++i) {
+      // member i: seed + i (vLLM's ParentRequest._get_child_sampling_params), or a seed of its own
+      group[i]->seed = sp && sp->has_seed ? sp->seed + static_cast<uint64_t>(i) : splitmix64(&g.seed_state);
+      group[i]->id = g.next_id++;
+      g.requests[group[i]->id] = group[i];
+      req_ids[i] = group[i]->id;
+    }
+    g.incoming.push_back(group[0]);
   }
   g.cv_work_.notify_one();
   return 0;
+}
+
+int b200_submit(b200_engine* e, const int32_t* prompt_ids, int32_t n, const b200_sampling* sp, uint64_t* req_id) {
+  return submit_impl(e, prompt_ids, n, sp, 1, req_id);
+}
+
+int b200_submit_n(b200_engine* e, const int32_t* prompt_ids, int32_t n_prompt, const b200_sampling* sp, int32_t n,
+                  uint64_t* req_ids) {
+  return submit_impl(e, prompt_ids, n_prompt, sp, n, req_ids);
 }
 
 int b200_engine_set_fixed_admission(b200_engine* e, int32_t on) {
@@ -1688,6 +1881,42 @@ int b200_wait(b200_engine* e, uint64_t req_id, int64_t timeout_us) {
   if (timeout_us < 0) { s->cv.wait(lk, ready); return 0; }
   if (!s->cv.wait_for(lk, std::chrono::microseconds(timeout_us), ready)) { set_error("timeout"); return B200_ERR_TIMEOUT; }
   return 0;
+}
+
+int b200_wait_any(b200_engine* e, const uint64_t* ids, int32_t count, int64_t timeout_us) {
+  if (!e || !ids || count < 1) { set_error("b200_wait_any: bad arguments"); return B200_ERR_INVALID; }
+  if (count == 1) return b200_wait(e, ids[0], timeout_us);
+  Engine& g = e->impl;
+  std::vector<std::shared_ptr<Seq>> ss;
+  {
+    std::lock_guard<std::mutex> lk(g.mu_);
+    for (int i = 0; i < count; ++i) {
+      auto s = find_req(g, ids[i]);
+      if (!s) { set_error("unknown request %llu", static_cast<unsigned long long>(ids[i])); return B200_ERR_NOT_FOUND; }
+      ss.push_back(std::move(s));
+    }
+  }
+  WaitGroup* wg = ss[0]->group.get();
+  for (auto& s : ss)
+    if (!wg || s->group.get() != wg) { set_error("b200_wait_any: the ids are not members of one b200_submit_n call"); return B200_ERR_INVALID; }
+  auto ready = [&] {
+    for (auto& s : ss) {
+      std::lock_guard<std::mutex> lk(s->m);
+      if (s->out.size() > s->drained || s->finished != 0) return true;
+    }
+    return false;
+  };
+  const auto deadline = std::chrono::steady_clock::now() + std::chrono::microseconds(std::max<int64_t>(timeout_us, 0));
+  for (;;) {
+    // a publish after this read of gen bumps it after changing the member: the check below or the wait sees it
+    uint64_t gen0;
+    { std::lock_guard<std::mutex> lk(wg->m); gen0 = wg->gen; }
+    if (ready()) return 0;
+    std::unique_lock<std::mutex> lk(wg->m);
+    auto bumped = [&] { return wg->gen != gen0; };
+    if (timeout_us < 0) wg->cv.wait(lk, bumped);
+    else if (!wg->cv.wait_until(lk, deadline, bumped)) { set_error("timeout"); return B200_ERR_TIMEOUT; }
+  }
 }
 
 int b200_abort(b200_engine* e, uint64_t req_id) {

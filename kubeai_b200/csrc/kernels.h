@@ -28,6 +28,11 @@ int silu_mul(const void* gate_up, void* out, int T, int I, cudaStream_t st, Part
 int permute_gate_up(void* dst, const void* src, int I, int H, int to_physical, cudaStream_t st);
 int argmax_rows(const void* logits, int* out, int S, int V, int ld, cudaStream_t st, PartialView pv = no_partials());
 int init_uniform(void* p, size_t n, uint32_t seed, float scale, float offset, cudaStream_t st);
+// Parallel sampling's fork (kv_fork.cu): for every pair i and every layer l, copy the block_bytes of page src[i] to page
+// dst[i] at kv + l * layer_stride_bytes (src / dst device int arrays; sizes and kv 16-byte aligned).  Bit-exact; nothing
+// outside the dst pages is written.
+int kv_copy_blocks(void* kv, int num_layers, int64_t layer_stride_bytes, int64_t block_bytes, const int* src, const int* dst,
+                   int n_pairs, cudaStream_t st);
 
 // Per-row sampling parameters (sampling.cu; b200_sample_row at the ABI): temperature < 1e-5 is greedy, top_k <= 0 or >= V,
 // top_p <= 0 or >= 1 and min_p <= 0 are off; the noise of the row is Philox4x32-10 keyed by the seed and counted by n, the

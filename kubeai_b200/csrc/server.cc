@@ -8,7 +8,7 @@
 // and the backend half the reference leaves to vLLM: tokenise + chat template, stream tokens as
 // OpenAI SSE chunks in vLLM's framing (api/openai/v1/reference/example-requests.vllm.output:139-160;
 // vllm/entrypoints/openai/chat_completion/serving.py) (K12, K13).
-// The HTTP hop of proxyHTTP (handler.go:116-158) is replaced by b200_submit/b200_wait/b200_poll.
+// The HTTP hop of proxyHTTP (handler.go:116-158) is replaced by b200_submit_n/b200_wait_any/b200_poll.
 #include <arpa/inet.h>
 #include <errno.h>
 #include <netinet/in.h>
@@ -52,6 +52,7 @@ struct Server {
   bool logprobs = false;   // b200_server_config.enable_logprobs: serve logprobs / top_logprobs (else a 400)
   bool edits = false;      // b200_server_config.enable_logits_processors: serve penalties, min_p, min_tokens, logit_bias
   bool prompt_lp = false;  // b200_server_config.enable_prompt_logprobs: serve prompt_logprobs and completions echo
+  int max_n = 0;           // b200_server_config.max_n: >= 2 serves n up to it (else n > 1 is a 400)
   // optional real tokenizer (b200_server_set_tokenizer): a checkpoint's tokenizer.json instead of the synthetic byte/word ids
   const b200_tokenizer* real_tok = nullptr;
 
@@ -171,6 +172,7 @@ struct ParsedRequest {
   // read only when the server serves them: prompt_logprobs (-1: absent) and completions echo
   int prompt_logprobs = -1;
   bool echo = false;
+  int n = 1;   // choices (parallel sampling), read only when the server serves n
   std::vector<int32_t> stop_ids;
   // logits edits (b200_sampling): read only when the server serves them
   double presence = 0.0, frequency = 0.0, repetition = 1.0, min_p = 0.0;
@@ -395,6 +397,26 @@ int parse_request(Server& sv, const std::string& path, const std::string& ctype,
       return 400;
     }
   }
+  if (sv.max_n >= 2) {
+    // vLLM's SamplingParams checks of n (_verify_args, then _verify_greedy_sampling); every choice runs at once, so the
+    // server's max_n bounds it.  null is absent.
+    std::string bad_n;
+    if (const JVal* v = root.get("n"); v && v->type != JVal::Null) {
+      if (v->type != JVal::Num || v->num != std::floor(v->num) || std::fabs(v->num) > 2147483647.0) {
+        bad_n = "n must be an integer";
+      } else {
+        const int k = static_cast<int>(v->num);
+        if (k < 1) bad_n = "n must be at least 1, got " + std::to_string(k) + ".";
+        else if (k > sv.max_n) bad_n = "n must be at most " + std::to_string(sv.max_n) + ", got " + std::to_string(k) + ".";
+        else if (k > 1 && pr->temperature < 1e-5) bad_n = "n must be 1 when using greedy sampling, got " + std::to_string(k) + ".";
+        else pr->n = k;
+      }
+    }
+    if (!bad_n.empty()) {
+      *err = "bad request: " + bad_n;
+      return 400;
+    }
+  }
   if (const JVal* v = root.get("stop_token_ids"); v && v->type == JVal::Arr)
     for (auto& e : v->arr)
       if (e.type == JVal::Num) pr->stop_ids.push_back(static_cast<int32_t>(e.num));
@@ -411,7 +433,7 @@ int parse_request(Server& sv, const std::string& path, const std::string& ctype,
                  (v->type == JVal::Obj && !v->obj.empty()));
   };
   const char* bad = nullptr;
-  if (num_of("n", 1) > 1) bad = "n > 1";
+  if (sv.max_n < 2 && num_of("n", 1) > 1) bad = "n > 1";
   else if (num_of("best_of", 1) > 1) bad = "best_of > 1";
   else if (!sv.logprobs && (truthy("logprobs") || truthy("top_logprobs") || (!sv.prompt_lp && truthy("prompt_logprobs")))) bad = "logprobs";
   else if (!sv.prompt_lp && truthy("prompt_logprobs")) bad = "prompt_logprobs";
@@ -706,16 +728,26 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
     }
     sp.num_stop_ids = static_cast<int>(stops.size());
     sp.stop_ids = stops.empty() ? nullptr : stops.data();
-    uint64_t rid = 0;
+    // one element per choice (vLLM's n): its request id, output ids and logprob records, detokeniser and text_offset
+    struct Choice {
+      uint64_t rid = 0;
+      std::vector<int32_t> all;
+      std::vector<LpRecord> all_lp;
+      DetokStream detok;
+      size_t text_off = 0;   // completions stream: text_offset runs across chunks
+      bool echoed = false;
+      int fin = 0;
+      b200_usage usage{};
+    };
+    std::vector<Choice> ch(static_cast<size_t>(pr.n));
+    std::vector<uint64_t> rids(ch.size());
     bool failed = false;
     if (sv.faults[replica]->load() < 0) failed = true;  // permanent fault: stands for an engine in the failed state
     else if (sv.faults[replica]->load() > 0 && sv.faults[replica]->fetch_sub(1) > 0) failed = true;
-    if (!failed && b200_submit(eng, ids.data(), static_cast<int>(ids.size()), &sp, &rid)) failed = true;
+    if (!failed && b200_submit_n(eng, ids.data(), static_cast<int>(ids.size()), &sp, pr.n, rids.data())) failed = true;
 
-    std::vector<int32_t> all;
-    std::vector<LpRecord> all_lp;
-    std::vector<LpRecord> prompt_lp;   // the prompt records (plp_n >= 0), read with the first token
-    bool have_plp = false, echoed = false;
+    std::vector<LpRecord> prompt_lp;   // the prompt records (plp_n >= 0), read with the first token; every choice shares them
+    bool have_plp = false;
     // an echo's leading records: the first prompt token's null entry, then the prompt records
     auto echo_recs = [&] {
       std::vector<LpRecord> e{LpRecord{ids[0], 0.f, {}}};
@@ -726,11 +758,10 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
     const bool want_lp = pr.logprobs >= 0;
     // a token's string in logprobs: the single-id lossy decode (vLLM's tokenizer.decode([id])), or the synthetic piece
     auto token_str = [&](int32_t id) { return sv.real_tok ? tokenizer_token_text(sv.real_tok, id) : sv.tok.piece(id); };
-    size_t text_off = 0;   // completions stream: text_offset runs across chunks
-    DetokStream detok;
-    detok.tok = sv.real_tok;
-    int fin = 0;
-    b200_usage usage{};
+    for (size_t c = 0; c < ch.size(); ++c) {
+      ch[c].rid = rids[c];
+      ch[c].detok.tok = sv.real_tok;
+    }
     bool sent_any = false;
     if (!failed) {
       int32_t buf[256];
@@ -741,79 +772,93 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
         top_lp.resize(256 * B200_MAX_LOGPROBS);
         top_ids.resize(256 * B200_MAX_LOGPROBS);
       }
-      while (!fin) {
-        b200_wait(eng, rid, 200000);
-        int n = 0;
-        const int prc = want_lp ? b200_poll_logprobs(eng, rid, buf, lpv.data(), top_ids.data(), top_lp.data(), 256, &n, &fin, &usage)
-                                : b200_poll(eng, rid, buf, 256, &n, &fin, &usage);
-        if (prc) { failed = true; break; }
-        if (fin == B200_FINISH_ERROR && !sent_any) { failed = true; break; }
-        if (plp_n >= 0 && !have_plp && n > 0) {   // published no later than the first token
-          const int np = static_cast<int>(ids.size()) - 1;
-          std::vector<float> plv(std::max(np, 1)), ptl(static_cast<size_t>(std::max(np, 1)) * B200_MAX_LOGPROBS);
-          std::vector<int32_t> prk(std::max(np, 1)), pti(static_cast<size_t>(std::max(np, 1)) * B200_MAX_LOGPROBS);
-          int got = 0;
-          if (b200_poll_prompt_logprobs(eng, rid, plv.data(), prk.data(), pti.data(), ptl.data(), np, &got) || got != np) { failed = true; break; }
-          for (int k = 0; k < np; ++k) {
-            LpRecord r{ids[k + 1], plv[k], {}};
-            r.rank = prk[k];
-            for (int j = 0; j < plp_n; ++j)
-              r.top.emplace_back(pti[static_cast<size_t>(k) * B200_MAX_LOGPROBS + j], ptl[static_cast<size_t>(k) * B200_MAX_LOGPROBS + j]);
-            prompt_lp.push_back(std::move(r));
-          }
-          have_plp = true;
-        }
-        std::vector<LpRecord> recs;
-        for (int i = 0; want_lp && i < n; ++i) {
-          LpRecord r{buf[i], lpv[i], {}};
-          for (int j = 0; j < pr.logprobs; ++j)
-            r.top.emplace_back(top_ids[static_cast<size_t>(i) * B200_MAX_LOGPROBS + j], top_lp[static_cast<size_t>(i) * B200_MAX_LOGPROBS + j]);
-          recs.push_back(std::move(r));
-        }
-        if (pr.stream && n > 0) {
-          if (!sent_any) {
-            w.begin(200, "text/event-stream; charset=utf-8");
-            if (pr.chat)
-              w.write("data: " + head + ",\"choices\":[{\"index\":0,\"delta\":{\"role\":\"assistant\",\"content\":\"\"},\"logprobs\":null,\"finish_reason\":null}]}\n\n");
-            sent_any = true;
-          }
-          for (int i = 0; i < n; ++i) {
-            const bool last = fin && i == n - 1;
-            const std::string fr = last ? std::string("\"") + finish_str(fin) + "\"" : "null";
-            // one chunk per token; with a real tokenizer a chunk carries the text that token completed (possibly none: a
-            // token may end inside a UTF-8 sequence), and the last chunk also what was still held
-            const std::string text = sv.real_tok ? detok.push(buf[i]) + (last ? detok.flush() : std::string()) : sv.tok.piece(buf[i]);
-            std::string piece = json_str(text);
-            std::string lpj = "null";
-            if (want_lp && pr.chat) lpj = "{\"content\":[" + chat_lp_content(recs[i], token_str) + "]}";
-            else if (want_lp) lpj = completion_lp({recs[i]}, text_off, token_str, pr.logprobs);
-            if (pr.echo && !echoed) {
-              // vLLM's first echo chunk: the prompt and its records, then the first token's unless max_tokens was 0.  The
-              // offsets of later chunks count the generated text only, as in vLLM.
-              piece = json_str(echo_text + (echo_only ? std::string() : text));
-              if (want_lp) {
-                std::vector<LpRecord> e = echo_recs();
-                if (!echo_only) e.push_back(recs[i]);
-                lpj = completion_lp(e, 0, token_str, pr.logprobs);
-              }
-              echoed = true;
+      std::vector<uint64_t> live;
+      for (;;) {
+        live.clear();
+        for (auto& c : ch)
+          if (!c.fin) live.push_back(c.rid);
+        if (live.empty()) break;
+        b200_wait_any(eng, live.data(), static_cast<int>(live.size()), 200000);
+        // the choices in ascending index: within one engine step their chunks go out in that order
+        for (size_t ci = 0; ci < ch.size() && !failed; ++ci) {
+          Choice& c = ch[ci];
+          if (c.fin) continue;
+          int n = 0;
+          const int prc = want_lp ? b200_poll_logprobs(eng, c.rid, buf, lpv.data(), top_ids.data(), top_lp.data(), 256, &n, &c.fin, &c.usage)
+                                  : b200_poll(eng, c.rid, buf, 256, &n, &c.fin, &c.usage);
+          if (prc) { failed = true; break; }
+          if (c.fin == B200_FINISH_ERROR && !sent_any) { failed = true; break; }
+          if (plp_n >= 0 && !have_plp && n > 0) {   // published no later than the first token
+            const int np = static_cast<int>(ids.size()) - 1;
+            std::vector<float> plv(std::max(np, 1)), ptl(static_cast<size_t>(std::max(np, 1)) * B200_MAX_LOGPROBS);
+            std::vector<int32_t> prk(std::max(np, 1)), pti(static_cast<size_t>(std::max(np, 1)) * B200_MAX_LOGPROBS);
+            int got = 0;
+            if (b200_poll_prompt_logprobs(eng, c.rid, plv.data(), prk.data(), pti.data(), ptl.data(), np, &got) || got != np) { failed = true; break; }
+            for (int k = 0; k < np; ++k) {
+              LpRecord r{ids[k + 1], plv[k], {}};
+              r.rank = prk[k];
+              for (int j = 0; j < plp_n; ++j)
+                r.top.emplace_back(pti[static_cast<size_t>(k) * B200_MAX_LOGPROBS + j], ptl[static_cast<size_t>(k) * B200_MAX_LOGPROBS + j]);
+              prompt_lp.push_back(std::move(r));
             }
-            text_off += utf8_len(text);
-            if (pr.chat)
-              w.write("data: " + head + ",\"choices\":[{\"index\":0,\"delta\":{\"content\":" + piece + "},\"logprobs\":" + lpj + ",\"finish_reason\":" + fr +
-                      (last ? ",\"stop_reason\":null" : "") + "}]}\n\n");
-            else
-              w.write("data: " + head + ",\"choices\":[{\"index\":0,\"text\":" + piece + ",\"logprobs\":" + lpj + ",\"finish_reason\":" + fr + ",\"stop_reason\":null}],\"usage\":null}\n\n");
+            have_plp = true;
           }
+          std::vector<LpRecord> recs;
+          for (int i = 0; want_lp && i < n; ++i) {
+            LpRecord r{buf[i], lpv[i], {}};
+            for (int j = 0; j < pr.logprobs; ++j)
+              r.top.emplace_back(top_ids[static_cast<size_t>(i) * B200_MAX_LOGPROBS + j], top_lp[static_cast<size_t>(i) * B200_MAX_LOGPROBS + j]);
+            recs.push_back(std::move(r));
+          }
+          const std::string index = "{\"index\":" + std::to_string(ci);
+          if (pr.stream && n > 0) {
+            if (!sent_any) {
+              w.begin(200, "text/event-stream; charset=utf-8");
+              // chat: one role chunk per choice first (vLLM's chat_completion/serving.py)
+              for (size_t k = 0; pr.chat && k < ch.size(); ++k)
+                w.write("data: " + head + ",\"choices\":[{\"index\":" + std::to_string(k) +
+                        ",\"delta\":{\"role\":\"assistant\",\"content\":\"\"},\"logprobs\":null,\"finish_reason\":null}]}\n\n");
+              sent_any = true;
+            }
+            for (int i = 0; i < n; ++i) {
+              const bool last = c.fin && i == n - 1;
+              const std::string fr = last ? std::string("\"") + finish_str(c.fin) + "\"" : "null";
+              // one chunk per token; with a real tokenizer a chunk carries the text that token completed (possibly none: a
+              // token may end inside a UTF-8 sequence), and the last chunk also what was still held
+              const std::string text = sv.real_tok ? c.detok.push(buf[i]) + (last ? c.detok.flush() : std::string()) : sv.tok.piece(buf[i]);
+              std::string piece = json_str(text);
+              std::string lpj = "null";
+              if (want_lp && pr.chat) lpj = "{\"content\":[" + chat_lp_content(recs[i], token_str) + "]}";
+              else if (want_lp) lpj = completion_lp({recs[i]}, c.text_off, token_str, pr.logprobs);
+              if (pr.echo && !c.echoed) {
+                // vLLM's first echo chunk: the prompt and its records, then the first token's unless max_tokens was 0.  The
+                // offsets of later chunks count the generated text only, as in vLLM.
+                piece = json_str(echo_text + (echo_only ? std::string() : text));
+                if (want_lp) {
+                  std::vector<LpRecord> e = echo_recs();
+                  if (!echo_only) e.push_back(recs[i]);
+                  lpj = completion_lp(e, 0, token_str, pr.logprobs);
+                }
+                c.echoed = true;
+              }
+              c.text_off += utf8_len(text);
+              if (pr.chat)
+                w.write("data: " + head + ",\"choices\":[" + index + ",\"delta\":{\"content\":" + piece + "},\"logprobs\":" + lpj + ",\"finish_reason\":" + fr +
+                        (last ? ",\"stop_reason\":null" : "") + "}]}\n\n");
+              else
+                w.write("data: " + head + ",\"choices\":[" + index + ",\"text\":" + piece + ",\"logprobs\":" + lpj + ",\"finish_reason\":" + fr + ",\"stop_reason\":null}],\"usage\":null}\n\n");
+            }
+          }
+          c.all.insert(c.all.end(), buf, buf + n);
+          c.all_lp.insert(c.all_lp.end(), recs.begin(), recs.end());
         }
-        all.insert(all.end(), buf, buf + n);
-        all_lp.insert(all_lp.end(), recs.begin(), recs.end());
-        if (w.gone) {  // client disconnected: abort the sequence and free its KV blocks
-          b200_abort(eng, rid);
+        if (failed) break;
+        if (w.gone) {  // client disconnected: abort every choice and free its KV blocks
+          for (auto& c : ch) b200_abort(eng, c.rid);
           break;
         }
       }
-      b200_release(eng, rid);
+      for (auto& c : ch) b200_release(eng, c.rid);
     }
     if (failed) {
       if (b200_engine_is_failed(eng) || sv.faults[replica]->load() < 0) sv.drop_replica(replica);
@@ -827,41 +872,48 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
     }
     release_all();
     if (w.gone) return 499;
+    // usage: the prompt once, the completion tokens of every choice
+    b200_usage usage = ch[0].usage;
+    for (size_t c = 1; c < ch.size(); ++c) usage.completion_tokens += ch[c].usage.completion_tokens;
     if (pr.stream) {
       if (!sent_any) w.begin(200, "text/event-stream; charset=utf-8");
       if (pr.include_usage) w.write("data: " + head + ",\"choices\":[],\"usage\":" + usage_json(usage) + "}\n\n");
       w.write("data: [DONE]\n\n");
     } else {
-      std::string text;
-      if (sv.real_tok) {
-        DetokStream whole;
-        whole.tok = sv.real_tok;
-        for (auto t : all) text += whole.push(t);
-        text += whole.flush();
-      } else {
-        for (auto t : all) text += sv.tok.piece(t);
-      }
-      std::string out = "{\"id\":\"" + id + "\",\"object\":\"" + (pr.chat ? "chat.completion" : "text_completion") +
-                        "\",\"created\":" + std::to_string(created) + ",\"model\":" + json_str(pr.requested_model) + ",\"choices\":[{\"index\":0,";
-      if (pr.echo) text = echo_text + (echo_only ? std::string() : text);
-      if (pr.chat) out += "\"message\":{\"role\":\"assistant\",\"content\":" + json_str(text) + "},";
-      else out += "\"text\":" + json_str(text) + ",";
-      std::string lpj = "null";
-      if (want_lp && pr.chat) {
-        lpj = "{\"content\":[";
-        for (size_t k = 0; k < all_lp.size(); ++k) lpj += (k ? "," : "") + chat_lp_content(all_lp[k], token_str);
-        lpj += "]}";
-      } else if (want_lp && pr.echo) {
-        std::vector<LpRecord> e = echo_recs();
-        if (!echo_only) e.insert(e.end(), all_lp.begin(), all_lp.end());
-        lpj = completion_lp(e, 0, token_str, pr.logprobs);
-      } else if (want_lp) {
-        lpj = completion_lp(all_lp, 0, token_str, pr.logprobs);
-      }
-      // vLLM's prompt_logprobs: on the completions choice, at the top level of a chat response
+      // vLLM's prompt_logprobs: on every completions choice, once at the top level of a chat response
       const std::string plj = plp_n >= 0 ? ",\"prompt_logprobs\":" + prompt_lp_json(prompt_lp, token_str) : std::string();
-      out += "\"logprobs\":" + lpj + ",\"finish_reason\":\"" + finish_str(fin) + "\",\"stop_reason\":null" + (pr.chat ? "" : plj) +
-             "}],\"usage\":" + usage_json(usage) + (pr.chat ? plj : "") + "}";
+      std::string out = "{\"id\":\"" + id + "\",\"object\":\"" + (pr.chat ? "chat.completion" : "text_completion") +
+                        "\",\"created\":" + std::to_string(created) + ",\"model\":" + json_str(pr.requested_model) + ",\"choices\":[";
+      for (size_t ci = 0; ci < ch.size(); ++ci) {
+        const Choice& c = ch[ci];
+        std::string text;
+        if (sv.real_tok) {
+          DetokStream whole;
+          whole.tok = sv.real_tok;
+          for (auto t : c.all) text += whole.push(t);
+          text += whole.flush();
+        } else {
+          for (auto t : c.all) text += sv.tok.piece(t);
+        }
+        out += (ci ? ",{\"index\":" : "{\"index\":") + std::to_string(ci) + ",";
+        if (pr.echo) text = echo_text + (echo_only ? std::string() : text);
+        if (pr.chat) out += "\"message\":{\"role\":\"assistant\",\"content\":" + json_str(text) + "},";
+        else out += "\"text\":" + json_str(text) + ",";
+        std::string lpj = "null";
+        if (want_lp && pr.chat) {
+          lpj = "{\"content\":[";
+          for (size_t k = 0; k < c.all_lp.size(); ++k) lpj += (k ? "," : "") + chat_lp_content(c.all_lp[k], token_str);
+          lpj += "]}";
+        } else if (want_lp && pr.echo) {
+          std::vector<LpRecord> e = echo_recs();
+          if (!echo_only) e.insert(e.end(), c.all_lp.begin(), c.all_lp.end());
+          lpj = completion_lp(e, 0, token_str, pr.logprobs);
+        } else if (want_lp) {
+          lpj = completion_lp(c.all_lp, 0, token_str, pr.logprobs);
+        }
+        out += "\"logprobs\":" + lpj + ",\"finish_reason\":\"" + finish_str(c.fin) + "\",\"stop_reason\":null" + (pr.chat ? "" : plj) + "}";
+      }
+      out += "],\"usage\":" + usage_json(usage) + (pr.chat ? plj : "") + "}";
       w.begin(200, "application/json");
       w.write(out);
     }
@@ -1101,6 +1153,7 @@ int b200_server_create(const b200_server_config* cfg, b200_engine* const* replic
   sv.logprobs = cfg->enable_logprobs != 0;
   sv.edits = cfg->enable_logits_processors != 0;
   sv.prompt_lp = cfg->enable_prompt_logprobs != 0;
+  sv.max_n = cfg->max_n;
   if (b200_router_create(sv.replication, &sv.router)) { delete s; return B200_ERR_INVALID; }
   std::vector<std::string> names;
   std::string ad = cfg->adapters ? cfg->adapters : "";

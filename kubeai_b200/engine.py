@@ -94,6 +94,15 @@ class Engine:
         poll_logprobs.  min_p 0, the penalties 0 (repetition 1), min_tokens 0 and logit_bias None ({id: bias}) are off.
         prompt_logprobs N (0..20): keep each prompt token's log-probability, rank and its position's top N, read with
         poll_prompt_logprobs; None is off."""
+        return self.submit_n(prompt_ids, 1, max_tokens, ignore_eos, stop_ids, temperature, top_p, top_k, seed, logprobs,
+                             top_logprobs, min_p, presence_penalty, frequency_penalty, repetition_penalty, min_tokens,
+                             logit_bias, prompt_logprobs, _single=True)
+
+    def submit_n(self, prompt_ids, n, max_tokens=16, ignore_eos=True, stop_ids=(), temperature=0.0, top_p=1.0, top_k=0,
+                 seed=None, logprobs=False, top_logprobs=0, min_p=0.0, presence_penalty=0.0, frequency_penalty=0.0,
+                 repetition_penalty=1.0, min_tokens=0, logit_bias=None, prompt_logprobs=None, _single=False):
+        """Parallel sampling (b200_submit_n): n request ids sharing one prefill; member i uses seed + i (seed None: one
+        drawn per member).  The parameters are submit()'s; n > 1 needs temperature >= 1e-5."""
         ids = np.ascontiguousarray(prompt_ids, dtype=np.int32)
         stops = np.ascontiguousarray(stop_ids, dtype=np.int32)
         bias = dict(logit_bias or {})
@@ -112,10 +121,23 @@ class Engine:
                       logit_bias_values=bias_vals.ctypes.data_as(C.POINTER(C.c_float)) if len(bias_ids) else None,
                       prompt_logprobs=0 if prompt_logprobs is None else 1,
                       top_prompt_logprobs=0 if prompt_logprobs is None else prompt_logprobs)
-        rid = C.c_uint64()
-        check(self._l.b200_submit(self._h, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), C.byref(sp),
-                                  C.byref(rid)))
-        return rid.value
+        if _single:
+            rid = C.c_uint64()
+            check(self._l.b200_submit(self._h, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), C.byref(sp),
+                                      C.byref(rid)))
+            return rid.value
+        rids = (C.c_uint64 * max(n, 1))()
+        check(self._l.b200_submit_n(self._h, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), C.byref(sp), n, rids))
+        return list(rids[:n])
+
+    def wait_any(self, rids, timeout_s: float = -1.0) -> bool:
+        """Block until any of rids (one submit_n group, or a single id) has undrained tokens or is finished."""
+        arr = (C.c_uint64 * len(rids))(*rids)
+        rc = self._l.b200_wait_any(self._h, arr, len(rids), int(timeout_s * 1e6) if timeout_s >= 0 else -1)
+        if rc == -7:
+            return False
+        check(rc)
+        return True
 
     def poll(self, rid: int, cap: int = 4096) -> PollResult:
         buf = (C.c_int32 * cap)()

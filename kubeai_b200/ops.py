@@ -247,3 +247,13 @@ def init_uniform(n, seed, scale, offset, device="cuda"):
     out = torch.empty(n, dtype=torch.bfloat16, device=device)
     check(lib().b200_op_init_uniform(_p(out), n, seed & 0xFFFFFFFF, scale, offset, _stream()))
     return out
+
+
+def kv_copy_blocks(kv, num_layers, layer_stride_bytes, block_bytes, src, dst):
+    """The fork's page copy (b200_op_kv_copy_blocks) on a KV pool tensor `kv` (any dtype, contiguous): for each pair i and
+    layer l, the block_bytes at byte l * layer_stride_bytes + src[i] * block_bytes go to dst[i]'s page.  In place."""
+    assert kv.is_cuda and kv.is_contiguous()
+    s = torch.as_tensor(np.asarray(src, dtype=np.int32), device=kv.device)
+    d = torch.as_tensor(np.asarray(dst, dtype=np.int32), device=kv.device)
+    check(lib().b200_op_kv_copy_blocks(_p(kv), num_layers, layer_stride_bytes, block_bytes, _p(s), _p(d), len(s), _stream()))
+    return kv

@@ -45,12 +45,13 @@ class Server:
     enable_logits_processors: serve presence / frequency / repetition penalties, min_p, min_tokens and logit_bias; off,
     they get a 400.
     enable_prompt_logprobs: serve prompt_logprobs (both routes) and echo (completions) in vLLM's response format; off,
-    they get a 400."""
+    they get a 400.
+    max_n: k >= 2 serves "n" up to k (parallel sampling, at most the engines' max_num_seqs); 0 or 1, n > 1 gets a 400."""
 
     def __init__(self, engines, model="llama-3-8b", adapters=None, strategy=LEAST_LOAD, mean_load_pct=125,
                  replication=256, prefix_char_length=100, max_retries=3, default_max_tokens=256, vocab=128256,
                  max_model_len=2048, enable_sampling=False, enable_logprobs=False, enable_logits_processors=False,
-                 enable_prompt_logprobs=False):
+                 enable_prompt_logprobs=False, max_n=0):
         self._l = lib()
         self._engines = list(engines)   # keep alive; entries may be None for parse-path-only tests
         n = len(self._engines)
@@ -62,7 +63,7 @@ class Server:
                            enable_sampling=1 if enable_sampling else 0,
                            enable_logprobs=1 if enable_logprobs else 0,
                            enable_logits_processors=1 if enable_logits_processors else 0,
-                           enable_prompt_logprobs=1 if enable_prompt_logprobs else 0)
+                           enable_prompt_logprobs=1 if enable_prompt_logprobs else 0, max_n=max_n)
         self._h = C.c_void_p()
         check(self._l.b200_server_create(C.byref(cfg), arr, n, C.byref(self._h)))
 

@@ -69,6 +69,29 @@ func (e *Engine) Poll(id uint64, buf []int32) (n int, finished int, u C.b200_usa
 	return int(cn), int(fin), u, nil
 }
 
+// SubmitN starts n parallel samples of one prompt (vLLM's n): one prefill, n request ids for Poll / Abort.
+func (e *Engine) SubmitN(prompt []int32, sp *C.b200_sampling, n int) ([]uint64, error) {
+	ids := make([]C.uint64_t, n)
+	if rc := C.b200_submit_n(e.h, (*C.int32_t)(unsafe.Pointer(&prompt[0])), C.int32_t(len(prompt)), sp, C.int32_t(n), &ids[0]); rc != 0 {
+		return nil, errors.New(C.GoString(C.b200_last_error()))
+	}
+	out := make([]uint64, n)
+	for i, id := range ids {
+		out[i] = uint64(id)
+	}
+	return out, nil
+}
+
+// WaitAny blocks (at most 200 ms) until any member of one SubmitN group has tokens to Poll or is finished, so a Go-side
+// writer streams n choices without waiting behind one that is preempted.
+func (e *Engine) WaitAny(ids []uint64) {
+	c := make([]C.uint64_t, len(ids))
+	for i, id := range ids {
+		c[i] = C.uint64_t(id)
+	}
+	C.b200_wait_any(e.h, &c[0], C.int32_t(len(c)), 200000)
+}
+
 func (e *Engine) Abort(id uint64) { C.b200_abort(e.h, C.uint64_t(id)) } // client went away: frees the KV blocks
 
 // Failed reports whether a CUDA failure has poisoned this replica; the serving shell then drops it from the endpoint
@@ -87,7 +110,8 @@ func NewServer(model string, strategy int, engines []*Engine) (*Server, error) {
 	defer C.free(unsafe.Pointer(cm))
 	cfg := C.b200_server_config{model: cm, strategy: C.int32_t(strategy), mean_load_pct: 125, replication: 256,
 		prefix_char_length: 100, max_retries: 3, default_max_tokens: 256, vocab: 128256, max_model_len: 2048,
-		enable_sampling: 1, enable_logprobs: 1, enable_logits_processors: 1, enable_prompt_logprobs: 1}
+		enable_sampling: 1, enable_logprobs: 1, enable_logits_processors: 1, enable_prompt_logprobs: 1,
+		max_n: 128} // the engines' max_num_seqs (b200_config_default)
 	hs := make([]*C.b200_engine, len(engines))
 	for i, e := range engines {
 		hs[i] = e.h
