@@ -206,8 +206,10 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const uint16_t* __rest
     __syncthreads();
     zmax = __fdiv_rn(bf16_bits_to_f32(bits_of_key(s_kmax)), T);
     if (minp_on) {
-      // the smallest key t with (z(t) - z_max) >= log(min_p): the row max satisfies it (min_p <= 1), and NaN keys sit below
-      // -inf and fail it, so the predicate is false then true along the keys
+      // the smallest key t with (z(t) - z_max) >= log(min_p): the row max satisfies it (min_p <= 1), and -NaN keys sit
+      // below -inf and fail it, so the predicate is false then true along the keys.  A +NaN key sits above +inf: a row
+      // holding +NaN has a NaN z_max, no key passes, tm is the NaN key and the race (NaN scores never win) returns token 0
+      // (so does top-p there: every mass is 0, so tp is 0xFFFF).  Greedy, temperature-only and top-k rows skip the NaN.
       if (threadIdx.x == 0) {
         const double lm = log(static_cast<double>(P.min_p));
         uint32_t lo = 0, hi = s_kmax;

@@ -248,11 +248,10 @@ def test_argmax_epilogue_equals_argmax_of_the_plain_logits(T, N, K, force, n_val
     lg = plain.float()
     if n_valid:
         lg = lg[:, :n_valid]
-    want = lg.argmax(-1)                                     # torch returns the first maximum: lowest index wins ties
     mx = lg.max(-1).values
-    first = (lg == mx[:, None]).float().argmax(-1)
+    first = (lg == mx[:, None]).float().argmax(-1)           # the first maximum: lowest index wins ties
     assert torch.equal(ids.long(), first), f"{int((ids.long() != first).sum())} rows differ ({sch})"
-    assert torch.equal(first, want) or True
+    # constructed exact ties (duplicated weight rows): tests/test_sampling_exact_gpu.py
 
 
 # ---------------------------------------------------------------------------------------------------------------------
