@@ -5,6 +5,7 @@
 // messengers) is out of scope.
 //
 //   b200serve --gpus 8 --model llama-3-8b [--model-dir /models/llama-3-8b] [--strategy PrefixHash] [--port 8000]
+//             [--speculative-config '{"method": "ngram", "num_speculative_tokens": 3, "prompt_lookup_max": 4}']
 #include <signal.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -25,6 +26,7 @@ int main(int argc, char** argv) {
   double kv_fraction = 0.85;
   unsigned long long seed = 0;
   bool greedy_only = false;
+  std::string spec_json;   // vLLM's --speculative-config; speculation stays off without it
   for (int i = 1; i < argc; ++i) {
     std::string a = argv[i];
     auto next = [&]() -> const char* { return i + 1 < argc ? argv[++i] : ""; };
@@ -42,6 +44,7 @@ int main(int argc, char** argv) {
     else if (a == "--gpu-memory-utilization") kv_fraction = atof(next());
     else if (a == "--seed") seed = strtoull(next(), nullptr, 10);
     else if (a == "--greedy-only") greedy_only = true;   // refuse temperature >= 1e-5 with a 400
+    else if (a == "--speculative-config") spec_json = next();
     else { fprintf(stderr, "unknown flag %s\n", a.c_str()); return 2; }
   }
   b200_config cfg;
@@ -52,6 +55,7 @@ int main(int argc, char** argv) {
   cfg.max_batched_tokens = budget;
   cfg.kv_fraction = static_cast<float>(kv_fraction);
   cfg.seed = seed;
+  if (!spec_json.empty() && b200_speculative_config_parse(spec_json.c_str(), &cfg)) { fprintf(stderr, "%s\n", b200_last_error()); return 2; }
   std::vector<b200_engine*> engines;
   for (int g = 0; g < gpus; ++g) {
     cfg.device = g;

@@ -64,7 +64,17 @@ typedef struct {
   int32_t rope_scaling_type;
   float rope_factor, rope_low_freq_factor, rope_high_freq_factor;
   int32_t rope_original_max_pos;
+  /* n-gram speculative decoding (vLLM's --speculative-config {"method": "ngram", ...}): each decoding sequence proposes up
+   * to num_speculative_tokens drafts, the tokens that followed the longest suffix n-gram (prompt_lookup_min..max tokens)
+   * at the earliest of its longest earlier occurrences in the context (vLLM's tie rule), and the step verifies them; a draft is accepted exactly when it
+   * equals the token the sampler draws from its row, so the output stream is the non-speculative one.
+   * num_speculative_tokens: 0 = off, else 1..B200_MAX_SPEC_TOKENS.  Lookup lengths: 0 = unset (both unset: 5 and 5; one
+   * unset takes the other's value); 1 <= min <= max otherwise B200_ERR_INVALID at b200_engine_create. */
+  int32_t num_speculative_tokens;
+  int32_t prompt_lookup_min, prompt_lookup_max;
 } b200_config;
+
+#define B200_MAX_SPEC_TOKENS 3   /* drafts per step: the last token and 3 drafts fill decode attention's 16-row tile */
 
 /* Sampling follows vLLM V1 (vllm/v1/sample/sampler.py, ops/topk_topp_sampler.py), made deterministic: the token is a pure
  * function of the logits row, these parameters, the seed and the index of the token in the generation (csrc/sampling.cu).
@@ -126,6 +136,10 @@ typedef struct {
   int64_t last_step_tokens;   /* tokens in the last forward (T) */
   int64_t kernel_launches;    /* kernels launched by this engine so far */
   int64_t h2d_bytes, d2h_bytes; /* step inputs copied to the device / sampled ids copied back, totals */
+  /* speculative decoding (vLLM's SpecDecodingStats): verify rows proposed, draft tokens in them, drafts accepted, and
+   * accepted drafts by position in the draft */
+  int64_t spec_drafts, spec_draft_tokens, spec_accepted_tokens;
+  int64_t spec_accepted_per_pos[B200_MAX_SPEC_TOKENS];
 } b200_stats;
 
 typedef struct {
@@ -133,6 +147,8 @@ typedef struct {
   int32_t decode_seqs, prefill_seqs, sampled;
   int64_t kv_tokens_read;     /* unique K/V tokens streamed by this step: sum over sequences of their context length */
   double device_us;
+  int32_t draft_tokens;       /* speculative drafts verified in the step, and those accepted */
+  int32_t accepted_tokens;
 } b200_step_info;
 
 void b200_config_default(b200_config* cfg);          /* Llama-3-8B shape, vLLM-like limits */
@@ -318,6 +334,11 @@ int b200_server_parse_request(b200_server* s, const char* path, const char* cont
 int b200_server_listen(b200_server* s, const char* host, int32_t port, int32_t* bound_port);
 /* Prometheus text (kubeai_inference_requests_active + engine gauges); returns the full length. */
 int b200_server_metrics(b200_server* s, char* buf, size_t cap);
+/* vLLM's --speculative-config JSON for the n-gram method, applied to cfg: {"method": "ngram", "num_speculative_tokens": k,
+ * "prompt_lookup_min": a, "prompt_lookup_max": b} (the lookup lengths optional, null = unset).  Any other method, k
+ * outside 1..B200_MAX_SPEC_TOKENS, a lookup length below 1, min > max or an unknown key is B200_ERR_INVALID with a message
+ * (b200_last_error) and leaves cfg unchanged.  Host-only. */
+int b200_speculative_config_parse(const char* json, b200_config* cfg);
 /* Fault injection for the retry path: the next `count` submits on `replica` fail; count < 0 = every submit fails, which
  * stands for an engine in the failed state: the first failure drops the replica from the router's endpoint set. */
 /* Attach a tokenizer (b200_tokenizer_load; not owned, must outlive the server; NULL detaches): prompts are then rendered with
@@ -404,6 +425,12 @@ int64_t b200_tokenizer_chat_llama3(const b200_tokenizer* t, const char* const* r
  * out8: [0] token-tile size, [1] token tiles, [2] tiles (128 weight rows x token tile), [3] K-splits per tile, [4] CTAs,
  * [5] rule that chose the splits (1 one token tile, 2 several), [6] 0, [7] 0. */
 int b200_schedule_query(int32_t N, int32_t K, int32_t T, int32_t sms, int32_t* out8);
+/* Host-only: the n-gram proposer of speculative decoding (vLLM's _find_longest_matched_ngram_and_propose_tokens) on
+ * toks[0..n): the longest suffix of length min_n..max_n that occurred earlier, at the earliest of its longest earlier
+ * occurrences (vLLM's tie rule), and up to k tokens that followed it, never past max_model_len - n nor the end of toks.
+ * Writes them to out[0..k) and returns their count (0: no match); B200_ERR_INVALID on bad arguments. */
+int32_t b200_ngram_propose(const int32_t* toks, int32_t n, int32_t min_n, int32_t max_n, int32_t k, int32_t max_model_len,
+                           int32_t* out);
 /* Host-only: CTAs per (sequence, KV head) the engine gives decode attention when `num_work` sequences decode. */
 int b200_attn_split_query(int32_t num_work, int32_t kv_heads, int32_t max_ctx, int32_t sms);
 /* GEMM phase tracing: the wgmma GEMM records no timestamps, so only NULL (tracing off) is accepted; any buffer is
@@ -496,12 +523,15 @@ typedef struct {
   const int32_t* stop_ids;
 } b200_penalty_row;
 int b200_op_penalize(void* logits, int32_t ld, int32_t S, int32_t V, const b200_penalty_row* rows, void* edited, void* stream);
-/* work: int32[num_work][4] = {q_tok0, q_count, q_pos0, seq}; kv_layer: [block][2][kv_heads][16][128] */
+/* work: int32[num_work][4] = {q_tok0, q_count, q_pos0, seq}; kv_layer: [block][2][kv_heads][16][128].  decode = 1: every
+ * item has 1 <= q_count <= B200_MAX_SPEC_TOKENS + 1 consecutive query positions (a speculative verify), position j masked
+ * causally at q_pos0 + j, and the item's K/V read once for all of them; decode = 0: q_count <= 16. */
 int b200_op_paged_attn(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                        const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
                        int32_t q_heads, int32_t kv_heads, float scale, int32_t decode, void* stream);
 /* Decode attention with each work item's context split over `split` >= 1 CTAs per KV head (what the engine does when a step
- * has fewer decoding sequences than the device has SMs / kv_heads) and a merge of the partial softmax states. */
+ * has fewer decoding sequences than the device has SMs / kv_heads) and a merge of the partial softmax states.  Work items
+ * as b200_op_paged_attn with decode = 1 (q_count up to B200_MAX_SPEC_TOKENS + 1). */
 int b200_op_paged_attn_decode_split(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                                     const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
                                     int32_t q_heads, int32_t kv_heads, float scale, int32_t split, void* stream);

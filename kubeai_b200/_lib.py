@@ -7,6 +7,7 @@ from pathlib import Path
 
 _LIB = None
 LIB_PATH = Path(__file__).resolve().parent / "lib" / "libb200engine.so"
+MAX_SPEC_TOKENS = 3   # B200_MAX_SPEC_TOKENS
 
 
 class B200Error(RuntimeError):
@@ -28,6 +29,7 @@ class Config(C.Structure):
         ("manual_step", C.c_int32), ("record_steps", C.c_int32),
         ("rope_scaling_type", C.c_int32), ("rope_factor", C.c_float), ("rope_low_freq_factor", C.c_float),
         ("rope_high_freq_factor", C.c_float), ("rope_original_max_pos", C.c_int32),
+        ("num_speculative_tokens", C.c_int32), ("prompt_lookup_min", C.c_int32), ("prompt_lookup_max", C.c_int32),
     ]
 
 
@@ -75,12 +77,15 @@ class Stats(C.Structure):
                 ("prompt_tokens", C.c_int64), ("cached_prompt_tokens", C.c_int64), ("generated_tokens", C.c_int64),
                 ("preemptions", C.c_int64), ("last_step_device_us", C.c_double), ("total_device_us", C.c_double),
                 ("last_step_tokens", C.c_int64), ("kernel_launches", C.c_int64),
-                ("h2d_bytes", C.c_int64), ("d2h_bytes", C.c_int64)]
+                ("h2d_bytes", C.c_int64), ("d2h_bytes", C.c_int64),
+                ("spec_drafts", C.c_int64), ("spec_draft_tokens", C.c_int64), ("spec_accepted_tokens", C.c_int64),
+                ("spec_accepted_per_pos", C.c_int64 * MAX_SPEC_TOKENS)]
 
 
 class StepInfo(C.Structure):
     _fields_ = [("tokens", C.c_int32), ("decode_seqs", C.c_int32), ("prefill_seqs", C.c_int32),
-                ("sampled", C.c_int32), ("kv_tokens_read", C.c_int64), ("device_us", C.c_double)]
+                ("sampled", C.c_int32), ("kv_tokens_read", C.c_int64), ("device_us", C.c_double),
+                ("draft_tokens", C.c_int32), ("accepted_tokens", C.c_int32)]
 
 
 BEGIN_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.c_char_p)
@@ -184,6 +189,7 @@ SYMBOLS = {
                                             C.c_size_t]),
     "b200_server_listen": (C.c_int, [_vp, C.c_char_p, _i32, _pi32]),
     "b200_server_metrics": (C.c_int, [_vp, C.c_char_p, C.c_size_t]),
+    "b200_speculative_config_parse": (C.c_int, [C.c_char_p, _vp]),
     "b200_server_inject_fault": (C.c_int, [_vp, _i32, _i32]),
     "b200_tokenize": (C.c_int, [_i32, C.c_char_p, C.c_size_t, _pi32, _i32]),
     "b200_detokenize": (C.c_int, [_i32, _pi32, _i32, C.c_char_p, C.c_size_t]),
@@ -220,6 +226,7 @@ SYMBOLS = {
     "b200_tokenizer_chat_llama3": (C.c_int64, [C.c_void_p, _vp, _vp, _i32, _i32, _vp, C.c_size_t]),
     "b200_schedule_query": (C.c_int, [_i32, _i32, _i32, _i32, _vp]),
     "b200_attn_split_query": (C.c_int, [_i32, _i32, _i32, _i32]),
+    "b200_ngram_propose": (C.c_int32, [_pi32, _i32, _i32, _i32, _i32, _i32, _pi32]),
     "b200_op_paged_attn_decode_split": (C.c_int, [_vp, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _f, _i32, _vp]),
     "b200_op_paged_attn_prefill_tc": (C.c_int, [_vp, _i32, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _f, _vp]),
     "b200_op_init_uniform": (C.c_int, [_vp, _u64, C.c_uint32, _f, _f, _vp]),

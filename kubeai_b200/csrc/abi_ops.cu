@@ -357,7 +357,7 @@ int b200_op_paged_attn_decode_split(const void* q, int32_t ldq, void* out, int32
   static size_t ws_bytes = 0;
   static std::mutex mu;
   std::lock_guard<std::mutex> lk(mu);
-  const size_t need = attn_split_ws_bytes(num_work, kv_heads, split);
+  const size_t need = attn_split_ws_bytes(num_work, kv_heads, split, kMaxDecodeQ);
   if (need > ws_bytes) {
     cudaDeviceSynchronize();
     if (ws) cudaFree(ws);

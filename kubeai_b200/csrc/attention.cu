@@ -15,6 +15,10 @@
 //   * decode: the CTA's 4 warps each own a 16-token strip of every tile and merge their
 //     (max, sum, acc) through smem at the end; prefill: a CTA owns 16 query tokens x 4 heads, one
 //     head per warp, and walks the causal prefix.
+//   * a decode work item may carry up to 4 consecutive query positions (speculative decoding's verify
+//     step: the last token and up to 3 drafts).  Tile row r = 4 * j + h is head h at position j, so the
+//     16 rows of the tile that a single-position decode leaves zero hold them, and the K/V of the group
+//     is still read once.  Fragment rows g cover positions 0/1, rows g + 8 positions 2/3.
 // Rows of a page that lie beyond the sequence's last token are loaded as they are in HBM and masked; the pool is
 // zero-initialised and only ever holds finite K/V values, so a masked probability of 0 never meets a NaN.
 #include <cuda.h>
@@ -128,7 +132,10 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
     const __nv_bfloat16* r0p = nullptr;
     const __nv_bfloat16* r1p = nullptr;
     if (DECODE) {
-      if (g < 4) r0p = q + static_cast<size_t>(wk.q_tok0) * ldq + (kvh * 4 + g) * kD;
+      // rows of positions past q_count stay zero: they never touch the rows of the positions that exist
+      const int j0 = g >> 2, j1 = 2 + (g >> 2), head = kvh * 4 + (g & 3);
+      if (j0 < wk.q_count) r0p = q + static_cast<size_t>(wk.q_tok0 + j0) * ldq + head * kD;
+      if (j1 < wk.q_count) r1p = q + static_cast<size_t>(wk.q_tok0 + j1) * ldq + head * kD;
     } else {
       const int head = kvh * 4 + warp;
       if (g < wk.q_count) r0p = q + static_cast<size_t>(wk.q_tok0 + g) * ldq + head * kD;
@@ -180,8 +187,8 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
         }
       }
       // ---- causal mask, online softmax (fp32, base-2)
-      const int qp0 = DECODE ? wk.q_pos0 : wk.q_pos0 + g;
-      const int qp1 = DECODE ? wk.q_pos0 : wk.q_pos0 + g + 8;
+      const int qp0 = DECODE ? wk.q_pos0 + (g >> 2) : wk.q_pos0 + g;
+      const int qp1 = DECODE ? wk.q_pos0 + 2 + (g >> 2) : wk.q_pos0 + g + 8;
       float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
       for (int nt = 0; nt < NT; ++nt) {
@@ -265,42 +272,57 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
         *reinterpret_cast<uint32_t*>(dst + dn * 8) = pack_bf16x2(o[dn][2] * i1, o[dn][3] * i1);
     }
   } else {
-    // merge the 4 warps' partial softmax states: rows 0..3 of each warp tile are the 4 heads.  The stages are free
-    // here (the loop's last barrier followed the last tile, and no gather is in flight).
-    float* so = reinterpret_cast<float*>(smem);            // [4 warps][4 heads][128]
-    float* sm = so + 4 * 4 * kD;                           // [4][4]
-    float* sl = sm + 16;                                   // [4][4]
-    if (g < 4) {
+    // merge the 4 warps' partial softmax states: row r = 4 * j + h of each warp tile is head h at query position j.  The
+    // stages are free here (the loop's last barrier followed the last tile, and no gather is in flight).
+    float* so = reinterpret_cast<float*>(smem);            // [4 warps][16 rows][128]
+    float* sm = so + 4 * 16 * kD;                          // [4][16]
+    float* sl = sm + 4 * 16;                               // [4][16]
+    const int nrows = 4 * wk.q_count;
+    if (g < nrows) {
 #pragma unroll
       for (int dn = 0; dn < 16; ++dn) {
         float2 v = make_float2(o[dn][0], o[dn][1]);
-        *reinterpret_cast<float2*>(so + (warp * 4 + g) * kD + dn * 8 + tq * 2) = v;
+        *reinterpret_cast<float2*>(so + (warp * 16 + g) * kD + dn * 8 + tq * 2) = v;
       }
       if (tq == 0) {
-        sm[warp * 4 + g] = m0;
-        sl[warp * 4 + g] = l0;
+        sm[warp * 16 + g] = m0;
+        sl[warp * 16 + g] = l0;
+      }
+    }
+    if (g + 8 < nrows) {
+#pragma unroll
+      for (int dn = 0; dn < 16; ++dn) {
+        float2 v = make_float2(o[dn][2], o[dn][3]);
+        *reinterpret_cast<float2*>(so + (warp * 16 + g + 8) * kD + dn * 8 + tq * 2) = v;
+      }
+      if (tq == 0) {
+        sm[warp * 16 + g + 8] = m1;
+        sl[warp * 16 + g + 8] = l1;
       }
     }
     __syncthreads();
     const int d = tid;
-#pragma unroll
-    for (int h = 0; h < 4; ++h) {
+    for (int r = 0; r < nrows; ++r) {
+      const int j = r >> 2, h = r & 3;
       float mm = -INFINITY;
 #pragma unroll
-      for (int w = 0; w < 4; ++w) mm = fmaxf(mm, sm[w * 4 + h]);
+      for (int w = 0; w < 4; ++w) mm = fmaxf(mm, sm[w * 16 + r]);
       float num = 0.f, den = 0.f;
 #pragma unroll
       for (int w = 0; w < 4; ++w) {
-        const float mw = sm[w * 4 + h];
+        const float mw = sm[w * 16 + r];
         const float wgt = (mw == -INFINITY) ? 0.f : exp2f(mw - mm);
-        num += so[(w * 4 + h) * kD + d] * wgt;
-        den += sl[w * 4 + h] * wgt;
+        num += so[(w * 16 + r) * kD + d] * wgt;
+        den += sl[w * 16 + r] * wgt;
       }
       if (parts == 1) {
-        out[static_cast<size_t>(wk.q_tok0) * ldo + (kvh * 4 + h) * kD + d] = __float2bfloat16_rn(den > 0.f ? num / den : 0.f);
+        out[static_cast<size_t>(wk.q_tok0 + j) * ldo + (kvh * 4 + h) * kD + d] = __float2bfloat16_rn(den > 0.f ? num / den : 0.f);
       } else {
-        // [work][kv head][part][4 heads][128 acc | max | sum]
-        float* dst = split_ws + ((static_cast<size_t>(blockIdx.y) * Hkv + kvh) * parts + part) * (4 * (kD + 2)) + h * (kD + 2);
+        // position j's slab of [position][work][kv head][part][4 heads][128 acc | max | sum]: a launch whose items all
+        // have q_count == 1 uses slab 0 only
+        const size_t slab = static_cast<size_t>(gridDim.y) * Hkv * parts * (4 * (kD + 2));
+        float* dst = split_ws + j * slab + ((static_cast<size_t>(blockIdx.y) * Hkv + kvh) * parts + part) * (4 * (kD + 2)) +
+                     h * (kD + 2);
         dst[d] = num;
         if (d == 0) {
           dst[kD] = mm;
@@ -318,9 +340,10 @@ attn_merge_kernel(const float* __restrict__ split_ws, __nv_bfloat16* __restrict_
   griddep_enter();
   const AttnWork wk = work[blockIdx.y];
   const int kvh = blockIdx.x, d = threadIdx.x;
-  const float* base = split_ws + (static_cast<size_t>(blockIdx.y) * Hkv + kvh) * parts * (4 * (kD + 2));
-#pragma unroll
-  for (int h = 0; h < 4; ++h) {
+  const size_t slab = static_cast<size_t>(gridDim.y) * Hkv * parts * (4 * (kD + 2));
+  for (int r = 0; r < 4 * wk.q_count; ++r) {
+    const int j = r >> 2, h = r & 3;
+    const float* base = split_ws + j * slab + (static_cast<size_t>(blockIdx.y) * Hkv + kvh) * parts * (4 * (kD + 2));
     float mm = -INFINITY;
     for (int p = 0; p < parts; ++p) mm = fmaxf(mm, base[(p * 4 + h) * (kD + 2) + kD]);
     float num = 0.f, den = 0.f;
@@ -330,7 +353,7 @@ attn_merge_kernel(const float* __restrict__ split_ws, __nv_bfloat16* __restrict_
       num += s[d] * wgt;
       den += s[kD + 1] * wgt;
     }
-    out[static_cast<size_t>(wk.q_tok0) * ldo + (kvh * 4 + h) * kD + d] = __float2bfloat16_rn(den > 0.f ? num / den : 0.f);
+    out[static_cast<size_t>(wk.q_tok0 + j) * ldo + (kvh * 4 + h) * kD + d] = __float2bfloat16_rn(den > 0.f ? num / den : 0.f);
   }
 }
 
@@ -387,8 +410,8 @@ int launch_attn(const CUtensorMap& tm, dim3 grid, cudaStream_t st, const __nv_bf
 
 }  // namespace
 
-size_t attn_split_ws_bytes(int num_work, int Hkv, int parts) {
-  return static_cast<size_t>(num_work) * Hkv * parts * 4 * (kD + 2) * sizeof(float);
+size_t attn_split_ws_bytes(int num_work, int Hkv, int parts, int max_q) {
+  return static_cast<size_t>(max_q) * num_work * Hkv * parts * 4 * (kD + 2) * sizeof(float);
 }
 
 // Parts per decode work item such that the launch has about two CTAs per SM, each with at least two 64-token tiles.

@@ -221,6 +221,8 @@ struct Seq {
   std::vector<std::shared_ptr<Seq>> children, fork;
   std::vector<int> fork_tails;
   std::shared_ptr<WaitGroup> group;
+  // speculative decoding (engine thread): the drafts proposed for the step being launched (Sched::n_draft of them)
+  std::vector<int32_t> draft;
   void notify_group() {
     if (!group) return;
     { std::lock_guard<std::mutex> lk(group->m); ++group->gen; }
@@ -242,6 +244,7 @@ struct Sched {
   std::shared_ptr<Seq> s;
   int n;
   int n_plp = 0;   // prompt-logprob rows this chunk produces
+  int n_draft = 0; // speculative drafts among the n tokens (after the sequence's last token); Seq::draft holds them
 };
 // a launched, not yet completed step
 struct InFlight {
@@ -280,6 +283,7 @@ struct StepMeta {
   int words = 0;
   int64_t kv_tokens = 0;
   int out_tokens = 0;  // sampled rows that produce a generated token
+  int draft_tokens = 0;  // speculative drafts verified by the step
   int dmax_ctx = 0;    // longest context among the decode work items (split-KV decision)
 };
 
@@ -287,12 +291,79 @@ struct XMaps {
   CUtensorMap m[kGemmNumBlockN];  // token tiles 32, 64, 128, 256, 512
 };
 
+// ------------------------------------------------------------------ speculative decoding
+// The speculative settings of a config with vLLM's defaults for the lookup lengths (config/speculative.py: both unset gives
+// 5 and 5, one unset takes the other's value); B200_ERR_INVALID when out of range.
+int spec_resolve(const b200_config& c, int* k, int* mn, int* mx) {
+  *k = *mn = *mx = 0;
+  if (c.num_speculative_tokens < 0 || c.num_speculative_tokens > B200_MAX_SPEC_TOKENS) {
+    set_error("num_speculative_tokens must be in 0..%d, got %d", B200_MAX_SPEC_TOKENS, c.num_speculative_tokens);
+    return B200_ERR_INVALID;
+  }
+  if (c.prompt_lookup_min < 0 || c.prompt_lookup_max < 0) {
+    set_error("prompt_lookup_min and prompt_lookup_max must be >= 1 (0 = unset)");
+    return B200_ERR_INVALID;
+  }
+  int a = c.prompt_lookup_min, b = c.prompt_lookup_max;
+  if (!a && !b) a = b = 5;
+  else if (!a) a = b;
+  else if (!b) b = a;
+  if (a > b) {
+    set_error("prompt_lookup_min=%d must be <= prompt_lookup_max=%d", a, b);
+    return B200_ERR_INVALID;
+  }
+  if (c.num_speculative_tokens == 0) return 0;
+  *k = c.num_speculative_tokens;
+  *mn = a;
+  *mx = b;
+  return 0;
+}
+
 }  // namespace
+
+// vLLM's _find_longest_matched_ngram_and_propose_tokens (v1/spec_decode/ngram_proposer.py): a KMP pass over the reversed
+// context finds the longest prefix of the reversal, length <= max_n, that recurs later in it, i.e. the longest suffix
+// n-gram of the context that occurred before.  Among equally long matches the last one found in the reversal wins, which
+// is the earliest occurrence in the context, as there.  Writes the up to k tokens that followed it (never past
+// max_model_len - n, nor past the context's end) and returns their count.
+int ngram_propose(const int32_t* toks, int n, int min_n, int max_n, int k, int max_model_len, int32_t* out) {
+  if (n < min_n) return 0;
+  k = std::min(k, max_model_len - n);
+  if (k <= 0) return 0;
+  auto rev = [&](int i) { return toks[n - 1 - i]; };
+  max_n = std::min(max_n, n);   // no match is longer than the context
+  thread_local std::vector<int> lps;
+  lps.assign(std::max(max_n, 1), 0);   // lps[i] = the longest proper prefix of rev[0..i] that is also its suffix, for i < max_n
+  int longest = 0, position = 0, prev = 0;
+  for (int i = 1; i < n;) {
+    if (rev(prev) == rev(i)) {
+      ++prev;
+      if (prev >= longest) {   // >=: the later position in the reversal, the earlier occurrence in the context
+        longest = prev;
+        position = i;
+      }
+      if (i < max_n) lps[i] = prev;
+      if (prev == max_n) prev = lps[max_n - 1];   // never match longer than max_n
+      ++i;
+    } else if (prev != 0) {
+      prev = lps[prev - 1];
+    } else {
+      ++i;
+    }
+  }
+  if (longest < min_n) return 0;
+  const int start = n - 1 - position + longest;
+  k = std::min(k, n - start);
+  for (int j = 0; j < k; ++j) out[j] = toks[start + j];
+  return k;
+}
 
 // ------------------------------------------------------------------ engine
 struct Engine {
   b200_config cfg;
   int L, H, Hq, Hkv, I, V, QKV;
+  // n-gram speculative decoding: drafts per decoding sequence (0 = off) and the lookup n-gram lengths
+  int spec_k = 0, spec_min = 0, spec_max = 0;
   int Tcap, Scap, max_blocks_per_seq;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
@@ -431,6 +502,8 @@ struct Engine {
   std::vector<int> lp_rows_, lp_n_;      // logprobs rows (indices into rows_) and their N
   std::vector<PenaltyRow> pen_;          // rows with logits edits
   std::vector<int> fork_src_, fork_dst_; // the step's fork page copies
+  std::vector<int32_t> draft_tmp_;
+  void add_drafts(std::vector<Sched>& sched, int* budget);
   int admit_edits(Seq& s);
   bool ensure_blocks(Seq& s, int upto, int tails = 0);
   int plan_fork(Seq& s, int n);
@@ -630,7 +703,7 @@ int Engine::alloc_all() {
   tensors["step.sampled"] = {sampled, static_cast<size_t>(Scap) * 4};
   tensors["step.argmax_candidates"] = {cand, static_cast<size_t>(std::min(Scap, 128)) * ((V + 127) / 128) * sizeof(float2)};
   tensors["step.logits"] = {logits, static_cast<size_t>(Scap) * V * 2};
-  CK(cudaMalloc(&attn_ws, attn_split_ws_bytes(kSplitMaxWork, Hkv, kSplitMaxParts)));
+  CK(cudaMalloc(&attn_ws, attn_split_ws_bytes(kSplitMaxWork, Hkv, kSplitMaxParts, 1 + spec_k)));
   { const char* e = getenv("B200_ATTN_SPLIT"); attn_split_force = e ? atoi(e) : 0; }
   // split-K workspace and arrival counters: the largest need of any projection at any step size up to Tcap
   {
@@ -708,11 +781,12 @@ int Engine::alloc_all() {
   // ---- logits-edit record lists, allocated after the KV pool is sized (they do not change num_kv_blocks).  A list holds
   // one record per distinct id: at most max_model_len history ids, B200_MAX_LOGIT_BIAS bias ids, as many stop ids and EOS.
   pen_cap = cfg.max_model_len + 2 * B200_MAX_LOGIT_BIAS + 1;
-  CK(cudaMalloc(&pen_recs, static_cast<size_t>(Scap) * pen_cap * sizeof(PenaltyRec)));
-  CK(cudaMalloc(&pen_lens, static_cast<size_t>(Scap) * sizeof(int)));
+  // (one list per running sequence; the saved entries are per edited row, and a speculating sequence edits 1 + k rows)
+  CK(cudaMalloc(&pen_recs, static_cast<size_t>(cfg.max_num_seqs) * pen_cap * sizeof(PenaltyRec)));
+  CK(cudaMalloc(&pen_lens, static_cast<size_t>(cfg.max_num_seqs) * sizeof(int)));
   CK(cudaMalloc(&pen_save, static_cast<size_t>(Scap) * pen_cap * sizeof(uint16_t)));
-  CK(cudaMemsetAsync(pen_lens, 0, static_cast<size_t>(Scap) * sizeof(int), stream));
-  for (int i = Scap - 1; i >= 0; --i) pen_free.push_back(i);
+  CK(cudaMemsetAsync(pen_lens, 0, static_cast<size_t>(cfg.max_num_seqs) * sizeof(int), stream));
+  for (int i = cfg.max_num_seqs - 1; i >= 0; --i) pen_free.push_back(i);
 
   // ---- prompt-logprob scratch and records, likewise after the KV pool.  A group of 512 rows reads the lm_head once for
   // 512 rows (compute-bound) and keeps the scratch at 512 * V bf16 (131 MB at Llama-3's vocabulary).
@@ -766,7 +840,9 @@ int Engine::init(const b200_config& c) {
     return B200_ERR_INVALID;
   }
   Tcap = (c.max_batched_tokens + 15) / 16 * 16;
-  Scap = c.max_num_seqs;
+  if (int rc = spec_resolve(c, &spec_k, &spec_min, &spec_max)) return rc;
+  // sampled rows: one per sequence, and one per draft position of a speculating sequence
+  Scap = c.max_num_seqs * (1 + spec_k);
   memset(&stats, 0, sizeof(stats));
   {
     std::random_device rd;
@@ -1061,6 +1137,34 @@ int Engine::admit_edits(Seq& s) {
   return 0;
 }
 
+// Speculative decoding's drafts, after the running sequences are scheduled and before any admission (vLLM's order: running
+// requests, drafts included, then waiting ones).  A running sequence whose prompt is computed and that decodes one token
+// this step proposes up to spec_k drafts and verifies them with that token, as n = 1 + m tokens.  The drafts take only
+// the budget the running sequences leave and only free pages: they never preempt, and admission gets what they leave.
+// Sequences with history penalties (row j would need drafts 0..j-1 in the device history) and a group's fork step do not
+// speculate.
+void Engine::add_drafts(std::vector<Sched>& sched, int* budget) {
+  for (auto& sc : sched) {
+    Seq& s = *sc.s;
+    const int len = static_cast<int>(s.toks.size());
+    if (*budget <= 0) break;
+    if (sc.n != 1 || len - s.n_computed != 1 || s.n_generated == 0 || !s.children.empty() || s.pen_history()) continue;
+    // the verify emits up to m + 1 tokens: within max_tokens, and the context stays below max_model_len
+    const int cap = std::min({spec_k, s.max_tokens - s.n_generated - 1, cfg.max_model_len - len - 1, *budget});
+    if (cap <= 0) continue;
+    draft_tmp_.resize(spec_k);
+    int m = ngram_propose(s.toks.data(), len, spec_min, spec_max, cap, cfg.max_model_len, draft_tmp_.data());
+    if (m <= 0) continue;
+    if (!ensure_blocks(s, s.n_computed + 1 + m))   // no free page: only the drafts that fit in the pages it holds
+      m = std::min(m, static_cast<int>(s.blocks.size()) * kPage - s.n_computed - 1);
+    if (m <= 0) continue;
+    s.draft.assign(draft_tmp_.begin(), draft_tmp_.begin() + m);
+    sc.n += m;
+    sc.n_draft = m;
+    *budget -= m;
+  }
+}
+
 // ------------------------------------------------------------------ one scheduler iteration + forward
 // launch(): schedule (running first, then admissions, vLLM v1 order), pack the step's device inputs, enqueue the
 // H2D copy, the kernels and the D2H of the sampled ids.  Returns 0 when there is nothing to run, 1 when a step is
@@ -1130,6 +1234,7 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
     budget -= n;
     ++i;
   }
+  if (spec_k > 0 && !preempted) add_drafts(sched, &budget);
   // 2. admit waiting requests.  A parallel-sampling group holds the running slots of its members from the admission of
   // its leader, so the fork always finds a slot, a sampled row and a logits-edit list for each of them.
   int reserved = 0;
@@ -1191,10 +1296,10 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
   f->ndec_seq = f->npre_seq = 0;
   for (int si = 0; si < m.nseq; ++si) {
     Seq& s = *sched[si].s;
-    const int n = sched[si].n, p0 = s.n_computed;
+    const int n = sched[si].n, p0 = s.n_computed, nd = sched[si].n_draft;
     for (int j = 0; j < n; ++j) {
       const int p = p0 + j;
-      h[m.off_ids + tok + j] = s.toks[p];
+      h[m.off_ids + tok + j] = j < n - nd ? s.toks[p] : s.draft[j - (n - nd)];
       h[m.off_pos + tok + j] = p;
       h[m.off_slots + tok + j] = s.blocks[p / kPage] * kPage + (p % kPage);
     }
@@ -1212,9 +1317,11 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
         s.plp_done = hi;
       }
     }
-    if (n == 1) {
-      dwork_.push_back({tok, 1, p0, si});
-      m.kv_tokens += p0 + 1;
+    if (n == 1 || nd > 0) {
+      // a decode, or a speculative verify: its 1 + nd positions share one decode work item (attention.cu)
+      dwork_.push_back({tok, n, p0, si});
+      m.kv_tokens += p0 + n;
+      m.draft_tokens += nd;
       ++f->ndec_seq;
     } else {
       const int qb = kPrefillQueryBlock;
@@ -1222,21 +1329,25 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
       m.kv_tokens += p0 + n;  // unique K/V tokens this sequence streams from HBM (query tiles re-read them from L2)
       ++f->npre_seq;
     }
-    if (p0 + n == static_cast<int>(s.toks.size())) {
-      rows_.push_back(tok + n - 1);
-      // n = the index of the token this row generates: a request recomputed after preemption draws the same noise
-      samp_.push_back({s.temperature, s.top_k, s.top_p, static_cast<uint32_t>(s.seed), static_cast<uint32_t>(s.seed >> 32),
-                       s.n_generated, s.min_p});
-      any_sampled |= s.temperature >= 1e-5f;
-      any_minp |= s.temperature >= 1e-5f && s.min_p > 0.f;
-      if (s.pen_slot >= 0) {
-        pen_.push_back({static_cast<int>(rows_.size()) - 1, s.pen_slot, s.presence, s.frequency, s.repetition, s.n_generated,
-                        s.min_tokens, s.pen_history() ? 1 : 0});
-        m.pen_update |= s.pen_history();
-      }
-      if (s.top_logprobs >= 0) {
-        lp_rows_.push_back(static_cast<int>(rows_.size()) - 1);
-        lp_n_.push_back(s.top_logprobs);
+    if (p0 + n - nd == static_cast<int>(s.toks.size())) {
+      // row j (0..nd) of a verify is drawn as the token with index n_generated + j: accepting draft j exactly when it
+      // equals row j's token gives the stream the non-speculative steps would
+      for (int j = 0; j <= nd; ++j) {
+        rows_.push_back(tok + n - 1 - nd + j);
+        // n = the index of the token this row generates: a request recomputed after preemption draws the same noise
+        samp_.push_back({s.temperature, s.top_k, s.top_p, static_cast<uint32_t>(s.seed), static_cast<uint32_t>(s.seed >> 32),
+                         s.n_generated + j, s.min_p});
+        any_sampled |= s.temperature >= 1e-5f;
+        any_minp |= s.temperature >= 1e-5f && s.min_p > 0.f;
+        if (s.pen_slot >= 0) {
+          pen_.push_back({static_cast<int>(rows_.size()) - 1, s.pen_slot, s.presence, s.frequency, s.repetition, s.n_generated + j,
+                          s.min_tokens, s.pen_history() ? 1 : 0});
+          m.pen_update |= s.pen_history();
+        }
+        if (s.top_logprobs >= 0) {
+          lp_rows_.push_back(static_cast<int>(rows_.size()) - 1);
+          lp_n_.push_back(s.top_logprobs);
+        }
       }
       if (!s.children.empty()) {
         // the fork: the last prompt position is sampled once more for every member that forks, each row with the member's
@@ -1276,7 +1387,7 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
   std::stable_sort(dwork_.begin(), dwork_.end(), longer);
   std::stable_sort(pwork_.begin(), pwork_.end(), longer);
   m.nd = static_cast<int>(dwork_.size());
-  m.dmax_ctx = m.nd ? dwork_[0].q_pos0 + 1 : 0;   // sorted longest-first
+  m.dmax_ctx = m.nd ? dwork_[0].q_pos0 + dwork_[0].q_count : 0;   // sorted longest-first
   m.np = static_cast<int>(pwork_.size());
   m.S = static_cast<int>(rows_.size());
   m.out_tokens = m.S;
@@ -1389,19 +1500,24 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
 
   int ri = 0, li = 0, pi = 0;
   int64_t gen = 0;
+  int step_accepted = 0, step_verifies = 0;
+  int64_t step_accepted_pos[B200_MAX_SPEC_TOKENS] = {};
   bool any_done = false;
   for (int si = 0; si < m.nseq; ++si) {
     const std::shared_ptr<Seq>& sp = f.sched[si].s;
     Seq& s = *sp;
-    const int n = f.sched[si].n;
-    const bool samples = (s.n_computed + n == static_cast<int>(s.toks.size()));
-    s.n_computed += n;
+    const int n = f.sched[si].n, nd = f.sched[si].n_draft;
+    const bool samples = (s.n_computed + n - nd == static_cast<int>(s.toks.size()));
+    s.n_computed += n - nd;
     // publish newly full blocks to the prefix cache
-    while ((s.n_published + 1) * kPage <= s.n_computed) {
-      const int b = s.n_published;
-      s.chain_uid = pool.publish(s.blocks[b], s.chain_uid, &s.toks[static_cast<size_t>(b) * kPage]);
-      ++s.n_published;
-    }
+    auto publish_blocks = [&] {
+      while ((s.n_published + 1) * kPage <= s.n_computed) {
+        const int b = s.n_published;
+        s.chain_uid = pool.publish(s.blocks[b], s.chain_uid, &s.toks[static_cast<size_t>(b) * kPage]);
+        ++s.n_published;
+      }
+    };
+    publish_blocks();
     // prompt records come back in step order; they are published with (or before) the first generated token
     const int plp0 = static_cast<int>(pending_plp.size()), n_plp = f.sched[si].n_plp;
     for (int k = 0; k < n_plp; ++k, ++pi) {
@@ -1441,6 +1557,38 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
       }
       return code;
     };
+    if (nd > 0) {
+      // a speculative verify: emit row j's token t_j for j = 0..nd, stopping after t_j when it differs from draft j, when it
+      // finishes the request, or at the last row.  Every emitted token is the one the non-speculative steps would give.
+      int code = 0, emitted = 0, accepted = 0;
+      for (int j = 0; j <= nd; ++j) {
+        int32_t t = 0;
+        int lp = -1;
+        code = take(s, &t, &lp);
+        pending_pub.push_back({sp, t, true, code, lp, j == 0 ? plp0 : 0, j == 0 ? n_plp : 0});
+        ++emitted;
+        const bool match = j < nd && t == s.draft[j];
+        if (match) ++step_accepted_pos[j];
+        accepted += match;
+        if (code || !match) break;
+      }
+      // the rows after the last emitted one are skipped, but their ids and records were copied back in step order
+      ri += nd + 1 - emitted;
+      if (s.top_logprobs >= 0) li += nd + 1 - emitted;
+      // KV at positions p0 .. p0 + emitted - 1 came from the last token and the drafts that equal the emitted tokens.  The
+      // KV a rejected draft left at a later position is never read: attention masks by position, and the next step
+      // writes that position before its attention reads it.
+      s.n_computed += emitted - 1;
+      publish_blocks();
+      ++step_verifies;
+      step_accepted += accepted;
+      if (code) {
+        release_blocks(s);
+        s.leaving = true;
+        any_done = true;
+      }
+      continue;
+    }
     int32_t t = 0;
     int lp = -1;
     int code = take(s, &t, &lp);
@@ -1505,6 +1653,10 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
     std::lock_guard<std::mutex> lk(mu_);
     ++stats.steps;
     stats.generated_tokens += gen;
+    stats.spec_drafts += step_verifies;
+    stats.spec_draft_tokens += m.draft_tokens;
+    stats.spec_accepted_tokens += step_accepted;
+    for (int j = 0; j < B200_MAX_SPEC_TOKENS; ++j) stats.spec_accepted_per_pos[j] += step_accepted_pos[j];
     stats.last_step_device_us = ms * 1000.0;
     stats.total_device_us += ms * 1000.0;
     stats.last_step_tokens = m.T;
@@ -1532,6 +1684,8 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
     info->sampled = m.S;
     info->kv_tokens_read = m.kv_tokens;
     info->device_us = ms * 1000.0;
+    info->draft_tokens = m.draft_tokens;
+    info->accepted_tokens = step_accepted;
   }
   return 1;
 }
@@ -1667,6 +1821,10 @@ void b200_config_default(b200_config* c) {
 
 int b200_engine_create(const b200_config* cfg, b200_engine** out) {
   if (!cfg || !out) { set_error("null argument"); return B200_ERR_INVALID; }
+  {
+    int k, mn, mx;   // checked before the device so that a bad speculative config reads the same on every host
+    if (int rc = spec_resolve(*cfg, &k, &mn, &mx)) return rc;
+  }
   if (int rc = require_device()) return rc;
   b200_engine* e = new (std::nothrow) b200_engine();
   if (!e) { set_error("host OOM"); return B200_ERR_OOM; }
@@ -1677,6 +1835,15 @@ int b200_engine_create(const b200_config* cfg, b200_engine** out) {
 }
 
 void b200_engine_destroy(b200_engine* e) { delete e; }
+
+int32_t b200_ngram_propose(const int32_t* toks, int32_t n, int32_t min_n, int32_t max_n, int32_t k, int32_t max_model_len,
+                           int32_t* out) {
+  if (!toks || !out || n < 0 || min_n < 1 || max_n < min_n || k < 0) {
+    set_error("b200_ngram_propose: bad arguments (n=%d min_n=%d max_n=%d k=%d)", n, min_n, max_n, k);
+    return B200_ERR_INVALID;
+  }
+  return ngram_propose(toks, n, min_n, max_n, k, max_model_len, out);
+}
 
 // b200_submit (members 1) and b200_submit_n
 static int submit_impl(b200_engine* e, const int32_t* prompt_ids, int32_t n, const b200_sampling* sp, int32_t members,

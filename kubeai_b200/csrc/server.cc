@@ -954,6 +954,19 @@ static std::string metrics_text(Server& sv) {
              (long long)st.prompt_tokens, i, (long long)st.cached_prompt_tokens, i, (long long)st.generated_tokens, i,
              (long long)st.preemptions, i, st.last_step_device_us);
     o += b;
+    // speculative decoding, vLLM's counters vllm:spec_decode_num_drafts, vllm:spec_decode_num_draft_tokens,
+    // vllm:spec_decode_num_accepted_tokens and vllm:spec_decode_num_accepted_tokens_per_pos{position} (zero when off)
+    snprintf(b, sizeof(b),
+             "b200_engine_spec_decode_num_drafts_total{replica=\"%zu\"} %lld\n"
+             "b200_engine_spec_decode_num_draft_tokens_total{replica=\"%zu\"} %lld\n"
+             "b200_engine_spec_decode_num_accepted_tokens_total{replica=\"%zu\"} %lld\n",
+             i, (long long)st.spec_drafts, i, (long long)st.spec_draft_tokens, i, (long long)st.spec_accepted_tokens);
+    o += b;
+    for (int j = 0; j < B200_MAX_SPEC_TOKENS; ++j) {
+      snprintf(b, sizeof(b), "b200_engine_spec_decode_num_accepted_tokens_per_pos_total{replica=\"%zu\",position=\"%d\"} %lld\n", i, j,
+               (long long)st.spec_accepted_per_pos[j]);
+      o += b;
+    }
   }
   return o;
 }
@@ -1245,6 +1258,52 @@ int b200_server_listen(b200_server* s, const char* host, int32_t port, int32_t* 
       std::thread(serve_conn, &sv, c).detach();
     }
   });
+  return 0;
+}
+
+int b200_speculative_config_parse(const char* json, b200_config* cfg) {
+  if (!json || !cfg) { set_error("b200_speculative_config_parse: bad arguments"); return B200_ERR_INVALID; }
+  JVal v;
+  std::string err;
+  JParser jp(json, strlen(json));
+  if (!jp.parse(&v, &err)) { set_error("speculative-config: %s", err.c_str()); return B200_ERR_INVALID; }
+  if (v.type != JVal::Obj) { set_error("speculative-config: expected a JSON object"); return B200_ERR_INVALID; }
+  int k = 0, mn = 0, mx = 0;
+  bool has_method = false;
+  for (auto& kv : v.obj) {
+    const JVal& x = kv.second;
+    if (kv.first == "method") {
+      if (x.type != JVal::Str || x.str != "ngram") {
+        set_error("speculative-config: only \"method\": \"ngram\" is supported (got %s)", x.type == JVal::Str ? x.str.c_str() : "a non-string");
+        return B200_ERR_INVALID;
+      }
+      has_method = true;
+    } else if (kv.first == "num_speculative_tokens" || kv.first == "prompt_lookup_min" || kv.first == "prompt_lookup_max") {
+      const bool lookup = kv.first != "num_speculative_tokens";
+      if (lookup && x.is_null()) continue;   // unset
+      if (x.type != JVal::Num || !x.is_int || x.num < 1 || x.num > 1e6) {
+        set_error("speculative-config: %s must be an integer >= 1", kv.first.c_str());
+        return B200_ERR_INVALID;
+      }
+      (kv.first == "num_speculative_tokens" ? k : kv.first == "prompt_lookup_min" ? mn : mx) = static_cast<int>(x.num);
+    } else {
+      set_error("speculative-config: unsupported key \"%s\" (the ngram method takes num_speculative_tokens, "
+                "prompt_lookup_min and prompt_lookup_max)", kv.first.c_str());
+      return B200_ERR_INVALID;
+    }
+  }
+  if (!has_method) { set_error("speculative-config: \"method\" is required (only \"ngram\" is supported)"); return B200_ERR_INVALID; }
+  if (k < 1 || k > B200_MAX_SPEC_TOKENS) {
+    set_error("speculative-config: num_speculative_tokens must be in 1..%d for the ngram method, got %d", B200_MAX_SPEC_TOKENS, k);
+    return B200_ERR_INVALID;
+  }
+  if (mn && mx && mn > mx) {
+    set_error("speculative-config: prompt_lookup_min=%d must be <= prompt_lookup_max=%d", mn, mx);
+    return B200_ERR_INVALID;
+  }
+  cfg->num_speculative_tokens = k;
+  cfg->prompt_lookup_min = mn;
+  cfg->prompt_lookup_max = mx;
   return 0;
 }
 

@@ -50,6 +50,18 @@ func New(device int, cfg func(*C.b200_config)) (*Engine, error) {
 	return &Engine{h}, nil
 }
 
+// SpeculativeConfig applies vLLM's --speculative-config JSON (the "ngram" method only; KubeAI passes it through
+// Model.spec.args) to an engine config; use it inside New's cfg callback.  Without it speculation stays off, the
+// b200_config_default setting.
+func SpeculativeConfig(c *C.b200_config, json string) error {
+	s := C.CString(json)
+	defer C.free(unsafe.Pointer(s))
+	if rc := C.b200_speculative_config_parse(s, c); rc != 0 {
+		return errors.New(C.GoString(C.b200_last_error()))
+	}
+	return nil
+}
+
 // Token-level API (what a Go-side SSE writer would use): submit, then wait+poll until finished.
 func (e *Engine) Submit(ids []int32, maxTokens int) (uint64, error) {
 	sp := C.b200_sampling{max_tokens: C.int32_t(maxTokens), ignore_eos: 0}
