@@ -68,13 +68,16 @@ typedef struct {
    * to num_speculative_tokens drafts, the tokens that followed the longest suffix n-gram (prompt_lookup_min..max tokens)
    * at the earliest of its longest earlier occurrences in the context (vLLM's tie rule), and the step verifies them; a draft is accepted exactly when it
    * equals the token the sampler draws from its row, so the output stream is the non-speculative one.
-   * num_speculative_tokens: 0 = off, else 1..B200_MAX_SPEC_TOKENS.  Lookup lengths: 0 = unset (both unset: 5 and 5; one
-   * unset takes the other's value); 1 <= min <= max otherwise B200_ERR_INVALID at b200_engine_create. */
+   * num_speculative_tokens: 0 = off, else 1..k_max(G), k_max(G) = min(B200_MAX_SPEC_TOKENS, 16 / G - 1) with G =
+   * q_heads / kv_heads (3 for G <= 4, 2 for G = 5, 1 for G = 6..8, 0 above).  Lookup lengths: 0 = unset (both unset: 5 and
+   * 5; one unset takes the other's value); 1 <= min <= max otherwise B200_ERR_INVALID at b200_engine_create. */
   int32_t num_speculative_tokens;
   int32_t prompt_lookup_min, prompt_lookup_max;
 } b200_config;
 
-#define B200_MAX_SPEC_TOKENS 3   /* drafts per step: the last token and 3 drafts fill decode attention's 16-row tile */
+/* drafts per step at most: a verify item's G query heads times its 1 + m positions share decode attention's 16-row tile,
+ * so 3 drafts fill it at G = 4 and fewer fit at larger G (k_max(G) above) */
+#define B200_MAX_SPEC_TOKENS 3
 
 /* Sampling follows vLLM V1 (vllm/v1/sample/sampler.py, ops/topk_topp_sampler.py), made deterministic: the token is a pure
  * function of the logits row, these parameters, the seed and the index of the token in the generation (csrc/sampling.cu).
@@ -246,7 +249,8 @@ int b200_engine_read_logits(b200_engine* e, void* host_logits_bf16, int32_t rows
 /* ------------------------------------------------------------------ checkpoints (SURVEY.md §8f-2)
  * HF-layout Llama checkpoints: <dir>/config.json + model.safetensors[.index.json] (BF16/F16/F32 tensors).
  * The reference mounts such a directory into the backend pod (internal/modelcontroller/model_source.go:231-287). */
-/* Fill the architecture fields of cfg from <dir>/config.json; rejects head_dim != 128 and GQA != 4:1. */
+/* Fill the architecture fields of cfg from <dir>/config.json; rejects head_dim != 128 and a GQA ratio whose kv_heads does
+ * not divide q_heads or that has more than 16 query heads per KV head. */
 int b200_config_from_hf(const char* dir, b200_config* cfg);
 /* Replace the seeded weights of an idle engine with the checkpoint's (q/k/v and gate/up fused on load). */
 int b200_engine_load_safetensors(b200_engine* e, const char* path);
@@ -523,20 +527,22 @@ typedef struct {
   const int32_t* stop_ids;
 } b200_penalty_row;
 int b200_op_penalize(void* logits, int32_t ld, int32_t S, int32_t V, const b200_penalty_row* rows, void* edited, void* stream);
-/* work: int32[num_work][4] = {q_tok0, q_count, q_pos0, seq}; kv_layer: [block][2][kv_heads][16][128].  decode = 1: every
- * item has 1 <= q_count <= B200_MAX_SPEC_TOKENS + 1 consecutive query positions (a speculative verify), position j masked
- * causally at q_pos0 + j, and the item's K/V read once for all of them; decode = 0: q_count <= 16. */
+/* work: int32[num_work][4] = {q_tok0, q_count, q_pos0, seq}; kv_layer: [block][2][kv_heads][16][128]; kv_heads divides
+ * q_heads and G = q_heads / kv_heads is 1..16.  decode = 1: every item has 1 <= q_count <= 16 / G consecutive query
+ * positions (a speculative verify), position j masked causally at q_pos0 + j, and the item's K/V read once for all of
+ * them; decode = 0: q_count <= 16 and G = 4 only (B200_ERR_INVALID otherwise). */
 int b200_op_paged_attn(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                        const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
                        int32_t q_heads, int32_t kv_heads, float scale, int32_t decode, void* stream);
 /* Decode attention with each work item's context split over `split` >= 1 CTAs per KV head (what the engine does when a step
  * has fewer decoding sequences than the device has SMs / kv_heads) and a merge of the partial softmax states.  Work items
- * as b200_op_paged_attn with decode = 1 (q_count up to B200_MAX_SPEC_TOKENS + 1). */
+ * and group sizes as b200_op_paged_attn with decode = 1 (q_count up to 16 / G). */
 int b200_op_paged_attn_decode_split(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                                     const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
                                     int32_t q_heads, int32_t kv_heads, float scale, int32_t split, void* stream);
 /* Chunked-prefill attention on wgmma (csrc/attention_wgmma.cu): work items (q_tok0, q_count <= 64, q_pos0, seq), one CTA per
- * (work item, q head); q rows are read from the fused qkv buffer [q_rows, ldq] (q heads first). */
+ * (work item, q head h, reading KV head h / G, G = q_heads / kv_heads in 1..16); q rows are read from the fused qkv buffer
+ * [q_rows, ldq] (q heads first). */
 int b200_op_paged_attn_prefill_tc(const void* qkv, int32_t q_rows, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                                   const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
                                   int32_t q_heads, int32_t kv_heads, float scale, void* stream);

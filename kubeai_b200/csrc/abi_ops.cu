@@ -342,6 +342,16 @@ int b200_op_paged_attn(const void* q, int32_t ldq, void* out, int32_t ldo, const
                        int32_t q_heads, int32_t kv_heads, float scale, int32_t decode, void* stream) {
   if (int rc = require_device()) return rc;
   static_assert(sizeof(AttnWork) == 16, "AttnWork is int32[4] on the wire");
+  if (!attn_group_ok(q_heads, kv_heads)) {
+    set_error("b200_op_paged_attn: q_heads=%d kv_heads=%d: kv_heads must divide q_heads with 1..16 query heads per KV head",
+              q_heads, kv_heads);
+    return B200_ERR_INVALID;
+  }
+  if (!decode && q_heads != 4 * kv_heads) {
+    set_error("b200_op_paged_attn: the prefill form (decode = 0) serves 4 query heads per KV head only, got %d:%d; "
+              "chunked prefill of any group size is b200_op_paged_attn_prefill_tc", q_heads, kv_heads);
+    return B200_ERR_INVALID;
+  }
   int rc = paged_attention(q, ldq, out, ldo, kv_layer, block_tables, max_blocks,
                            reinterpret_cast<const AttnWork*>(work), num_work, q_heads, kv_heads, scale, decode,
                            static_cast<cudaStream_t>(stream));
@@ -352,12 +362,15 @@ int b200_op_paged_attn_decode_split(const void* q, int32_t ldq, void* out, int32
                                     const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
                                     int32_t q_heads, int32_t kv_heads, float scale, int32_t split, void* stream) {
   if (int rc = require_device()) return rc;
-  if (split < 1 || split > 64 || num_work <= 0) { set_error("b200_op_paged_attn_decode_split: bad arguments"); return B200_ERR_INVALID; }
+  if (split < 1 || split > 64 || num_work <= 0 || !attn_group_ok(q_heads, kv_heads)) {
+    set_error("b200_op_paged_attn_decode_split: bad arguments");
+    return B200_ERR_INVALID;
+  }
   static float* ws = nullptr;
   static size_t ws_bytes = 0;
   static std::mutex mu;
   std::lock_guard<std::mutex> lk(mu);
-  const size_t need = attn_split_ws_bytes(num_work, kv_heads, split, kMaxDecodeQ);
+  const size_t need = attn_split_ws_bytes(num_work, q_heads, split, kDecodeRows / (q_heads / kv_heads));
   if (need > ws_bytes) {
     cudaDeviceSynchronize();
     if (ws) cudaFree(ws);

@@ -1,6 +1,6 @@
 // Paged causal attention for the per-step hot path (SURVEY.md §8a K6 decode, K7 chunked prefill).
 // Computes softmax(q . K^T / sqrt(128)) . V over the tokens reachable through a sequence's block
-// table, GQA 4:1 — the operation the reference backend delegates to FlashInfer/FlashAttention
+// table, with G = Hq / Hkv query heads per KV head — the operation the reference backend delegates to FlashInfer/FlashAttention
 // (vllm/model_executor/models/llama.py:223-233, vllm/v1/attention/backends/flashinfer.py).
 //
 // Design: this op is an HBM stream (decode reads 4 KiB of K+V per context token per layer),
@@ -10,15 +10,17 @@
 //     64-token tile (4 pages x {K,V} x two 64-column halves = 16 TMA boxes of 2 KiB, 128-byte swizzle)
 //     and signals an mbarrier.  The per-thread cp.async gather this replaces spent ~45% of the kernel's
 //     issue slots on address arithmetic (ncu: issue-active 43% at 12 warps/SM, 4.8 TB/s).
-//   * the 4 query heads of a KV head ride in one m16n8k16 tensor-core tile so K/V bytes are read
-//     once per group (fp32 softmax, warp-shuffle row reductions, P rounded to bf16 for P.V).
-//   * decode: the CTA's 4 warps each own a 16-token strip of every tile and merge their
-//     (max, sum, acc) through smem at the end; prefill: a CTA owns 16 query tokens x 4 heads, one
-//     head per warp, and walks the causal prefix.
-//   * a decode work item may carry up to 4 consecutive query positions (speculative decoding's verify
-//     step: the last token and up to 3 drafts).  Tile row r = 4 * j + h is head h at position j, so the
-//     16 rows of the tile that a single-position decode leaves zero hold them, and the K/V of the group
-//     is still read once.  Fragment rows g cover positions 0/1, rows g + 8 positions 2/3.
+//   * decode: the G query heads of a KV head (1 <= G <= 16) ride in one m16n8k16 tensor-core tile so
+//     K/V bytes are read once per group (fp32 softmax, warp-shuffle row reductions, P rounded to bf16
+//     for P.V).  The CTA's 4 warps each own a 16-token strip of every tile and merge their
+//     (max, sum, acc) through smem at the end.
+//   * a decode work item may carry q_count consecutive query positions with G * q_count <= 16
+//     (speculative decoding's verify step: the last token and its drafts).  Tile row r = G * j + h is
+//     head kvh * G + h at position j; rows past G * q_count stay zero, and the K/V of the group is still
+//     read once.  The decode kernel is compiled twice: for G = 4 (the row map folds to shifts and masks)
+//     and for a group size read at run time.
+//   * prefill (op-level only, G = 4): a CTA owns 16 query tokens x 4 heads, one head per warp, and
+//     walks the causal prefix.
 // Rows of a page that lie beyond the sequence's last token are loaded as they are in HBM and masked; the pool is
 // zero-initialised and only ever holds finite K/V values, so a masked probability of 0 never meets a NaN.
 #include <cuda.h>
@@ -51,13 +53,16 @@ constexpr int attn_smem_bytes() {
   return S * kStageBytes + 64 + 1024;  // stages + mbarriers + slack for the 1 KiB alignment the swizzle needs
 }
 
-template <bool DECODE, int S>  // S = tiles in flight per CTA
+// S = tiles in flight per CTA; GC = the group size G when it is known at compile time (4), 0 = read G from group
+template <bool DECODE, int S, int GC>
 __global__ void __launch_bounds__(128)
 paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16* __restrict__ q, int ldq,
                   __nv_bfloat16* __restrict__ out, int ldo, const int* __restrict__ block_tables, int max_blocks,
-                  const AttnWork* __restrict__ work, int Hkv, float scale_log2, float* __restrict__ split_ws) {
+                  const AttnWork* __restrict__ work, int Hkv, int group, float scale_log2, float* __restrict__ split_ws) {
+  static_assert(DECODE || GC == 4, "the prefill form is specialised for G = 4");
   constexpr int WT = DECODE ? 16 : 64;  // tokens of each tile handled by one warp
   constexpr int NT = WT / 8;
+  const int G = GC ? GC : group;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem = smem_raw + (sbase - smem_u32(smem_raw));
@@ -127,15 +132,17 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
   if (!waited) griddep_enter();
 
   // ---- Q fragments (A operand, 16 rows x 128 d as 8 k-steps)
+  // decode: fragment rows g and g + 8 are tile rows r = G * j + h, i.e. (j, h) = divmod(r, G); prefill: query tokens
+  const int j0 = DECODE ? g / G : g, j1 = DECODE ? (g + 8) / G : g + 8;
   uint32_t qf[8][4];
   {
     const __nv_bfloat16* r0p = nullptr;
     const __nv_bfloat16* r1p = nullptr;
     if (DECODE) {
-      // rows of positions past q_count stay zero: they never touch the rows of the positions that exist
-      const int j0 = g >> 2, j1 = 2 + (g >> 2), head = kvh * 4 + (g & 3);
-      if (j0 < wk.q_count) r0p = q + static_cast<size_t>(wk.q_tok0 + j0) * ldq + head * kD;
-      if (j1 < wk.q_count) r1p = q + static_cast<size_t>(wk.q_tok0 + j1) * ldq + head * kD;
+      // rows past the live ones (G * q_count) stay zero: they never touch the rows of the positions that exist
+      const int nrows = G * wk.q_count;
+      if (g < nrows) r0p = q + static_cast<size_t>(wk.q_tok0 + j0) * ldq + (kvh * G + g - j0 * G) * kD;
+      if (g + 8 < nrows) r1p = q + static_cast<size_t>(wk.q_tok0 + j1) * ldq + (kvh * G + g + 8 - j1 * G) * kD;
     } else {
       const int head = kvh * 4 + warp;
       if (g < wk.q_count) r0p = q + static_cast<size_t>(wk.q_tok0 + g) * ldq + head * kD;
@@ -187,8 +194,8 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
         }
       }
       // ---- causal mask, online softmax (fp32, base-2)
-      const int qp0 = DECODE ? wk.q_pos0 + (g >> 2) : wk.q_pos0 + g;
-      const int qp1 = DECODE ? wk.q_pos0 + 2 + (g >> 2) : wk.q_pos0 + g + 8;
+      const int qp0 = DECODE ? wk.q_pos0 + j0 : wk.q_pos0 + g;
+      const int qp1 = DECODE ? wk.q_pos0 + j1 : wk.q_pos0 + g + 8;
       float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
       for (int nt = 0; nt < NT; ++nt) {
@@ -272,12 +279,12 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
         *reinterpret_cast<uint32_t*>(dst + dn * 8) = pack_bf16x2(o[dn][2] * i1, o[dn][3] * i1);
     }
   } else {
-    // merge the 4 warps' partial softmax states: row r = 4 * j + h of each warp tile is head h at query position j.  The
-    // stages are free here (the loop's last barrier followed the last tile, and no gather is in flight).
+    // merge the 4 warps' partial softmax states: row r = G * j + h of each warp tile is head kvh * G + h at query position
+    // j.  The stages are free here (the loop's last barrier followed the last tile, and no gather is in flight).
     float* so = reinterpret_cast<float*>(smem);            // [4 warps][16 rows][128]
     float* sm = so + 4 * 16 * kD;                          // [4][16]
     float* sl = sm + 4 * 16;                               // [4][16]
-    const int nrows = 4 * wk.q_count;
+    const int nrows = G * wk.q_count;
     if (g < nrows) {
 #pragma unroll
       for (int dn = 0; dn < 16; ++dn) {
@@ -303,7 +310,7 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
     __syncthreads();
     const int d = tid;
     for (int r = 0; r < nrows; ++r) {
-      const int j = r >> 2, h = r & 3;
+      const int j = r / G, h = r - j * G;
       float mm = -INFINITY;
 #pragma unroll
       for (int w = 0; w < 4; ++w) mm = fmaxf(mm, sm[w * 16 + r]);
@@ -316,12 +323,12 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
         den += sl[w * 16 + r] * wgt;
       }
       if (parts == 1) {
-        out[static_cast<size_t>(wk.q_tok0 + j) * ldo + (kvh * 4 + h) * kD + d] = __float2bfloat16_rn(den > 0.f ? num / den : 0.f);
+        out[static_cast<size_t>(wk.q_tok0 + j) * ldo + (kvh * G + h) * kD + d] = __float2bfloat16_rn(den > 0.f ? num / den : 0.f);
       } else {
-        // position j's slab of [position][work][kv head][part][4 heads][128 acc | max | sum]: a launch whose items all
+        // position j's slab of [position][work][kv head][part][G heads][128 acc | max | sum]: a launch whose items all
         // have q_count == 1 uses slab 0 only
-        const size_t slab = static_cast<size_t>(gridDim.y) * Hkv * parts * (4 * (kD + 2));
-        float* dst = split_ws + j * slab + ((static_cast<size_t>(blockIdx.y) * Hkv + kvh) * parts + part) * (4 * (kD + 2)) +
+        const size_t slab = static_cast<size_t>(gridDim.y) * Hkv * parts * (G * (kD + 2));
+        float* dst = split_ws + j * slab + ((static_cast<size_t>(blockIdx.y) * Hkv + kvh) * parts + part) * (G * (kD + 2)) +
                      h * (kD + 2);
         dst[d] = num;
         if (d == 0) {
@@ -336,24 +343,24 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
 // out[token, head, :] = sum_p acc_p 2^(m_p - M) / sum_p l_p 2^(m_p - M) over the parts of a split decode work item
 __global__ void __launch_bounds__(128)
 attn_merge_kernel(const float* __restrict__ split_ws, __nv_bfloat16* __restrict__ out, int ldo, const AttnWork* __restrict__ work,
-                  int Hkv, int parts) {
+                  int Hkv, int G, int parts) {
   griddep_enter();
   const AttnWork wk = work[blockIdx.y];
   const int kvh = blockIdx.x, d = threadIdx.x;
-  const size_t slab = static_cast<size_t>(gridDim.y) * Hkv * parts * (4 * (kD + 2));
-  for (int r = 0; r < 4 * wk.q_count; ++r) {
-    const int j = r >> 2, h = r & 3;
-    const float* base = split_ws + j * slab + (static_cast<size_t>(blockIdx.y) * Hkv + kvh) * parts * (4 * (kD + 2));
+  const size_t slab = static_cast<size_t>(gridDim.y) * Hkv * parts * (G * (kD + 2));
+  for (int r = 0; r < G * wk.q_count; ++r) {
+    const int j = r / G, h = r - j * G;
+    const float* base = split_ws + j * slab + (static_cast<size_t>(blockIdx.y) * Hkv + kvh) * parts * (G * (kD + 2));
     float mm = -INFINITY;
-    for (int p = 0; p < parts; ++p) mm = fmaxf(mm, base[(p * 4 + h) * (kD + 2) + kD]);
+    for (int p = 0; p < parts; ++p) mm = fmaxf(mm, base[(p * G + h) * (kD + 2) + kD]);
     float num = 0.f, den = 0.f;
     for (int p = 0; p < parts; ++p) {
-      const float* s = base + (p * 4 + h) * (kD + 2);
+      const float* s = base + (p * G + h) * (kD + 2);
       const float wgt = (s[kD] == -INFINITY) ? 0.f : exp2f(s[kD] - mm);
       num += s[d] * wgt;
       den += s[kD + 1] * wgt;
     }
-    out[static_cast<size_t>(wk.q_tok0 + j) * ldo + (kvh * 4 + h) * kD + d] = __float2bfloat16_rn(den > 0.f ? num / den : 0.f);
+    out[static_cast<size_t>(wk.q_tok0 + j) * ldo + (kvh * G + h) * kD + d] = __float2bfloat16_rn(den > 0.f ? num / den : 0.f);
   }
 }
 
@@ -391,27 +398,38 @@ int kv_map_for(const void* kv_layer, CUtensorMap* out) {
 
 namespace {
 
-template <bool DECODE, int S>
+template <bool DECODE, int S, int GC>
 int launch_attn(const CUtensorMap& tm, dim3 grid, cudaStream_t st, const __nv_bfloat16* q, int ldq, __nv_bfloat16* out,
-                int ldo, const int* block_tables, int max_blocks, const AttnWork* work, int Hkv, float scale_log2,
+                int ldo, const int* block_tables, int max_blocks, const AttnWork* work, int Hkv, int G, float scale_log2,
                 float* split_ws = nullptr) {
   static std::atomic<unsigned long long> attr_done{0};
-  if (!ensure_dynamic_smem(paged_attn_kernel<DECODE, S>, attn_smem_bytes<S>(), &attr_done)) return -3;
-  launch_pdl(paged_attn_kernel<DECODE, S>, grid, dim3(128), attn_smem_bytes<S>(), st, tm, q, ldq, out, ldo, block_tables,
-             max_blocks, work, Hkv, scale_log2, split_ws);
+  if (!ensure_dynamic_smem(paged_attn_kernel<DECODE, S, GC>, attn_smem_bytes<S>(), &attr_done)) return -3;
+  launch_pdl(paged_attn_kernel<DECODE, S, GC>, grid, dim3(128), attn_smem_bytes<S>(), st, tm, q, ldq, out, ldo, block_tables,
+             max_blocks, work, Hkv, G, scale_log2, split_ws);
   if (cudaGetLastError() != cudaSuccess) return -2;
   if (DECODE && grid.z > 1) {
     launch_pdl(attn_merge_kernel, dim3(grid.x, grid.y), dim3(128), 0, st, static_cast<const float*>(split_ws), out, ldo, work, Hkv,
-               static_cast<int>(grid.z));
+               G, static_cast<int>(grid.z));
     if (cudaGetLastError() != cudaSuccess) return -2;
   }
   return 0;
 }
 
+template <int GC>
+int launch_decode(const CUtensorMap& tm, dim3 grid, cudaStream_t st, const __nv_bfloat16* q, int ldq, __nv_bfloat16* out,
+                  int ldo, const int* block_tables, int max_blocks, const AttnWork* work, int Hkv, int G, float scale_log2,
+                  float* split_ws) {
+  switch (decode_stages()) {
+    case 3: return launch_attn<true, 3, GC>(tm, grid, st, q, ldq, out, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
+    case 4: return launch_attn<true, 4, GC>(tm, grid, st, q, ldq, out, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
+    default: return launch_attn<true, 2, GC>(tm, grid, st, q, ldq, out, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
+  }
+}
+
 }  // namespace
 
-size_t attn_split_ws_bytes(int num_work, int Hkv, int parts, int max_q) {
-  return static_cast<size_t>(max_q) * num_work * Hkv * parts * 4 * (kD + 2) * sizeof(float);
+size_t attn_split_ws_bytes(int num_work, int Hq, int parts, int max_q) {
+  return static_cast<size_t>(max_q) * num_work * Hq * parts * (kD + 2) * sizeof(float);
 }
 
 // Parts per decode work item such that the launch has about two CTAs per SM, each with at least two 64-token tiles.
@@ -429,8 +447,9 @@ int paged_attention(const void* q, int ldq, void* out, int ldo, const void* kv_l
                     int max_blocks, const AttnWork* work, int num_work, int Hq, int Hkv, float scale,
                     int decode, cudaStream_t st, float* split_ws, int split) {
   if (num_work <= 0) return 0;
-  if (Hq != 4 * Hkv) return -1;
+  if (!attn_group_ok(Hq, Hkv) || (!decode && Hq != 4 * Hkv)) return -1;
   if (split > 1 && (!decode || !split_ws)) return -1;
+  const int G = Hq / Hkv;
   CUtensorMap tm;
   if (int rc = kv_map_for(kv_layer, &tm)) return rc;
   const float scale_log2 = scale * 1.4426950408889634f;
@@ -438,12 +457,9 @@ int paged_attention(const void* q, int ldq, void* out, int ldo, const void* kv_l
   const __nv_bfloat16* qq = static_cast<const __nv_bfloat16*>(q);
   __nv_bfloat16* oo = static_cast<__nv_bfloat16*>(out);
   if (!decode)
-    return launch_attn<false, kPrefillStages>(tm, grid, st, qq, ldq, oo, ldo, block_tables, max_blocks, work, Hkv, scale_log2);
-  switch (decode_stages()) {
-    case 3: return launch_attn<true, 3>(tm, grid, st, qq, ldq, oo, ldo, block_tables, max_blocks, work, Hkv, scale_log2, split_ws);
-    case 4: return launch_attn<true, 4>(tm, grid, st, qq, ldq, oo, ldo, block_tables, max_blocks, work, Hkv, scale_log2, split_ws);
-    default: return launch_attn<true, 2>(tm, grid, st, qq, ldq, oo, ldo, block_tables, max_blocks, work, Hkv, scale_log2, split_ws);
-  }
+    return launch_attn<false, kPrefillStages, 4>(tm, grid, st, qq, ldq, oo, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2);
+  if (G == 4) return launch_decode<4>(tm, grid, st, qq, ldq, oo, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
+  return launch_decode<0>(tm, grid, st, qq, ldq, oo, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
 }
 
 }  // namespace b200

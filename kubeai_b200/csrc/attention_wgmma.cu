@@ -1,8 +1,9 @@
 // Chunked-prefill paged attention on the Hopper tensor cores (SURVEY.md §8a K7): for every query token of a work item,
-// softmax(q . K^T / sqrt(128)) . V over the causal prefix gathered through the sequence's block table, GQA 4:1 — the
+// softmax(q . K^T / sqrt(128)) . V over the causal prefix gathered through the sequence's block table, with G = Hq / Hkv
+// query heads per KV head (1 <= G <= 16) — the
 // operation the reference backend delegates to FlashInfer/FlashAttention (vllm/model_executor/models/llama.py:223-233).
 //
-// H100 design: one CTA = one warpgroup = (work item of up to 64 query tokens, one query head).
+// H100 design: one CTA = one warpgroup = (work item of up to 64 query tokens, one query head h, reading KV head h / G).
 //   * Q [64 tokens][128] sits in shared memory as two 64-column halves in the 128-byte-swizzled K-major layout wgmma reads;
 //     each 64-token K tile goes to the same layout, V is transposed into [128 dims][64 tokens] (K-major for P . V).
 //   * S = Q K^T: wgmma m64n64k16 with both operands from shared-memory descriptors, fp32 accumulators in registers.
@@ -37,7 +38,8 @@ __global__ void __launch_bounds__(128) prefill_attn_wgmma_kernel(const __nv_bflo
                                                                  __nv_bfloat16* __restrict__ out, int ldo,
                                                                  const __nv_bfloat16* __restrict__ kv_layer,
                                                                  const int* __restrict__ block_tables, int max_blocks,
-                                                                 const AttnWork* __restrict__ work, int Hkv, float scale_log2) {
+                                                                 const AttnWork* __restrict__ work, int Hkv, int G,
+                                                                 float scale_log2) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem = smem_raw + (sbase - smem_u32(smem_raw));
@@ -48,7 +50,7 @@ __global__ void __launch_bounds__(128) prefill_attn_wgmma_kernel(const __nv_bflo
 
   // work[] and block_tables were uploaded before the first kernel of the step: readable ahead of the dependency wait
   const AttnWork wk = work[blockIdx.y];
-  const int h = blockIdx.x, kvh = h >> 2;
+  const int h = blockIdx.x, kvh = h / G;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int* btab = block_tables + static_cast<size_t>(wk.seq) * max_blocks;
   const int kv_end = wk.q_pos0 + wk.q_count;
@@ -193,12 +195,12 @@ __global__ void __launch_bounds__(128) prefill_attn_wgmma_kernel(const __nv_bflo
 int paged_attention_prefill_tc(const void* qkv, int qkv_rows, int ldq, void* out, int ldo, const void* kv_layer, const int* block_tables,
                                int max_blocks, const AttnWork* work, int num_work, int Hq, int Hkv, float scale, cudaStream_t st) {
   if (num_work <= 0) return 0;
-  if (Hq != 4 * Hkv || qkv_rows <= 0 || ldq % 8 || ldo % 2) return -1;
+  if (!attn_group_ok(Hq, Hkv) || qkv_rows <= 0 || ldq % 8 || ldo % 2) return -1;
   static std::atomic<unsigned long long> attr_done{0};
   if (!ensure_dynamic_smem(prefill_attn_wgmma_kernel, kSmem, &attr_done)) return -3;
   cudaError_t e = launch_pdl(prefill_attn_wgmma_kernel, dim3(Hq, num_work), dim3(128), kSmem, st,
                              static_cast<const __nv_bfloat16*>(qkv), qkv_rows, ldq, static_cast<__nv_bfloat16*>(out), ldo,
-                             static_cast<const __nv_bfloat16*>(kv_layer), block_tables, max_blocks, work, Hkv,
+                             static_cast<const __nv_bfloat16*>(kv_layer), block_tables, max_blocks, work, Hkv, Hq / Hkv,
                              scale * 1.4426950408889634f);
   return e == cudaSuccess ? 0 : -2;
 }

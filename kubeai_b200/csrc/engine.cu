@@ -293,12 +293,22 @@ struct XMaps {
 
 // ------------------------------------------------------------------ speculative decoding
 // The speculative settings of a config with vLLM's defaults for the lookup lengths (config/speculative.py: both unset gives
-// 5 and 5, one unset takes the other's value); B200_ERR_INVALID when out of range.
+// 5 and 5, one unset takes the other's value); B200_ERR_INVALID when out of range.  A verify item of the last token and m
+// drafts fills G * (1 + m) rows of decode attention's 16-row tile, so G = q_heads / kv_heads caps the drafts at
+// 16 / G - 1 (a config whose heads the kernels cannot serve is refused by Engine::init).
 int spec_resolve(const b200_config& c, int* k, int* mn, int* mx) {
   *k = *mn = *mx = 0;
   if (c.num_speculative_tokens < 0 || c.num_speculative_tokens > B200_MAX_SPEC_TOKENS) {
     set_error("num_speculative_tokens must be in 0..%d, got %d", B200_MAX_SPEC_TOKENS, c.num_speculative_tokens);
     return B200_ERR_INVALID;
+  }
+  if (attn_group_ok(c.q_heads, c.kv_heads)) {
+    const int G = c.q_heads / c.kv_heads, k_max = std::min(B200_MAX_SPEC_TOKENS, kDecodeRows / G - 1);
+    if (c.num_speculative_tokens > k_max) {
+      set_error("num_speculative_tokens=%d exceeds %d, the most drafts a verify step holds with %d query heads per KV head",
+                c.num_speculative_tokens, k_max, G);
+      return B200_ERR_INVALID;
+    }
   }
   if (c.prompt_lookup_min < 0 || c.prompt_lookup_max < 0) {
     set_error("prompt_lookup_min and prompt_lookup_max must be >= 1 (0 = unset)");
@@ -703,7 +713,7 @@ int Engine::alloc_all() {
   tensors["step.sampled"] = {sampled, static_cast<size_t>(Scap) * 4};
   tensors["step.argmax_candidates"] = {cand, static_cast<size_t>(std::min(Scap, 128)) * ((V + 127) / 128) * sizeof(float2)};
   tensors["step.logits"] = {logits, static_cast<size_t>(Scap) * V * 2};
-  CK(cudaMalloc(&attn_ws, attn_split_ws_bytes(kSplitMaxWork, Hkv, kSplitMaxParts, 1 + spec_k)));
+  CK(cudaMalloc(&attn_ws, attn_split_ws_bytes(kSplitMaxWork, Hq, kSplitMaxParts, 1 + spec_k)));
   { const char* e = getenv("B200_ATTN_SPLIT"); attn_split_force = e ? atoi(e) : 0; }
   // split-K workspace and arrival counters: the largest need of any projection at any step size up to Tcap
   {
@@ -827,10 +837,10 @@ int Engine::init(const b200_config& c) {
   // the constraints of every kernel the forward launches, checked here so that a bad shape fails at create time with a
   // message instead of poisoning the replica at its first step: RMSNorm rows are 256-element multiples up to 8192,
   // argmax and the partial readers use 8-element vectors, GEMM K dims are 64-element TMA boxes
-  if (L < 1 || H % 256 || H > 8192 || Hq != 4 * Hkv || Hkv < 1 || I % 64 || V < 8 || V % 8 || c.max_model_len < 16 ||
+  if (L < 1 || H % 256 || H > 8192 || !attn_group_ok(Hq, Hkv) || I % 64 || V < 8 || V % 8 || c.max_model_len < 16 ||
       c.max_num_seqs < 1 || c.max_batched_tokens < 16) {
-    set_error("unsupported model/config (need q_heads == 4*kv_heads, hidden %% 256 == 0 and <= 8192, intermediate %% 64 == 0, "
-              "vocab %% 8 == 0, max_model_len >= 16)");
+    set_error("unsupported model/config (need kv_heads to divide q_heads with 1..16 query heads per KV head, hidden %% 256 == 0 "
+              "and <= 8192, intermediate %% 64 == 0, vocab %% 8 == 0, max_model_len >= 16)");
     return B200_ERR_INVALID;
   }
   if (c.rope_scaling_type < 0 || c.rope_scaling_type > 2 ||

@@ -93,26 +93,30 @@ int logprobs_rows(const void* logits, int ld, int V, const int* rows, const int*
 // step's token batch; the first of them sits at absolute position q_pos0 in the sequence.
 struct AttnWork {
   int q_tok0;
-  int q_count;  // decode: 1, or up to kMaxDecodeQ consecutive positions (a speculative verify); <= 16 for a prefill tile
+  int q_count;  // decode: 1, or up to kDecodeRows / G consecutive positions (a speculative verify); <= 16 for a prefill tile
   int q_pos0;
   int seq;      // row of block_tables
 };
 
-// query positions of one decode work item: the last token and up to 3 speculative drafts share the 16-row tile
-constexpr int kMaxDecodeQ = 4;
+// rows of decode attention's mma tile: a work item's G query heads times its q_count positions (the last token and its
+// speculative drafts) must fit in it
+constexpr int kDecodeRows = 16;
 
-// Paged causal attention, head_dim 128, GQA group 4 (Hq = 4 * Hkv), page = 16 tokens.
+// the group sizes G = Hq / Hkv the attention kernels serve: Hkv divides Hq and 1 <= G <= 16
+inline bool attn_group_ok(int Hq, int Hkv) { return Hkv >= 1 && Hq % Hkv == 0 && Hq / Hkv >= 1 && Hq / Hkv <= kDecodeRows; }
+
+// Paged causal attention, head_dim 128, G = Hq / Hkv query heads per KV head (attn_group_ok), page = 16 tokens.
 //   q: rows of the fused qkv buffer (leading dim ldq), out: [T, Hq*128] (leading dim ldo)
 //   kv_layer: [block][2][Hkv][16][128];  block_tables: [num_seqs, max_blocks] int32
-//   decode != 0: every work item has 1 <= q_count <= kMaxDecodeQ (position j causally masked at q_pos0 + j) and the CTA's
-//   4 warps split the KV range.
+//   decode != 0: every work item has 1 <= q_count and G * q_count <= kDecodeRows (position j causally masked at q_pos0 + j)
+//   and the CTA's 4 warps split the KV range.  decode == 0 (the op-level prefill form) needs G == 4.
 int paged_attention(const void* q, int ldq, void* out, int ldo, const void* kv_layer, const int* block_tables,
                     int max_blocks, const AttnWork* work, int num_work, int Hq, int Hkv, float scale,
                     int decode, cudaStream_t st, float* split_ws = nullptr, int split = 1);
 // split-KV decode (few sequences): `split` CTAs per (work item, KV head) each stream a slice of the context and leave an
-// unnormalised partial in split_ws (attn_split_ws_bytes, max_q = the largest q_count of the launch), merged by a second
-// tiny kernel.  attn_decode_split picks `split`.
-size_t attn_split_ws_bytes(int num_work, int Hkv, int parts, int max_q = 1);
+// unnormalised partial per query head in split_ws (attn_split_ws_bytes, max_q = the largest q_count of the launch), merged
+// by a second tiny kernel.  attn_decode_split picks `split`.
+size_t attn_split_ws_bytes(int num_work, int Hq, int parts, int max_q = 1);
 int attn_decode_split(int num_work, int Hkv, int max_ctx, int sms);
 
 // Chunked-prefill attention on wgmma (attention_wgmma.cu): work items of up to kPrefillQueryBlock query tokens, one CTA per

@@ -302,7 +302,11 @@ int b200_config_from_hf(const char* dir, b200_config* cfg) {
   }
   const int head_dim = static_cast<int>(num("head_dim", cfg->q_heads ? cfg->hidden / cfg->q_heads : 0));
   if (head_dim != 128) { set_error("head_dim %d is not supported (kernels are specialised for 128)", head_dim); return B200_ERR_INVALID; }
-  if (cfg->q_heads != 4 * cfg->kv_heads) { set_error("GQA ratio %d:%d is not supported (kernels are specialised for 4:1)", cfg->q_heads, cfg->kv_heads); return B200_ERR_INVALID; }
+  if (cfg->kv_heads < 1 || cfg->q_heads % cfg->kv_heads || cfg->q_heads / cfg->kv_heads > 16) {
+    set_error("GQA ratio %d:%d is not supported (kv_heads must divide q_heads, with 1 to 16 query heads per KV head)",
+              cfg->q_heads, cfg->kv_heads);
+    return B200_ERR_INVALID;
+  }
   if (const JVal* e = root.get("eos_token_id"); e && e->type == JVal::Num) cfg->eos_token_id = static_cast<int>(e->num);
   return 0;
 }
