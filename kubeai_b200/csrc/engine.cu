@@ -249,7 +249,6 @@ struct Sched {
 // a launched, not yet completed step
 struct InFlight {
   std::vector<Sched> sched;
-  int words = 0, ndec_seq = 0, npre_seq = 0;
   double t_enter = 0, t_packed = 0, t_launched = 0;
 };
 // a result not yet visible to the API threads (published while the next step runs on the GPU)
@@ -264,6 +263,7 @@ struct Pub {
 
 struct StepMeta {
   int T = 0, nd = 0, np = 0, S = 0, nseq = 0;
+  int ndec_seq = 0, npre_seq = 0;   // sequences that decode (or verify drafts) and that prefill a chunk
   int off_ids = 0, off_pos = 0, off_slots = 0, off_rows = 0, off_dwork = 0, off_pwork = 0, off_btab = 0;
   int off_samp = -1;   // SampleRow per sampled row, packed only when one of them has temperature >= 1e-5
   int samp_words = 6;  // words per SampleRow: 7 when a sampled row has min_p, else 6 (min_p off)
@@ -394,14 +394,35 @@ struct Engine {
   // activations
   bf16 *res = nullptr, *x = nullptr, *normed = nullptr, *qkv = nullptr, *attn = nullptr, *gu = nullptr, *act = nullptr,
        *last_hidden = nullptr, *logits = nullptr;
+  // step outputs read back by the host: device arrays and their pinned mirrors.  In step order, per sampled row its id;
+  // per logprobs row a record of 1 + N floats (the token's lp, then the top N) and N ids; per prompt-logprob row the same
+  // and the rank of its target (N = kMaxLogprobs).  for_each_readback: fn(device array, pinned mirror, bytes) for S
+  // sampled rows, n_lp logprobs rows and n_plp prompt-logprob rows.
   int* sampled = nullptr;
-  int32_t* sampled_host = nullptr;  // pinned
-  // logprobs of the rows that asked, in step order: [Scap][1 + kMaxLogprobs] floats (the token's lp, then the top N) and
-  // [Scap][kMaxLogprobs] ids; device and pinned host copies
-  float* lp_dev = nullptr;
-  int* lp_ids_dev = nullptr;
-  float* lp_host = nullptr;
-  int32_t* lp_ids_host = nullptr;
+  float *lp_dev = nullptr, *plp_f_dev = nullptr;
+  int *lp_ids_dev = nullptr, *plp_ids_dev = nullptr, *plp_rank_dev = nullptr;
+  int32_t *sampled_host = nullptr, *lp_ids_host = nullptr, *plp_ids_host = nullptr, *plp_rank_host = nullptr;
+  float *lp_host = nullptr, *plp_f_host = nullptr;
+  template <class F>
+  void for_each_readback(size_t S, size_t n_lp, size_t n_plp, F fn) {
+    const size_t rec = (1 + kMaxLogprobs) * sizeof(float), ids = kMaxLogprobs * sizeof(int32_t);
+    fn(sampled, sampled_host, S * sizeof(int32_t));
+    fn(lp_dev, lp_host, n_lp * rec);
+    fn(lp_ids_dev, lp_ids_host, n_lp * ids);
+    fn(plp_f_dev, plp_f_host, n_plp * rec);
+    fn(plp_ids_dev, plp_ids_host, n_plp * ids);
+    fn(plp_rank_dev, plp_rank_host, n_plp * sizeof(int32_t));
+  }
+  int alloc_readbacks(int S, int n_lp, int n_plp);
+  // record i of the token (prompt = false) or prompt-logprob readbacks
+  LogprobRecord read_record(bool prompt, int i) const {
+    const float* src = (prompt ? plp_f_host : lp_host) + static_cast<size_t>(i) * (1 + kMaxLogprobs);
+    LogprobRecord r;
+    r.lp = src[0];
+    memcpy(r.top_lp, src + 1, sizeof(r.top_lp));
+    memcpy(r.top_ids, (prompt ? plp_ids_host : lp_ids_host) + static_cast<size_t>(i) * kMaxLogprobs, sizeof(r.top_ids));
+    return r;
+  }
   // fused epilogues (gemm_wgmma.cu): RoPE + KV write, residual add, SiLU * up and per-slab argmax ride in the projection
   // that produces their input; off (B200_FUSED_DECODE=0 / B200_FUSED_PREFILL=0) each runs as its own elementwise kernel
   float2* cand = nullptr;    // argmax candidates [token][V / 128 slab]
@@ -431,18 +452,11 @@ struct Engine {
   std::vector<PenaltyRec> pen_tmp_;
 
   // prompt logprobs: a step's rows go through the final norm, the lm_head and logprobs_rows in groups of plp_G, each
-  // group's hidden rows in prompt_hidden [plp_G, H] and its logits in prompt_logits [plp_G, V]; the records of the step's
-  // rows in step order: plp_f [Tcap][1 + kMaxLogprobs] floats (lp, then the top N), plp_ids [Tcap][kMaxLogprobs],
-  // plp_rank [Tcap]; device and pinned host copies
+  // group's hidden rows in prompt_hidden [plp_G, H] and its logits in prompt_logits [plp_G, V]; the records go to the
+  // prompt-logprob readbacks
   int plp_G = 0;
   bf16 *prompt_hidden = nullptr, *prompt_logits = nullptr;
   XMaps xm_phid;
-  float* plp_f_dev = nullptr;
-  int* plp_ids_dev = nullptr;
-  int* plp_rank_dev = nullptr;
-  float* plp_f_host = nullptr;
-  int32_t* plp_ids_host = nullptr;
-  int32_t* plp_rank_host = nullptr;
 
   // step input staging
   int step_words_cap = 0;
@@ -494,6 +508,10 @@ struct Engine {
     return paged_attention_prefill_tc(qkv, Tcap, QKV, attn, Hq * kD, kv_l, btab, max_blocks_per_seq, pwork, np, Hq, Hkv, scale, stream);
   }
   // one scheduler iteration = launch (schedule, pack, H2D, kernels, D2H enqueue) + complete (sync, apply) + publish
+  int schedule(std::vector<Sched>& sched);
+  int pack(const std::vector<Sched>& sched, StepMeta* m);
+  void add_row(const Seq& q, int token_row, int gen_index);
+  int step_words_bound() const;
   int launch(InFlight* f, StepMeta* m);
   int complete(InFlight& f, const StepMeta& m, b200_step_info* info);
   void publish();
@@ -578,16 +596,17 @@ Engine::~Engine() {
   }
   cudaSetDevice(cfg.device);
   if (stream) cudaStreamSynchronize(stream);
-  void* frees[] = {weights_blob, res, x, normed, qkv, attn, gu, act, last_hidden, logits, sampled, gemm_ws,
-                   gemm_counters, kv, cand, attn_ws, lp_dev, lp_ids_dev, pen_recs, pen_lens, pen_save, prompt_hidden,
-                   prompt_logits, plp_f_dev, plp_ids_dev, plp_rank_dev};
+  void* frees[] = {weights_blob, res, x, normed, qkv, attn, gu, act, last_hidden, logits, gemm_ws, gemm_counters, kv,
+                   cand, attn_ws, pen_recs, pen_lens, pen_save, prompt_hidden, prompt_logits};
   for (void* p : frees)
     if (p) cudaFree(p);
   for (auto p : stage_dev)
     if (p) cudaFree(p);
-  void* host_frees[] = {stage_host, sampled_host, lp_host, lp_ids_host, plp_f_host, plp_ids_host, plp_rank_host};
-  for (void* p : host_frees)
-    if (p) cudaFreeHost(p);
+  if (stage_host) cudaFreeHost(stage_host);
+  for_each_readback(0, 0, 0, [](auto* dev, auto* host, size_t) {
+    if (dev) cudaFree(dev);
+    if (host) cudaFreeHost(host);
+  });
   if (ev0) cudaEventDestroy(ev0);
   if (ev1) cudaEventDestroy(ev1);
   if (stream) cudaStreamDestroy(stream);
@@ -600,6 +619,18 @@ static uint64_t splitmix64(uint64_t* state) {
   z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
   z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
   return z ^ (z >> 31);
+}
+
+// the readbacks of up to S sampled, n_lp logprobs and n_plp prompt-logprob rows that are not allocated yet
+int Engine::alloc_readbacks(int S, int n_lp, int n_plp) {
+  cudaError_t ce = cudaSuccess;
+  for_each_readback(S, n_lp, n_plp, [&](auto*& dev, auto*& host, size_t bytes) {
+    if (bytes == 0 || dev || ce != cudaSuccess) return;
+    ce = cudaMalloc(&dev, bytes);
+    if (ce == cudaSuccess) ce = cudaMallocHost(&host, bytes);
+  });
+  CK(ce);
+  return 0;
 }
 
 int Engine::alloc_all() {
@@ -697,16 +728,11 @@ int Engine::alloc_all() {
   CK(cudaMalloc(&act, static_cast<size_t>(Tcap) * I * 2));
   CK(cudaMalloc(&last_hidden, static_cast<size_t>(Scap) * H * 2));
   CK(cudaMalloc(&logits, static_cast<size_t>(Scap) * V * 2));
-  CK(cudaMalloc(&sampled, static_cast<size_t>(Scap) * 4));
   CK(cudaMemset(normed, 0, static_cast<size_t>(Tcap) * H * 2));
   CK(cudaMemset(attn, 0, static_cast<size_t>(Tcap) * Hq * kD * 2));
   CK(cudaMemset(act, 0, static_cast<size_t>(Tcap) * I * 2));
   CK(cudaMemset(last_hidden, 0, static_cast<size_t>(Scap) * H * 2));
-  CK(cudaMallocHost(&sampled_host, static_cast<size_t>(Scap) * 4));
-  CK(cudaMalloc(&lp_dev, static_cast<size_t>(Scap) * (1 + kMaxLogprobs) * sizeof(float)));
-  CK(cudaMalloc(&lp_ids_dev, static_cast<size_t>(Scap) * kMaxLogprobs * sizeof(int)));
-  CK(cudaMallocHost(&lp_host, static_cast<size_t>(Scap) * (1 + kMaxLogprobs) * sizeof(float)));
-  CK(cudaMallocHost(&lp_ids_host, static_cast<size_t>(Scap) * kMaxLogprobs * sizeof(int32_t)));
+  if (int rc = alloc_readbacks(Scap, Scap, 0)) return rc;   // the prompt-logprob records come after the KV pool
   CK(cudaMalloc(&cand, static_cast<size_t>(std::min(Scap, 128)) * ((V + 127) / 128) * sizeof(float2)));
   // outputs of the last step, readable by name (b200_engine_tensor_read): sampled ids int32 [S]; the lm_head's per-slab
   // {best logit, index} candidates float2 [S][ceil(V / 128)] when the step sampled through them, else bf16 logits [S][V]
@@ -804,12 +830,7 @@ int Engine::alloc_all() {
   CK(cudaMalloc(&prompt_hidden, static_cast<size_t>(plp_G) * H * 2));
   CK(cudaMalloc(&prompt_logits, static_cast<size_t>(plp_G) * V * 2));
   CK(cudaMemset(prompt_hidden, 0, static_cast<size_t>(plp_G) * H * 2));
-  CK(cudaMalloc(&plp_f_dev, static_cast<size_t>(Tcap) * (1 + kMaxLogprobs) * sizeof(float)));
-  CK(cudaMalloc(&plp_ids_dev, static_cast<size_t>(Tcap) * kMaxLogprobs * sizeof(int)));
-  CK(cudaMalloc(&plp_rank_dev, static_cast<size_t>(Tcap) * sizeof(int)));
-  CK(cudaMallocHost(&plp_f_host, static_cast<size_t>(Tcap) * (1 + kMaxLogprobs) * sizeof(float)));
-  CK(cudaMallocHost(&plp_ids_host, static_cast<size_t>(Tcap) * kMaxLogprobs * sizeof(int32_t)));
-  CK(cudaMallocHost(&plp_rank_host, static_cast<size_t>(Tcap) * sizeof(int32_t)));
+  if (int rc = alloc_readbacks(Scap, Scap, Tcap)) return rc;
   // bf16 logits [plp_G, V] of the last group of prompt-logprob rows of the last step
   tensors["step.prompt_logits"] = {prompt_logits, static_cast<size_t>(plp_G) * V * 2};
   for (int i = 0; i < kGemmNumBlockN; ++i)
@@ -817,10 +838,7 @@ int Engine::alloc_all() {
 
   // ---- step input ring
   max_blocks_per_seq = (cfg.max_model_len + kPage - 1) / kPage;
-  step_words_cap = 3 * Tcap + Scap + 4 * Scap + 4 * (Tcap / 16 + Scap + 1) + Scap * max_blocks_per_seq + 7 * Scap + 2 * Scap +
-                   8 * Scap + 3 * Tcap + 2 * Scap + 64;
-  static_assert(sizeof(SampleRow) == 7 * sizeof(int32_t), "SampleRow is 7 words of the step input");
-  static_assert(sizeof(PenaltyRow) == 8 * sizeof(int32_t), "PenaltyRow is 8 words of the step input");
+  step_words_cap = step_words_bound();
   ring_n = std::max(1, cfg.record_steps) + 1;  // last slot = scratch for unrecorded steps
   CK(cudaMallocHost(&stage_host, static_cast<size_t>(step_words_cap) * 4));
   stage_dev.assign(ring_n, nullptr);
@@ -1176,12 +1194,10 @@ void Engine::add_drafts(std::vector<Sched>& sched, int* budget) {
 }
 
 // ------------------------------------------------------------------ one scheduler iteration + forward
-// launch(): schedule (running first, then admissions, vLLM v1 order), pack the step's device inputs, enqueue the
-// H2D copy, the kernels and the D2H of the sampled ids.  Returns 0 when there is nothing to run, 1 when a step is
-// in flight, negative on error.
-int Engine::launch(InFlight* f, StepMeta* mp) {
-  static const bool timing = [] { const char* e = getenv("B200_STEP_TIMING"); return e && atoi(e) != 0; }();
-  f->t_enter = timing ? now_s() : 0.0;
+// schedule(): take the requests that arrived and drop the aborted ones, then schedule the running sequences (running
+// first, then admissions, vLLM v1 order).  Every change to sequence state before the step runs is made here, so that
+// pack() only reads.  Returns 0, or negative on error.
+int Engine::schedule(std::vector<Sched>& sched) {
   {
     // arrival order (vLLM's FCFS); with fixed_admission the requests that arrived since the last step join the queue in
     // a fixed order (prompt content, then length) instead of the order their client threads reached b200_submit
@@ -1222,7 +1238,6 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
     }
   }
 
-  std::vector<Sched>& sched = f->sched;
   sched.clear();
   int budget = cfg.max_batched_tokens;
   bool preempted = false;
@@ -1275,16 +1290,57 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
     sched.push_back({s, n});
     budget -= n;
   }
+  // 3. what the step produces for the sequences it runs
+  for (auto& sc : sched) {
+    Seq& s = *sc.s;
+    if (s.prompt_logprobs >= 0) {
+      // positions p in [p0, p0 + n) that still need a record: the row at p gives prompt token p + 1's.  The last prompt
+      // position is the sampled row, whose record (if asked for) is the first generated token's.
+      const int hi = std::min(s.n_computed + sc.n, s.n_prompt - 1);
+      sc.n_plp = std::max(hi - std::max(s.n_computed, s.plp_done), 0);
+      if (sc.n_plp > 0) s.plp_done = hi;
+    }
+    if (!s.children.empty() && s.n_computed + sc.n == static_cast<int>(s.toks.size())) {
+      // the fork (plan_fork): a member aborted before it leaves here, the others get their logits-edit lists
+      for (auto& c : s.children)
+        if (std::find(s.fork.begin(), s.fork.end(), c) == s.fork.end()) finish(c, B200_FINISH_ABORTED);
+      s.children.clear();
+      for (auto& c : s.fork)
+        if (c->edits())
+          if (int rc = admit_edits(*c)) return rc;
+    }
+  }
   {
     std::lock_guard<std::mutex> lk(mu_);
     stats.running = static_cast<int>(running.size());
     stats.waiting = static_cast<int>(waiting.size());
     stats.kv_blocks_free = pool.free_count();
   }
-  if (sched.empty()) return 0;
+  return 0;
+}
 
-  // ---- pack the step's device inputs
-  StepMeta m;
+// One sampled row: logits row `token_row`, drawn as the token with index gen_index of q's generation (so a request
+// recomputed after preemption draws the same noise), with q's logits edits and logprobs
+void Engine::add_row(const Seq& q, int token_row, int gen_index) {
+  rows_.push_back(token_row);
+  const int row = static_cast<int>(rows_.size()) - 1;
+  samp_.push_back({q.temperature, q.top_k, q.top_p, static_cast<uint32_t>(q.seed), static_cast<uint32_t>(q.seed >> 32),
+                   gen_index, q.min_p});
+  if (q.pen_slot >= 0)
+    pen_.push_back({row, q.pen_slot, q.presence, q.frequency, q.repetition, gen_index, q.min_tokens, q.pen_history() ? 1 : 0});
+  if (q.top_logprobs >= 0) {
+    lp_rows_.push_back(row);
+    lp_n_.push_back(q.top_logprobs);
+  }
+}
+
+// pack(): the step's device inputs in stage_host, from the sequence state schedule() left, which it only reads.  The
+// sections in word order: token ids, positions and KV slots [T] each; the sampled rows' token indices [S]; 4-word aligned,
+// the decode and the prefill work lists; the block tables [nseq][max_blocks_per_seq]; then, each only in steps that have
+// such a row, the SampleRows, PenaltyRows, logprobs rows, prompt-logprob rows and fork page copies.
+int Engine::pack(const std::vector<Sched>& sched, StepMeta* mp) {
+  StepMeta& m = *mp;
+  m = StepMeta();
   m.nseq = static_cast<int>(sched.size());
   for (auto& sc : sched) m.T += sc.n;
   dwork_.clear();
@@ -1299,93 +1355,48 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
   plp_n_.clear();
   fork_src_.clear();
   fork_dst_.clear();
-  bool any_sampled = false, any_minp = false;
   int32_t* h = stage_host;
   m.off_ids = 0; m.off_pos = m.T; m.off_slots = 2 * m.T;
   int tok = 0;
-  f->ndec_seq = f->npre_seq = 0;
   for (int si = 0; si < m.nseq; ++si) {
-    Seq& s = *sched[si].s;
-    const int n = sched[si].n, p0 = s.n_computed, nd = sched[si].n_draft;
+    const Sched& sc = sched[si];
+    const Seq& s = *sc.s;
+    const int n = sc.n, p0 = s.n_computed, nd = sc.n_draft;
     for (int j = 0; j < n; ++j) {
       const int p = p0 + j;
       h[m.off_ids + tok + j] = j < n - nd ? s.toks[p] : s.draft[j - (n - nd)];
       h[m.off_pos + tok + j] = p;
       h[m.off_slots + tok + j] = s.blocks[p / kPage] * kPage + (p % kPage);
     }
-    if (s.prompt_logprobs >= 0) {
-      // positions p in [p0, p0 + n) that still need a record: the row at p gives prompt token p + 1's.  The last prompt
-      // position is the sampled row, whose record (if asked for) is the first generated token's.
-      const int lo = std::max(p0, s.plp_done), hi = std::min(p0 + n, s.n_prompt - 1);
-      for (int p = lo; p < hi; ++p) {
-        plp_tok_.push_back(tok + p - p0);
-        plp_tgt_.push_back(s.toks[p + 1]);
-        plp_n_.push_back(s.prompt_logprobs);
-      }
-      if (hi > lo) {
-        sched[si].n_plp = hi - lo;
-        s.plp_done = hi;
-      }
+    // the chunk's prompt-logprob rows: the last sc.n_plp positions before min(p0 + n, n_prompt - 1)
+    const int plp_hi = std::min(p0 + n, s.n_prompt - 1);
+    for (int p = plp_hi - sc.n_plp; p < plp_hi; ++p) {
+      plp_tok_.push_back(tok + p - p0);
+      plp_tgt_.push_back(s.toks[p + 1]);
+      plp_n_.push_back(s.prompt_logprobs);
     }
     if (n == 1 || nd > 0) {
       // a decode, or a speculative verify: its 1 + nd positions share one decode work item (attention.cu)
       dwork_.push_back({tok, n, p0, si});
-      m.kv_tokens += p0 + n;
       m.draft_tokens += nd;
-      ++f->ndec_seq;
+      ++m.ndec_seq;
     } else {
       const int qb = kPrefillQueryBlock;
       for (int j = 0; j < n; j += qb) pwork_.push_back({tok + j, std::min(qb, n - j), p0 + j, si});
-      m.kv_tokens += p0 + n;  // unique K/V tokens this sequence streams from HBM (query tiles re-read them from L2)
-      ++f->npre_seq;
+      ++m.npre_seq;
     }
+    m.kv_tokens += p0 + n;  // unique K/V tokens this sequence streams from HBM (query tiles re-read them from L2)
     if (p0 + n - nd == static_cast<int>(s.toks.size())) {
       // row j (0..nd) of a verify is drawn as the token with index n_generated + j: accepting draft j exactly when it
       // equals row j's token gives the stream the non-speculative steps would
-      for (int j = 0; j <= nd; ++j) {
-        rows_.push_back(tok + n - 1 - nd + j);
-        // n = the index of the token this row generates: a request recomputed after preemption draws the same noise
-        samp_.push_back({s.temperature, s.top_k, s.top_p, static_cast<uint32_t>(s.seed), static_cast<uint32_t>(s.seed >> 32),
-                         s.n_generated + j, s.min_p});
-        any_sampled |= s.temperature >= 1e-5f;
-        any_minp |= s.temperature >= 1e-5f && s.min_p > 0.f;
-        if (s.pen_slot >= 0) {
-          pen_.push_back({static_cast<int>(rows_.size()) - 1, s.pen_slot, s.presence, s.frequency, s.repetition, s.n_generated + j,
-                          s.min_tokens, s.pen_history() ? 1 : 0});
-          m.pen_update |= s.pen_history();
-        }
-        if (s.top_logprobs >= 0) {
-          lp_rows_.push_back(static_cast<int>(rows_.size()) - 1);
-          lp_n_.push_back(s.top_logprobs);
-        }
-      }
-      if (!s.children.empty()) {
-        // the fork: the last prompt position is sampled once more for every member that forks, each row with the member's
-        // own seed, logits-edit list and logprobs (the gathered final norm reads a row index any number of times).  A
-        // member aborted before the fork leaves here.
-        for (auto& c : s.children)
-          if (std::find(s.fork.begin(), s.fork.end(), c) == s.fork.end()) finish(c, B200_FINISH_ABORTED);
-        s.children.clear();
-        for (size_t k = 0; k < s.fork.size(); ++k) {
-          Seq& c = *s.fork[k];
-          rows_.push_back(tok + n - 1);
-          samp_.push_back({c.temperature, c.top_k, c.top_p, static_cast<uint32_t>(c.seed), static_cast<uint32_t>(c.seed >> 32),
-                           0, c.min_p});
-          any_minp |= c.min_p > 0.f;
-          if (c.edits()) {
-            if (int rc = admit_edits(c)) return rc;
-            pen_.push_back({static_cast<int>(rows_.size()) - 1, c.pen_slot, c.presence, c.frequency, c.repetition, 0,
-                            c.min_tokens, c.pen_history() ? 1 : 0});
-            m.pen_update |= c.pen_history();
-          }
-          if (c.top_logprobs >= 0) {
-            lp_rows_.push_back(static_cast<int>(rows_.size()) - 1);
-            lp_n_.push_back(c.top_logprobs);
-          }
-          if (!s.fork_tails.empty()) {   // the prompt ends inside its last page: each member gets its own copy
-            fork_src_.push_back(s.blocks[s.n_prompt / kPage]);
-            fork_dst_.push_back(s.fork_tails[k]);
-          }
+      for (int j = 0; j <= nd; ++j) add_row(s, tok + n - 1 - nd + j, s.n_generated + j);
+      // the fork: the last prompt position is sampled once more for every member that forks, each row with the member's
+      // own seed, logits-edit list and logprobs (the gathered final norm reads a row index any number of times)
+      for (size_t k = 0; k < s.fork.size(); ++k) {
+        add_row(*s.fork[k], tok + n - 1, 0);
+        if (!s.fork_tails.empty()) {   // the prompt ends inside its last page: each member gets its own copy
+          fork_src_.push_back(s.blocks[s.n_prompt / kPage]);
+          fork_dst_.push_back(s.fork_tails[k]);
         }
       }
     }
@@ -1401,56 +1412,89 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
   m.np = static_cast<int>(pwork_.size());
   m.S = static_cast<int>(rows_.size());
   m.out_tokens = m.S;
+  m.n_pen = static_cast<int>(pen_.size());
+  m.n_lp = static_cast<int>(lp_rows_.size());
+  m.n_plp = static_cast<int>(plp_tok_.size());
+  m.n_fork = static_cast<int>(fork_src_.size());
+  bool any_sampled = false, any_minp = false;   // (submit zeroes min_p for greedy requests)
+  for (auto& r : samp_) {
+    any_sampled |= r.temperature >= 1e-5f;
+    any_minp |= r.min_p > 0.f;
+  }
+  for (auto& r : pen_) m.pen_update |= r.history != 0;
+
   int w = 3 * m.T;
-  m.off_rows = w; memcpy(h + w, rows_.data(), rows_.size() * 4); w += m.S;
+  auto put = [&](const auto& v) {   // appends a section, returns its offset
+    const int off = w;
+    memcpy(h + w, v.data(), v.size() * sizeof(v[0]));
+    w += static_cast<int>(v.size() * sizeof(v[0]) / sizeof(int32_t));
+    return off;
+  };
+  m.off_rows = put(rows_);
   w = (w + 3) & ~3;
-  m.off_dwork = w; memcpy(h + w, dwork_.data(), dwork_.size() * 16); w += 4 * m.nd;
-  m.off_pwork = w; memcpy(h + w, pwork_.data(), pwork_.size() * 16); w += 4 * m.np;
+  m.off_dwork = put(dwork_);
+  m.off_pwork = put(pwork_);
   m.off_btab = w;
   for (int si = 0; si < m.nseq; ++si) {
-    Seq& s = *sched[si].s;
+    const Seq& s = *sched[si].s;
     memcpy(h + w + static_cast<size_t>(si) * max_blocks_per_seq, s.blocks.data(), s.blocks.size() * 4);
   }
   w += m.nseq * max_blocks_per_seq;
-  if (any_sampled) {   // greedy-only steps carry no sampling section: the same words as without one
+  if (any_sampled) {   // greedy-only steps carry no sampling section, and min_p takes a word only in steps that have it
     m.off_samp = w;
-    m.samp_words = any_minp ? 7 : 6;   // likewise min_p takes a word per row only in steps that have it
+    m.samp_words = any_minp ? 7 : 6;
     for (int i = 0; i < m.S; ++i) memcpy(h + w + i * m.samp_words, &samp_[i], m.samp_words * sizeof(int32_t));
     w += m.samp_words * m.S;
   }
-  m.n_pen = static_cast<int>(pen_.size());
-  if (m.n_pen > 0) {   // and logits edits
-    m.off_pen = w;
-    memcpy(h + w, pen_.data(), pen_.size() * sizeof(PenaltyRow));
-    w += 8 * m.n_pen;
+  if (m.n_pen > 0) m.off_pen = put(pen_);
+  if (m.n_lp > 0) {
+    m.off_lp = put(lp_rows_);
+    put(lp_n_);
   }
-  m.n_lp = static_cast<int>(lp_rows_.size());
-  if (m.n_lp > 0) {   // likewise steps without a logprobs row carry no logprobs section
-    m.off_lp = w;
-    memcpy(h + w, lp_rows_.data(), lp_rows_.size() * 4);
-    memcpy(h + w + m.n_lp, lp_n_.data(), lp_n_.size() * 4);
-    w += 2 * m.n_lp;
+  if (m.n_plp > 0) {
+    m.off_plp = put(plp_tok_);
+    put(plp_tgt_);
+    put(plp_n_);
   }
-  m.n_plp = static_cast<int>(plp_tok_.size());
-  if (m.n_plp > 0) {   // and prompt logprobs
-    m.off_plp = w;
-    memcpy(h + w, plp_tok_.data(), plp_tok_.size() * 4);
-    memcpy(h + w + m.n_plp, plp_tgt_.data(), plp_tgt_.size() * 4);
-    memcpy(h + w + 2 * m.n_plp, plp_n_.data(), plp_n_.size() * 4);
-    w += 3 * m.n_plp;
-  }
-  m.n_fork = static_cast<int>(fork_src_.size());
-  if (m.n_fork > 0) {   // and fork page copies
-    m.off_fork = w;
-    memcpy(h + w, fork_src_.data(), fork_src_.size() * 4);
-    memcpy(h + w + m.n_fork, fork_dst_.data(), fork_dst_.size() * 4);
-    w += 2 * m.n_fork;
+  if (m.n_fork > 0) {
+    m.off_fork = put(fork_src_);
+    put(fork_dst_);
   }
   m.words = w;
   if (w > step_words_cap) {
     set_error("step staging overflow (%d > %d words)", w, step_words_cap);
     return B200_ERR_INVALID;
   }
+  return 0;
+}
+
+// The most words pack() writes, section by section.  A step runs at most max_num_seqs sequences (a parallel-sampling
+// group holds a running slot per member from its leader's admission) and T <= Tcap tokens; it samples S <= Scap rows (one
+// per sequence and fork member, plus one per draft).
+int Engine::step_words_bound() const {
+  static_assert(sizeof(SampleRow) == 7 * sizeof(int32_t), "SampleRow is 7 words of the step input");
+  static_assert(sizeof(PenaltyRow) == 8 * sizeof(int32_t), "PenaltyRow is 8 words of the step input");
+  static_assert(sizeof(AttnWork) == 4 * sizeof(int32_t), "AttnWork is 4 words of the step input");
+  const int seqs = cfg.max_num_seqs;
+  return 3 * Tcap                                 // token ids, positions, KV slots
+         + Scap + 3                               // sampled rows' token indices, then the alignment
+         + 4 * seqs                               // decode work: one item per decoding sequence
+         + 4 * (Tcap / kPrefillQueryBlock + seqs) // prefill work: ceil(n / kPrefillQueryBlock) items per chunk of n tokens
+         + seqs * max_blocks_per_seq              // block tables
+         + 7 * Scap + 8 * Scap + 2 * Scap         // SampleRows, PenaltyRows, logprobs rows (row, N): at most one each per row
+         + 3 * Tcap                               // prompt-logprob rows (token, target, N): at most one per token
+         + 2 * seqs;                              // fork page copies (source, destination): at most one per member
+}
+
+// launch(): schedule, pack, then enqueue the H2D copy of the step's inputs, the kernels and the D2H of its outputs.
+// Returns 0 when there is nothing to run, 1 when a step is in flight, negative on error.
+int Engine::launch(InFlight* f, StepMeta* mp) {
+  static const bool timing = [] { const char* e = getenv("B200_STEP_TIMING"); return e && atoi(e) != 0; }();
+  f->t_enter = timing ? now_s() : 0.0;
+  if (int rc = schedule(f->sched)) return rc;
+  if (f->sched.empty()) return 0;
+  StepMeta m;
+  if (int rc = pack(f->sched, &m)) return rc;
 
   int slot = ring_n - 1;  // scratch
   if (recording && ring_n > 1) {
@@ -1463,9 +1507,9 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
   f->t_packed = timing ? now_s() : 0.0;
   // NVTX range per step (SURVEY.md §5): visible in nsys / ncu --nvtx timelines as "step T=<tokens> dec=<n> pre=<n>"
   char nv[64];
-  snprintf(nv, sizeof(nv), "step T=%d dec=%d pre=%d", m.T, f->ndec_seq, f->npre_seq);
+  snprintf(nv, sizeof(nv), "step T=%d dec=%d pre=%d", m.T, m.ndec_seq, m.npre_seq);
   nvtxRangePushA(nv);
-  CK(cudaMemcpyAsync(dbuf, h, static_cast<size_t>(w) * 4, cudaMemcpyHostToDevice, stream));
+  CK(cudaMemcpyAsync(dbuf, stage_host, static_cast<size_t>(m.words) * 4, cudaMemcpyHostToDevice, stream));
   CK(cudaEventRecord(ev0, stream));
   int frc = forward(m, dbuf, false, nullptr);
   if (!frc && m.pen_update) {   // here, not in forward(): a replay must not change any history
@@ -1483,18 +1527,12 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
   nvtxRangePop();
   if (frc) return frc;
   CK(cudaEventRecord(ev1, stream));
-  if (m.S) CK(cudaMemcpyAsync(sampled_host, sampled, static_cast<size_t>(m.S) * 4, cudaMemcpyDeviceToHost, stream));
-  if (m.n_lp) {
-    CK(cudaMemcpyAsync(lp_host, lp_dev, static_cast<size_t>(m.n_lp) * (1 + kMaxLogprobs) * sizeof(float), cudaMemcpyDeviceToHost, stream));
-    CK(cudaMemcpyAsync(lp_ids_host, lp_ids_dev, static_cast<size_t>(m.n_lp) * kMaxLogprobs * sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
-  }
-  if (m.n_plp) {
-    CK(cudaMemcpyAsync(plp_f_host, plp_f_dev, static_cast<size_t>(m.n_plp) * (1 + kMaxLogprobs) * sizeof(float), cudaMemcpyDeviceToHost, stream));
-    CK(cudaMemcpyAsync(plp_ids_host, plp_ids_dev, static_cast<size_t>(m.n_plp) * kMaxLogprobs * sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
-    CK(cudaMemcpyAsync(plp_rank_host, plp_rank_dev, static_cast<size_t>(m.n_plp) * sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
-  }
+  cudaError_t readback = cudaSuccess;
+  for_each_readback(m.S, m.n_lp, m.n_plp, [&](auto* dev, auto* host, size_t bytes) {
+    if (bytes > 0 && readback == cudaSuccess) readback = cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, stream);
+  });
+  CK(readback);
   f->t_launched = timing ? now_s() : 0.0;
-  f->words = w;
   *mp = m;
   return 1;
 }
@@ -1530,15 +1568,7 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
     publish_blocks();
     // prompt records come back in step order; they are published with (or before) the first generated token
     const int plp0 = static_cast<int>(pending_plp.size()), n_plp = f.sched[si].n_plp;
-    for (int k = 0; k < n_plp; ++k, ++pi) {
-      PromptLogprobRecord r;
-      const float* src = plp_f_host + static_cast<size_t>(pi) * (1 + kMaxLogprobs);
-      r.r.lp = src[0];
-      memcpy(r.r.top_lp, src + 1, sizeof(r.r.top_lp));
-      memcpy(r.r.top_ids, plp_ids_host + static_cast<size_t>(pi) * kMaxLogprobs, sizeof(r.r.top_ids));
-      r.rank = plp_rank_host[pi];
-      pending_plp.push_back(r);
-    }
+    for (int k = 0; k < n_plp; ++k, ++pi) pending_plp.push_back({read_record(true, pi), plp_rank_host[pi]});
     if (!samples) {
       if (n_plp > 0) pending_pub.push_back({sp, 0, false, 0, -1, plp0, n_plp});
       continue;
@@ -1556,62 +1586,47 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
       if (!code && static_cast<int>(q.toks.size()) >= cfg.max_model_len) code = B200_FINISH_LENGTH;
       *lp = -1;
       if (q.top_logprobs >= 0) {   // records come back in step order, as the ids do
-        LogprobRecord r;
-        const float* src = lp_host + static_cast<size_t>(li) * (1 + kMaxLogprobs);
-        r.lp = src[0];
-        memcpy(r.top_lp, src + 1, sizeof(r.top_lp));
-        memcpy(r.top_ids, lp_ids_host + static_cast<size_t>(li) * kMaxLogprobs, sizeof(r.top_ids));
-        ++li;
         *lp = static_cast<int>(pending_lp.size());
-        pending_lp.push_back(r);
+        pending_lp.push_back(read_record(false, li++));
       }
       return code;
     };
+    // emit row j's token t_j for j = 0..nd, stopping after t_j when it differs from draft j (a speculative verify), when
+    // it finishes the request, or at the last row.  Every emitted token is the one the non-speculative steps would give.
+    int code = 0, emitted = 0;
+    for (int j = 0; j <= nd; ++j) {
+      int32_t t = 0;
+      int lp = -1;
+      code = take(s, &t, &lp);
+      pending_pub.push_back({sp, t, true, code, lp, j == 0 ? plp0 : 0, j == 0 ? n_plp : 0});
+      ++emitted;
+      const bool match = j < nd && t == s.draft[j];
+      if (match) ++step_accepted_pos[j];
+      step_accepted += match;
+      if (code || !match) break;
+    }
+    // the rows after the last emitted one are skipped, but their ids and records were copied back in step order
+    ri += nd + 1 - emitted;
+    if (s.top_logprobs >= 0) li += nd + 1 - emitted;
     if (nd > 0) {
-      // a speculative verify: emit row j's token t_j for j = 0..nd, stopping after t_j when it differs from draft j, when it
-      // finishes the request, or at the last row.  Every emitted token is the one the non-speculative steps would give.
-      int code = 0, emitted = 0, accepted = 0;
-      for (int j = 0; j <= nd; ++j) {
-        int32_t t = 0;
-        int lp = -1;
-        code = take(s, &t, &lp);
-        pending_pub.push_back({sp, t, true, code, lp, j == 0 ? plp0 : 0, j == 0 ? n_plp : 0});
-        ++emitted;
-        const bool match = j < nd && t == s.draft[j];
-        if (match) ++step_accepted_pos[j];
-        accepted += match;
-        if (code || !match) break;
-      }
-      // the rows after the last emitted one are skipped, but their ids and records were copied back in step order
-      ri += nd + 1 - emitted;
-      if (s.top_logprobs >= 0) li += nd + 1 - emitted;
       // KV at positions p0 .. p0 + emitted - 1 came from the last token and the drafts that equal the emitted tokens.  The
       // KV a rejected draft left at a later position is never read: attention masks by position, and the next step
       // writes that position before its attention reads it.
       s.n_computed += emitted - 1;
       publish_blocks();
       ++step_verifies;
-      step_accepted += accepted;
-      if (code) {
-        release_blocks(s);
-        s.leaving = true;
-        any_done = true;
-      }
-      continue;
     }
-    int32_t t = 0;
-    int lp = -1;
-    int code = take(s, &t, &lp);
     const bool fork = !s.fork.empty();
-    // a leader aborted before its fork computed the prompt for its members only: it leaves with no token
-    const bool gone = fork && s.abort_requested.load(std::memory_order_relaxed);
-    if (gone) {
+    if (fork && s.abort_requested.load(std::memory_order_relaxed)) {
+      // a leader aborted before its fork computed the prompt for its members only: it leaves with no token
       s.toks.pop_back();
       --s.n_generated;
       --gen;
-      code = B200_FINISH_ABORTED;
+      Pub& p = pending_pub.back();
+      p.has_tok = false;
+      p.lp = -1;
+      p.code = code = B200_FINISH_ABORTED;
     }
-    pending_pub.push_back({sp, t, !gone, code, gone ? -1 : lp, plp0, n_plp});
     if (fork) {
       // members 1..n-1 become running sequences: the prompt's full pages by reference, their own copy of its partly
       // filled last page, the leader's cache chain and prompt records, and the token their own row sampled
@@ -1670,9 +1685,8 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
     stats.last_step_device_us = ms * 1000.0;
     stats.total_device_us += ms * 1000.0;
     stats.last_step_tokens = m.T;
-    stats.h2d_bytes += static_cast<int64_t>(f.words) * 4;
-    stats.d2h_bytes += static_cast<int64_t>(m.S) * 4 + static_cast<int64_t>(m.n_lp) * (1 + 2 * kMaxLogprobs) * 4 +
-                       static_cast<int64_t>(m.n_plp) * (2 + 2 * kMaxLogprobs) * 4;
+    stats.h2d_bytes += static_cast<int64_t>(m.words) * 4;
+    for_each_readback(m.S, m.n_lp, m.n_plp, [&](auto*, auto*, size_t bytes) { stats.d2h_bytes += static_cast<int64_t>(bytes); });
     stats.running = static_cast<int>(running.size());
     stats.waiting = static_cast<int>(waiting.size());
     stats.kv_blocks_free = pool.free_count();
@@ -1689,8 +1703,8 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
   }
   if (info) {
     info->tokens = m.T;
-    info->decode_seqs = f.ndec_seq;
-    info->prefill_seqs = f.npre_seq;
+    info->decode_seqs = m.ndec_seq;
+    info->prefill_seqs = m.npre_seq;
     info->sampled = m.S;
     info->kv_tokens_read = m.kv_tokens;
     info->device_us = ms * 1000.0;
@@ -2337,44 +2351,29 @@ int b200_engine_forward_logits(b200_engine* e, const int32_t* ids, int32_t n, vo
   if (!g.cfg.manual_step) { set_error("forward_logits needs manual_step"); return B200_ERR_INVALID; }
   if (n > g.Tcap || n > g.cfg.max_model_len) { set_error("too many tokens"); return B200_ERR_INVALID; }
   cudaSetDevice(g.cfg.device);
-  Seq s;
-  s.toks.assign(ids, ids + n);
-  if (!g.ensure_blocks(s, n)) { set_error("KV pool exhausted"); return B200_ERR_OOM; }
+  // one greedy prompt from position 0, packed as a step and staged in the scratch ring slot: the recorded steps stay
+  // replayable
+  auto s = std::make_shared<Seq>();
+  s->toks.assign(ids, ids + n);
+  s->n_prompt = n;
+  if (!g.ensure_blocks(*s, n)) { set_error("KV pool exhausted"); return B200_ERR_OOM; }
+  const std::vector<Sched> sched = {{s, n}};
   StepMeta m;
-  m.T = n; m.nseq = 1;
-  int32_t* h = g.stage_host;
-  m.off_ids = 0; m.off_pos = n; m.off_slots = 2 * n;
-  for (int j = 0; j < n; ++j) {
-    h[j] = ids[j];
-    h[n + j] = j;
-    h[2 * n + j] = s.blocks[j / kPage] * kPage + j % kPage;
-  }
-  int w = (3 * n + 3) & ~3;
-  m.off_rows = w;
-  m.off_dwork = w;
-  std::vector<AttnWork> pw;
-  if (n == 1) { m.nd = 1; h[w] = 0; h[w + 1] = 1; h[w + 2] = 0; h[w + 3] = 0; w += 4; m.off_pwork = w; }
-  else {
-    m.off_pwork = w;
-    const int qb = kPrefillQueryBlock;
-    for (int j = 0; j < n; j += qb) { h[w] = j; h[w + 1] = std::min(qb, n - j); h[w + 2] = j; h[w + 3] = 0; w += 4; ++m.np; }
-  }
-  m.off_btab = w;
-  memcpy(h + w, s.blocks.data(), s.blocks.size() * 4);
-  w += g.max_blocks_per_seq;
-  m.words = w;
+  int rc = g.pack(sched, &m);
   bf16* dl = nullptr;
-  CK(cudaMalloc(&dl, static_cast<size_t>(n) * g.V * 2));
-  int32_t* dbuf = g.stage_dev[0];
-  cudaError_t ce = cudaMemcpyAsync(dbuf, h, static_cast<size_t>(w) * 4, cudaMemcpyHostToDevice, g.stream);
-  int rc = ce == cudaSuccess ? g.forward(m, dbuf, true, dl) : B200_ERR_CUDA;
+  if (!rc && cudaMalloc(&dl, static_cast<size_t>(n) * g.V * 2) != cudaSuccess) { set_error("forward_logits: no memory for the logits"); rc = B200_ERR_OOM; }
   if (!rc) {
-    ce = cudaMemcpyAsync(host_logits_bf16, dl, static_cast<size_t>(n) * g.V * 2, cudaMemcpyDeviceToHost, g.stream);
-    if (ce == cudaSuccess) ce = cudaStreamSynchronize(g.stream);
-    if (ce != cudaSuccess) { set_error("forward_logits: %s", cudaGetErrorString(ce)); rc = B200_ERR_CUDA; }
+    int32_t* dbuf = g.stage_dev[g.ring_n - 1];
+    cudaError_t ce = cudaMemcpyAsync(dbuf, g.stage_host, static_cast<size_t>(m.words) * 4, cudaMemcpyHostToDevice, g.stream);
+    rc = ce == cudaSuccess ? g.forward(m, dbuf, true, dl) : B200_ERR_CUDA;
+    if (!rc) {
+      ce = cudaMemcpyAsync(host_logits_bf16, dl, static_cast<size_t>(n) * g.V * 2, cudaMemcpyDeviceToHost, g.stream);
+      if (ce == cudaSuccess) ce = cudaStreamSynchronize(g.stream);
+      if (ce != cudaSuccess) { set_error("forward_logits: %s", cudaGetErrorString(ce)); rc = B200_ERR_CUDA; }
+    }
   }
   cudaFree(dl);
-  for (auto it = s.blocks.rbegin(); it != s.blocks.rend(); ++it) g.pool.unref(*it);
+  for (auto it = s->blocks.rbegin(); it != s->blocks.rend(); ++it) g.pool.unref(*it);
   return rc;
 }
 
