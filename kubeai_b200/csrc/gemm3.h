@@ -14,7 +14,9 @@ enum { GEMM3_PRO_NONE = 0, GEMM3_PRO_NORM = 1 };
 enum { GEMM3_EPI_PLAIN = 0, GEMM3_EPI_RESADD = 1, GEMM3_EPI_SILU = 2, GEMM3_EPI_ROPE_KV = 3, GEMM3_EPI_ARGMAX = 4 };
 
 struct Gemm3Params {
-  CUtensorMap tm_w;   // weight [N, K] bf16, box 128 rows x 64 cols, 128B swizzle (GemmPlan::tm_w)
+  // weight [N, K] bf16, box 128 rows x 64 cols, 128B swizzle (GemmPlan::tm_w).  Read before the PDL dependency wait: the
+  // kernel launched just before this one must not write it.
+  CUtensorMap tm_w;
   CUtensorMap tm_x;   // token tile source [rows, K] bf16, box block_n rows x 64 cols: activations, or the residual for PRO_NORM
   int N, T, K;
   int pro, epi;

@@ -7,10 +7,12 @@
 //   * "swap-AB": the 128-row weight slab is the wgmma M operand (two consumer warpgroups of 64 rows each), the token tile
 //     (64 / 128 / 256 tokens) is the N operand, so a decode step streams every weight byte once per token tile.
 //   * one producer thread issues TMA loads (128B swizzle) of the weight slab and the token tile into a ring of shared
-//     memory stages guarded by full / empty mbarriers; the consumers run wgmma.mma_async on the stages directly.
+//     memory stages guarded by full / empty mbarriers; the consumers run wgmma.mma_async on the stages directly.  The
+//     weight loads of the first ring fill go out before the PDL dependency wait (weights are static).
 //   * split-K: with fewer tiles than SMs (o_proj / down_proj / qkv of a decode step) each tile's K range is cut into S
 //     pieces on S CTAs.  Every piece leaves its fp32 partial in an L2-resident workspace; the last CTA to arrive sums the S
-//     partials in split order (a fixed order: the result does not depend on timing) and runs the epilogue.
+//     partials in split order (a fixed order: the result does not depend on timing) and runs the epilogue.  It loads 16
+//     float4 of a piece per thread before it adds any, so the reduction of a decode-step tile costs about S L2 round trips.
 //   * epilogues: the fp32 tile is staged in shared memory (reusing the ring) and rounded to bf16 once, the rounding point
 //     of a bf16 GEMM output; the elementwise op that follows a projection (residual add, SiLU * up, RoPE + paged KV write,
 //     per-slab argmax) is applied to that rounded value with the same arithmetic as the standalone kernels (elementwise.cu).
@@ -101,20 +103,32 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_wgmma_kernel(const __grid_co
   }
   __syncthreads();
   griddep_launch();
-  griddep_wait();   // activations, residual and norm sums come from the previous kernels
 
   if (tid < 128) {
     // ---------------- producer
     if (tid == 0) {
       // a decode step reads each weight byte once; several token tiles read a slab once per tile, close together in time
       const uint64_t w_hint = ntt > 1 ? kEvictNormal : kEvictFirst;
+      // the first ring fill: weights are static, so their loads go out before the dependency wait and stream while the
+      // previous kernel finishes; the token tiles (activations written by the previous kernels) only after it.  Every
+      // stage is armed for all its bytes (weight slab and token tile) when its weight load is issued.  The 256-token
+      // instance (prefill steps, launches of hundreds of µs) loads in order after the wait: at its register cap the early
+      // loads cost it a spill.
+      const int pre = BN < 256 ? min(C::kStages, kb1 - kb0) : 0;
+      for (int i = 0; i < pre; ++i) {
+        mbar_arrive_expect_tx(full_bar(i), C::kStageBytes);
+        tma_load_2d(sbase + i * C::kStageBytes, &P.tm_w, full_bar(i), (kb0 + i) * kBlockK, n0, w_hint);
+      }
+      griddep_wait();
       int stage = 0;
       uint32_t phase = 0;
       for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(empty_bar(stage), phase ^ 1);
         const uint32_t a = sbase + stage * C::kStageBytes;
-        mbar_arrive_expect_tx(full_bar(stage), C::kStageBytes);
-        tma_load_2d(a, &P.tm_w, full_bar(stage), kb * kBlockK, n0, w_hint);
+        if (kb - kb0 >= pre) {
+          mbar_wait(empty_bar(stage), phase ^ 1);
+          mbar_arrive_expect_tx(full_bar(stage), C::kStageBytes);
+          tma_load_2d(a, &P.tm_w, full_bar(stage), kb * kBlockK, n0, w_hint);
+        }
         tma_load_2d(a + kABytes, &P.tm_x, full_bar(stage), kb * kBlockK, t0, kEvictLast);
         if (++stage == C::kStages) {
           stage = 0;
@@ -126,6 +140,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_wgmma_kernel(const __grid_co
   }
 
   // ---------------- consumers
+  griddep_wait();   // activations, residual and norm sums come from the previous kernels
   const int ctid = tid - 128, wg = ctid >> 7, wtid = ctid & 127, warp = ctid >> 5, lane = tid & 31;
   if (P.pro == GEMM3_PRO_NORM) {
     for (int t = ctid; t < BN; t += kConsumers) {
@@ -219,23 +234,71 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_wgmma_kernel(const __grid_co
     consumer_sync();
     if (!*flag_s) return;
     __threadfence();
-    const float* base = P.ws + static_cast<size_t>(tile) * S * (BN * kSlab);
-    for (int i = ctid; i < BN * kSlab / 4; i += kConsumers) {
-      float4 v = __ldcg(reinterpret_cast<const float4*>(base) + i);
+    const float4* base = reinterpret_cast<const float4*>(P.ws + static_cast<size_t>(tile) * S * (BN * kSlab));
+    // U float4 of the tile per thread at a time, all S partials of them loaded one piece after the other: U loads in
+    // flight per thread instead of one, so the sum costs S L2 round trips per U float4 rather than one per float4
+    constexpr int kPer = BN * kSlab / 4 / kConsumers, U = kPer < 16 ? kPer : 16;
+    for (int c = 0; c < kPer; c += U) {
+      float4 v[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u) v[u] = __ldcg(base + ctid + (c + u) * kConsumers);
       for (int s = 1; s < S; ++s) {   // split order: independent of which piece finished last
-        const float4 w = __ldcg(reinterpret_cast<const float4*>(base + static_cast<size_t>(s) * (BN * kSlab)) + i);
-        v.x += w.x; v.y += w.y; v.z += w.z; v.w += w.w;
+        float4 w[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) w[u] = __ldcg(base + static_cast<size_t>(s) * (BN * kSlab / 4) + ctid + (c + u) * kConsumers);
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          v[u].x += w[u].x; v[u].y += w[u].y; v[u].z += w[u].z; v[u].w += w[u].w;
+        }
       }
-      const int t = (i * 4) / kSlab, r = (i * 4) % kSlab;
-      *reinterpret_cast<float4*>(stg + t * kPitch + r) = v;
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int i = ctid + (c + u) * kConsumers, t = (i * 4) / kSlab, r = (i * 4) % kSlab;
+        *reinterpret_cast<float4*>(stg + t * kPitch + r) = v[u];
+      }
     }
     consumer_sync();
   }
 
   // ---------------- epilogue: one warp per token, each lane 4 consecutive rows of the slab
+  constexpr int kWarps = kConsumers / 32;
   const int slabs = tiles_n;
   const int t_end = min(BN, P.T - t0);
-  for (int tl = warp; tl < t_end; tl += kConsumers / 32) {
+  if (P.epi == GEMM3_EPI_RESADD) {
+    // the residual of 4 of the warp's tokens is read before any of them is written back: 4 round trips in flight per
+    // lane instead of one
+    for (int tl0 = warp; tl0 < t_end; tl0 += 4 * kWarps) {
+      float res[4][4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int tl = tl0 + j * kWarps, r = lane * 4 + e;
+          res[j][e] = tl < t_end && n0 + r < P.N ? ldbf(P.out + static_cast<size_t>(t0 + tl) * P.ldo + n0 + r) : 0.f;
+        }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int tl = tl0 + j * kWarps, t = t0 + tl;
+        if (tl >= t_end) break;
+        const float* row = stg + tl * kPitch;
+        float ss = 0.f;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int r = lane * 4 + e;
+          if (n0 + r < P.N) {
+            const __nv_bfloat16 z = __float2bfloat16_rn(bf16r(row[r]) + res[j][e]);
+            P.out[static_cast<size_t>(t) * P.ldo + n0 + r] = z;
+            const float zf = __bfloat162float(z);
+            ss += zf * zf;
+          }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+        if (lane == 0 && P.ssq_out) P.ssq_out[static_cast<size_t>(t) * slabs + slab] = ss;
+      }
+    }
+  }
+  for (int tl = warp; tl < t_end && P.epi != GEMM3_EPI_RESADD; tl += kWarps) {
     const int t = t0 + tl;
     const float* row = stg + tl * kPitch;
     if (P.epi == GEMM3_EPI_PLAIN) {
@@ -244,22 +307,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_wgmma_kernel(const __grid_co
         const int r = lane * 4 + e;
         if (n0 + r < P.N) P.out[static_cast<size_t>(t) * P.ldo + n0 + r] = __float2bfloat16_rn(row[r]);
       }
-    } else if (P.epi == GEMM3_EPI_RESADD) {
-      float ss = 0.f;
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int r = lane * 4 + e;
-        if (n0 + r < P.N) {
-          __nv_bfloat16* d = P.out + static_cast<size_t>(t) * P.ldo + n0 + r;
-          const __nv_bfloat16 z = __float2bfloat16_rn(bf16r(row[r]) + __bfloat162float(*d));
-          *d = z;
-          const float zf = __bfloat162float(z);
-          ss += zf * zf;
-        }
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-      if (lane == 0 && P.ssq_out) P.ssq_out[static_cast<size_t>(t) * slabs + slab] = ss;
     } else if (P.epi == GEMM3_EPI_SILU) {
       // rows 0..63 of the slab are gate rows, 64..127 the matching up rows; act columns [slab*64, slab*64+64)
 #pragma unroll

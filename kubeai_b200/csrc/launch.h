@@ -1,5 +1,5 @@
 // Kernel launch with the programmatic-stream-serialization attribute (PDL): the next kernel's
-// prologue (and, for the GEMM, its weight prefetch) overlaps the tail of the previous kernel.
+// prologue (and, for a decode-step GEMM, the weight loads of its first ring fill) overlaps the tail of the previous kernel.
 // Every kernel launched this way executes griddepcontrol.wait before touching dependent memory.
 #pragma once
 #include <cuda_runtime.h>
