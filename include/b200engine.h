@@ -43,7 +43,7 @@ typedef struct b200_engine b200_engine;
 
 typedef struct {
   int32_t device;             /* CUDA ordinal */
-  /* model architecture (Llama family; head_dim is fixed at 128, q_heads == 4 * kv_heads) */
+  /* model architecture (Llama family; q_heads / kv_heads = 1..16 query heads per KV head, head size in head_dim below) */
   int32_t num_layers, hidden, q_heads, kv_heads, intermediate, vocab;
   float rms_eps;              /* 1e-5 */
   float rope_theta;           /* 500000 */
@@ -73,6 +73,10 @@ typedef struct {
    * 5; one unset takes the other's value); 1 <= min <= max otherwise B200_ERR_INVALID at b200_engine_create. */
   int32_t num_speculative_tokens;
   int32_t prompt_lookup_min, prompt_lookup_max;
+  /* head size D: 64 or 128; 0 = 128.  q_heads * D and (q_heads + 2 * kv_heads) * D must be multiples of 128 (at D = 64:
+   * an even q_heads), otherwise B200_ERR_INVALID at b200_engine_create.  The KV pool holds 2 * kv_heads * 16 * D bf16 per
+   * page and layer, so D = 64 fits twice the tokens in the same memory. */
+  int32_t head_dim;
 } b200_config;
 
 /* drafts per step at most: a verify item's G query heads times its 1 + m positions share decode attention's 16-row tile,
@@ -249,7 +253,9 @@ int b200_engine_read_logits(b200_engine* e, void* host_logits_bf16, int32_t rows
 /* ------------------------------------------------------------------ checkpoints (SURVEY.md §8f-2)
  * HF-layout Llama checkpoints: <dir>/config.json + model.safetensors[.index.json] (BF16/F16/F32 tensors).
  * The reference mounts such a directory into the backend pod (internal/modelcontroller/model_source.go:231-287). */
-/* Fill the architecture fields of cfg from <dir>/config.json; rejects head_dim != 128 and a GQA ratio whose kv_heads does
+/* Fill the architecture fields of cfg from <dir>/config.json, head_dim included (config.json "head_dim", else hidden /
+ * q_heads); rejects a head_dim other than 64 and 128, an odd q_heads at head_dim 64, a head_dim that contradicts the
+ * q_proj / k_proj rows of the safetensors in <dir> (when there are any), and a GQA ratio whose kv_heads does
  * not divide q_heads or that has more than 16 query heads per KV head. */
 int b200_config_from_hf(const char* dir, b200_config* cfg);
 /* Replace the seeded weights of an idle engine with the checkpoint's (q/k/v and gate/up fused on load). */
@@ -475,6 +481,8 @@ typedef struct {
   /* epi 1 only, optional: also write normed_out [T, N] = RMSNorm(new residual) * norm_w_out (the next projection's input) */
   void* normed_out;
   const void* norm_w_out;
+  /* epi 3: head size 64 or 128 (0 = 128); a 128-row slab of w holds 128 / head_dim heads, each classified on its own */
+  int32_t head_dim;
 } b200_gemm3_args;
 int b200_op_gemm3(const b200_gemm3_args* a, void* stream, int32_t* schedule_out);
 int b200_op_embed(const void* table, const int32_t* ids, void* out, int32_t T, int32_t H, int32_t vocab, void* stream);
@@ -482,6 +490,11 @@ int b200_op_rmsnorm(const void* x, void* residual, const void* w, void* out, con
                     int32_t H, float eps, void* stream);
 int b200_op_rope_kvwrite(void* qkv, const int32_t* positions, const int32_t* slots, const void* cos_sin,
                          void* kv_layer, int32_t T, int32_t q_heads, int32_t kv_heads, int32_t max_pos, void* stream);
+/* b200_op_rope_kvwrite at head size head_dim = 64 or 128: qkv rows of (q_heads + 2 * kv_heads) * head_dim, cos_sin rows of
+ * head_dim (cos | sin), kv_layer [block][2][kv_heads][16][head_dim].  b200_op_rope_kvwrite is this at 128. */
+int b200_op_rope_kvwrite_hd(void* qkv, const int32_t* positions, const int32_t* slots, const void* cos_sin,
+                            void* kv_layer, int32_t T, int32_t q_heads, int32_t kv_heads, int32_t max_pos, int32_t head_dim,
+                            void* stream);
 int b200_op_silu_mul(const void* gate_up, void* out, int32_t T, int32_t I, void* stream);
 int b200_op_argmax(const void* logits, int32_t* out, int32_t S, int32_t V, int32_t ld, void* stream);
 /* One sampled row's parameters, as the engine packs them into a step: temperature < 1e-5 = greedy; top_k <= 0 or >= V and
@@ -534,18 +547,31 @@ int b200_op_penalize(void* logits, int32_t ld, int32_t S, int32_t V, const b200_
 int b200_op_paged_attn(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                        const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
                        int32_t q_heads, int32_t kv_heads, float scale, int32_t decode, void* stream);
+/* The attention entry points at head size head_dim = 64 or 128: q / out rows of head_dim per head, kv_layer
+ * [block][2][kv_heads][16][head_dim].  Each function without _hd is its _hd sibling at 128.  The prefill form of
+ * b200_op_paged_attn_hd (decode = 0) serves head_dim 128 only. */
+int b200_op_paged_attn_hd(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
+                          const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
+                          int32_t q_heads, int32_t kv_heads, float scale, int32_t decode, int32_t head_dim, void* stream);
 /* Decode attention with each work item's context split over `split` >= 1 CTAs per KV head (what the engine does when a step
  * has fewer decoding sequences than the device has SMs / kv_heads) and a merge of the partial softmax states.  Work items
  * and group sizes as b200_op_paged_attn with decode = 1 (q_count up to 16 / G). */
 int b200_op_paged_attn_decode_split(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                                     const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
                                     int32_t q_heads, int32_t kv_heads, float scale, int32_t split, void* stream);
+int b200_op_paged_attn_decode_split_hd(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
+                                       const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
+                                       int32_t q_heads, int32_t kv_heads, float scale, int32_t split, int32_t head_dim,
+                                       void* stream);
 /* Chunked-prefill attention on wgmma (csrc/attention_wgmma.cu): work items (q_tok0, q_count <= 64, q_pos0, seq), one CTA per
  * (work item, q head h, reading KV head h / G, G = q_heads / kv_heads in 1..16); q rows are read from the fused qkv buffer
  * [q_rows, ldq] (q heads first). */
 int b200_op_paged_attn_prefill_tc(const void* qkv, int32_t q_rows, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                                   const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
                                   int32_t q_heads, int32_t kv_heads, float scale, void* stream);
+int b200_op_paged_attn_prefill_tc_hd(const void* qkv, int32_t q_rows, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
+                                     const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
+                                     int32_t q_heads, int32_t kv_heads, float scale, int32_t head_dim, void* stream);
 int b200_op_init_uniform(void* p, uint64_t n, uint32_t seed, float scale, float offset, void* stream);
 /* The fork's page copy: for i < n_pairs and every layer l, the block_bytes at kv + l * layer_stride_bytes + src[i] * block_bytes
  * are copied to dst[i]'s page (src / dst device int32 arrays; a src may repeat).  block_bytes and layer_stride_bytes are

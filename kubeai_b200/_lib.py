@@ -30,6 +30,7 @@ class Config(C.Structure):
         ("rope_scaling_type", C.c_int32), ("rope_factor", C.c_float), ("rope_low_freq_factor", C.c_float),
         ("rope_high_freq_factor", C.c_float), ("rope_original_max_pos", C.c_int32),
         ("num_speculative_tokens", C.c_int32), ("prompt_lookup_min", C.c_int32), ("prompt_lookup_max", C.c_int32),
+        ("head_dim", C.c_int32),
     ]
 
 
@@ -40,7 +41,8 @@ class Gemm3Args(C.Structure):
                 ("norm_w", C.c_void_p), ("eps", C.c_float), ("out", C.c_void_p), ("ldo", C.c_int32),
                 ("ssq_out", C.c_void_p), ("positions", C.c_void_p), ("slots", C.c_void_p), ("cos_sin", C.c_void_p),
                 ("kv_layer", C.c_void_p), ("q_heads", C.c_int32), ("kv_heads", C.c_int32), ("max_pos", C.c_int32),
-                ("argmax_out", C.c_void_p), ("n_valid", C.c_int32), ("normed_out", C.c_void_p), ("norm_w_out", C.c_void_p)]
+                ("argmax_out", C.c_void_p), ("n_valid", C.c_int32), ("normed_out", C.c_void_p), ("norm_w_out", C.c_void_p),
+                ("head_dim", C.c_int32)]
 
 
 class Sampling(C.Structure):
@@ -205,6 +207,7 @@ SYMBOLS = {
     "b200_op_embed": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "b200_op_rmsnorm": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _f, _vp]),
     "b200_op_rope_kvwrite": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
+    "b200_op_rope_kvwrite_hd": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
     "b200_op_silu_mul": (C.c_int, [_vp, _vp, _i32, _i32, _vp]),
     "b200_op_argmax": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _vp]),
     "b200_op_sample": (C.c_int, [_vp, _i32, _vp, _i32, _i32, _vp, _vp]),
@@ -212,6 +215,7 @@ SYMBOLS = {
     "b200_op_logprobs": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "b200_op_logprobs_rank": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "b200_op_paged_attn": (C.c_int, [_vp, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _f, _i32, _vp]),
+    "b200_op_paged_attn_hd": (C.c_int, [_vp, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _f, _i32, _i32, _vp]),
     "b200_server_set_tokenizer": (C.c_int, [C.c_void_p, C.c_void_p]),
     "b200_server_render_prompt": (C.c_int64, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_size_t, _vp, C.c_size_t]),
     "b200_tokenizer_load": (C.c_int, [C.c_char_p, C.POINTER(C.c_void_p)]),
@@ -228,7 +232,11 @@ SYMBOLS = {
     "b200_attn_split_query": (C.c_int, [_i32, _i32, _i32, _i32]),
     "b200_ngram_propose": (C.c_int32, [_pi32, _i32, _i32, _i32, _i32, _i32, _pi32]),
     "b200_op_paged_attn_decode_split": (C.c_int, [_vp, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _f, _i32, _vp]),
+    "b200_op_paged_attn_decode_split_hd": (C.c_int, [_vp, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _f, _i32,
+                                                     _i32, _vp]),
     "b200_op_paged_attn_prefill_tc": (C.c_int, [_vp, _i32, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _f, _vp]),
+    "b200_op_paged_attn_prefill_tc_hd": (C.c_int, [_vp, _i32, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _f,
+                                                   _i32, _vp]),
     "b200_op_init_uniform": (C.c_int, [_vp, _u64, C.c_uint32, _f, _f, _vp]),
     "b200_op_kv_copy_blocks": (C.c_int, [_vp, _i32, _i64, _i64, _vp, _vp, _i32, _vp]),
 }

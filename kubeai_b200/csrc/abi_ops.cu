@@ -158,6 +158,11 @@ int b200_op_gemm3(const b200_gemm3_args* a, void* stream, int32_t* schedule_out)
   p.out = static_cast<__nv_bfloat16*>(a->out); p.ldo = a->ldo; p.ssq_out = a->ssq_out;
   p.positions = a->positions; p.slots = a->slots; p.cos_sin = static_cast<const __nv_bfloat16*>(a->cos_sin);
   p.kv_layer = static_cast<__nv_bfloat16*>(a->kv_layer); p.Hq = a->q_heads; p.Hkv = a->kv_heads; p.max_pos = a->max_pos;
+  p.head_dim = a->head_dim ? a->head_dim : 128;
+  if (a->epi == GEMM3_EPI_ROPE_KV && !attn_head_dim_ok(p.head_dim)) {
+    set_error("b200_op_gemm3: head_dim=%d; 64 and 128 are served", a->head_dim);
+    return B200_ERR_INVALID;
+  }
   p.cand = cand; p.n_valid = a->n_valid > 0 ? a->n_valid : a->N;
   if (a->epi == GEMM3_EPI_RESADD && a->normed_out) {
     if (!a->norm_w_out || !a->ssq_out) { set_error("b200_op_gemm3: the fused norm needs norm_w_out and ssq_out"); return B200_ERR_INVALID; }
@@ -220,9 +225,19 @@ int b200_op_rmsnorm(const void* x, void* residual, const void* w, void* out, con
 int b200_op_rope_kvwrite(void* qkv, const int32_t* positions, const int32_t* slots, const void* cos_sin,
                          void* kv_layer, int32_t T, int32_t q_heads, int32_t kv_heads, int32_t max_pos,
                          void* stream) {
+  return b200_op_rope_kvwrite_hd(qkv, positions, slots, cos_sin, kv_layer, T, q_heads, kv_heads, max_pos, 128, stream);
+}
+
+int b200_op_rope_kvwrite_hd(void* qkv, const int32_t* positions, const int32_t* slots, const void* cos_sin,
+                            void* kv_layer, int32_t T, int32_t q_heads, int32_t kv_heads, int32_t max_pos, int32_t head_dim,
+                            void* stream) {
   if (int rc = require_device()) return rc;
+  if (!attn_head_dim_ok(head_dim)) {
+    set_error("b200_op_rope_kvwrite_hd: head_dim=%d; 64 and 128 are served", head_dim);
+    return B200_ERR_INVALID;
+  }
   int rc = rope_kv_write(qkv, positions, slots, cos_sin, kv_layer, T, q_heads, kv_heads, max_pos,
-                         static_cast<cudaStream_t>(stream));
+                         static_cast<cudaStream_t>(stream), no_partials(), head_dim);
   return rc ? cuda_fail("rope_kv_write", rc) : 0;
 }
 
@@ -340,8 +355,24 @@ int b200_op_logprobs_rank(const void* logits, int32_t ld, int32_t S, int32_t V, 
 int b200_op_paged_attn(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                        const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
                        int32_t q_heads, int32_t kv_heads, float scale, int32_t decode, void* stream) {
+  return b200_op_paged_attn_hd(q, ldq, out, ldo, kv_layer, block_tables, max_blocks, work, num_work, q_heads, kv_heads, scale,
+                               decode, 128, stream);
+}
+
+int b200_op_paged_attn_hd(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
+                          const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
+                          int32_t q_heads, int32_t kv_heads, float scale, int32_t decode, int32_t head_dim, void* stream) {
   if (int rc = require_device()) return rc;
   static_assert(sizeof(AttnWork) == 16, "AttnWork is int32[4] on the wire");
+  if (!attn_head_dim_ok(head_dim)) {
+    set_error("b200_op_paged_attn: head_dim=%d; 64 and 128 are served", head_dim);
+    return B200_ERR_INVALID;
+  }
+  if (!decode && head_dim != 128) {
+    set_error("b200_op_paged_attn: the prefill form (decode = 0) serves head_dim 128 only, got %d; "
+              "chunked prefill of any head size is b200_op_paged_attn_prefill_tc_hd", head_dim);
+    return B200_ERR_INVALID;
+  }
   if (!attn_group_ok(q_heads, kv_heads)) {
     set_error("b200_op_paged_attn: q_heads=%d kv_heads=%d: kv_heads must divide q_heads with 1..16 query heads per KV head",
               q_heads, kv_heads);
@@ -354,15 +385,23 @@ int b200_op_paged_attn(const void* q, int32_t ldq, void* out, int32_t ldo, const
   }
   int rc = paged_attention(q, ldq, out, ldo, kv_layer, block_tables, max_blocks,
                            reinterpret_cast<const AttnWork*>(work), num_work, q_heads, kv_heads, scale, decode,
-                           static_cast<cudaStream_t>(stream));
+                           static_cast<cudaStream_t>(stream), nullptr, 1, head_dim);
   return rc ? cuda_fail("paged_attention", rc) : 0;
 }
 
 int b200_op_paged_attn_decode_split(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                                     const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
                                     int32_t q_heads, int32_t kv_heads, float scale, int32_t split, void* stream) {
+  return b200_op_paged_attn_decode_split_hd(q, ldq, out, ldo, kv_layer, block_tables, max_blocks, work, num_work, q_heads,
+                                            kv_heads, scale, split, 128, stream);
+}
+
+int b200_op_paged_attn_decode_split_hd(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
+                                       const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
+                                       int32_t q_heads, int32_t kv_heads, float scale, int32_t split, int32_t head_dim,
+                                       void* stream) {
   if (int rc = require_device()) return rc;
-  if (split < 1 || split > 64 || num_work <= 0 || !attn_group_ok(q_heads, kv_heads)) {
+  if (split < 1 || split > 64 || num_work <= 0 || !attn_group_ok(q_heads, kv_heads) || !attn_head_dim_ok(head_dim)) {
     set_error("b200_op_paged_attn_decode_split: bad arguments");
     return B200_ERR_INVALID;
   }
@@ -370,7 +409,7 @@ int b200_op_paged_attn_decode_split(const void* q, int32_t ldq, void* out, int32
   static size_t ws_bytes = 0;
   static std::mutex mu;
   std::lock_guard<std::mutex> lk(mu);
-  const size_t need = attn_split_ws_bytes(num_work, q_heads, split, kDecodeRows / (q_heads / kv_heads));
+  const size_t need = attn_split_ws_bytes(num_work, q_heads, split, kDecodeRows / (q_heads / kv_heads), head_dim);
   if (need > ws_bytes) {
     cudaDeviceSynchronize();
     if (ws) cudaFree(ws);
@@ -380,17 +419,24 @@ int b200_op_paged_attn_decode_split(const void* q, int32_t ldq, void* out, int32
     ws_bytes = need;
   }
   int rc = paged_attention(q, ldq, out, ldo, kv_layer, block_tables, max_blocks, reinterpret_cast<const AttnWork*>(work), num_work,
-                           q_heads, kv_heads, scale, 1, static_cast<cudaStream_t>(stream), ws, split);
+                           q_heads, kv_heads, scale, 1, static_cast<cudaStream_t>(stream), ws, split, head_dim);
   return rc ? cuda_fail("paged_attention(split)", rc) : 0;
 }
 
 int b200_op_paged_attn_prefill_tc(const void* qkv, int32_t q_rows, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                                   const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
                                   int32_t q_heads, int32_t kv_heads, float scale, void* stream) {
+  return b200_op_paged_attn_prefill_tc_hd(qkv, q_rows, ldq, out, ldo, kv_layer, block_tables, max_blocks, work, num_work, q_heads,
+                                          kv_heads, scale, 128, stream);
+}
+
+int b200_op_paged_attn_prefill_tc_hd(const void* qkv, int32_t q_rows, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
+                                     const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
+                                     int32_t q_heads, int32_t kv_heads, float scale, int32_t head_dim, void* stream) {
   if (int rc = require_device()) return rc;
   int rc = paged_attention_prefill_tc(qkv, q_rows, ldq, out, ldo, kv_layer, block_tables, max_blocks,
                                       reinterpret_cast<const AttnWork*>(work), num_work, q_heads, kv_heads, scale,
-                                      static_cast<cudaStream_t>(stream));
+                                      static_cast<cudaStream_t>(stream), head_dim);
   return rc ? cuda_fail("paged_attention_prefill_tc", rc) : 0;
 }
 

@@ -1,15 +1,17 @@
 // Paged causal attention for the per-step hot path (SURVEY.md §8a K6 decode, K7 chunked prefill).
-// Computes softmax(q . K^T / sqrt(128)) . V over the tokens reachable through a sequence's block
-// table, with G = Hq / Hkv query heads per KV head — the operation the reference backend delegates to FlashInfer/FlashAttention
+// Computes softmax(q . K^T / sqrt(D)) . V over the tokens reachable through a sequence's block
+// table, with head size D = 64 or 128 and G = Hq / Hkv query heads per KV head — the operation the reference backend
+// delegates to FlashInfer/FlashAttention
 // (vllm/model_executor/models/llama.py:223-233, vllm/v1/attention/backends/flashinfer.py).
 //
 // Design: this op is an HBM stream (decode reads 4 KiB of K+V per context token per layer),
 // so the kernel is organised around the page gather, not around the math:
-//   * KV layout is [block][K|V][kv_head][16 tokens][128] so one (page, head) is a contiguous 4 KiB
-//     run.  A layer is addressed as one 2-D tensor of 256-byte rows; ONE thread per CTA pulls a
-//     64-token tile (4 pages x {K,V} x two 64-column halves = 16 TMA boxes of 2 KiB, 128-byte swizzle)
-//     and signals an mbarrier.  The per-thread cp.async gather this replaces spent ~45% of the kernel's
-//     issue slots on address arithmetic (ncu: issue-active 43% at 12 warps/SM, 4.8 TB/s).
+//   * KV layout is [block][K|V][kv_head][16 tokens][D] so one (page, head) is a contiguous 2 * 16 * D-byte
+//     run.  A layer is addressed as one 2-D tensor of 2 * D-byte rows; ONE thread per CTA pulls a
+//     64-token tile (4 pages x {K,V} x D / 64 column halves = 8 * D / 64 TMA boxes of 2 KiB, 128-byte swizzle)
+//     and signals an mbarrier.  At D = 64 a tile is half the bytes and twice as many tiles are kept in flight.
+//     The per-thread cp.async gather this replaces spent ~45% of the kernel's issue slots on address arithmetic
+//     (ncu: issue-active 43% at 12 warps/SM, 4.8 TB/s).
 //   * decode: the G query heads of a KV head (1 <= G <= 16) ride in one m16n8k16 tensor-core tile so
 //     K/V bytes are read once per group (fp32 softmax, warp-shuffle row reductions, P rounded to bf16
 //     for P.V).  The CTA's 4 warps each own a 16-token strip of every tile and merge their
@@ -30,8 +32,10 @@
 #include <stdint.h>
 #include <stdlib.h>
 
+#include <functional>
 #include <mutex>
 #include <unordered_map>
+#include <utility>
 
 #include "gemm.h"
 #include "kernels.h"
@@ -42,24 +46,30 @@ namespace b200 {
 
 namespace {
 
-constexpr int kD = 128;
 constexpr int kTile = 64;                       // tokens per smem tile (4 pages)
 constexpr int kHalfBytes = kTile * 128;         // [64 tokens][64 dims] bf16, 128-byte rows, 128B swizzle
-constexpr int kTileBytes = 2 * kHalfBytes;      // 16 KiB for K, same for V
-constexpr int kStageBytes = 2 * kTileBytes;     // K + V
+// head size D (64 or 128): a K (or V) tile is D / 64 halves, 16 KiB at D = 128 and 8 KiB at D = 64
+template <int D>
+__host__ __device__ constexpr int tile_bytes() { return (D / 64) * kHalfBytes; }
+template <int D>
+__host__ __device__ constexpr int stage_bytes() { return 2 * tile_bytes<D>(); }  // K + V
 
-template <int S>
+template <int S, int D>
 constexpr int attn_smem_bytes() {
-  return S * kStageBytes + 64 + 1024;  // stages + mbarriers + slack for the 1 KiB alignment the swizzle needs
+  return S * stage_bytes<D>() + 64 + 1024;  // stages + mbarriers + slack for the 1 KiB alignment the swizzle needs
 }
 
-// S = tiles in flight per CTA; GC = the group size G when it is known at compile time (4), 0 = read G from group
-template <bool DECODE, int S, int GC>
+// S = tiles in flight per CTA; GC = the group size G when it is known at compile time (4), 0 = read G from group;
+// D = head size (64 or 128)
+template <bool DECODE, int S, int GC, int D>
 __global__ void __launch_bounds__(128)
 paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16* __restrict__ q, int ldq,
                   __nv_bfloat16* __restrict__ out, int ldo, const int* __restrict__ block_tables, int max_blocks,
                   const AttnWork* __restrict__ work, int Hkv, int group, float scale_log2, float* __restrict__ split_ws) {
-  static_assert(DECODE || GC == 4, "the prefill form is specialised for G = 4");
+  static_assert(DECODE || (GC == 4 && D == 128), "the prefill form is specialised for G = 4 and D = 128");
+  static_assert(D == 64 || D == 128, "head size 64 or 128");
+  constexpr int kTileBytes = tile_bytes<D>(), kStageBytes = stage_bytes<D>();
+  constexpr int KS = D / 16;  // k-steps of Q K^T, and n16 column pairs of P V
   constexpr int WT = DECODE ? 16 : 64;  // tokens of each tile handled by one warp
   constexpr int NT = WT / 8;
   const int G = GC ? GC : group;
@@ -105,10 +115,10 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
       int page = tile * 4 + pg;
       page = page > last_page ? last_page : page;
       const int blk = __ldg(btab + page);
-      const int row_k = ((blk * 2) * Hkv + kvh) * 16;  // row of the layer's [rows][128] view
+      const int row_k = ((blk * 2) * Hkv + kvh) * 16;  // row of the layer's [rows][D] view
       const int row_v = row_k + Hkv * 16;
 #pragma unroll
-      for (int half = 0; half < 2; ++half) {
+      for (int half = 0; half < D / 64; ++half) {
         tma_load_2d(dst + half * kHalfBytes + pg * 2048, &tm_kv, full_bar(stage), half * 64, row_k, hint);
         tma_load_2d(dst + kTileBytes + half * kHalfBytes + pg * 2048, &tm_kv, full_bar(stage), half * 64, row_v, hint);
       }
@@ -131,25 +141,25 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
   }
   if (!waited) griddep_enter();
 
-  // ---- Q fragments (A operand, 16 rows x 128 d as 8 k-steps)
+  // ---- Q fragments (A operand, 16 rows x D dims as D / 16 k-steps)
   // decode: fragment rows g and g + 8 are tile rows r = G * j + h, i.e. (j, h) = divmod(r, G); prefill: query tokens
   const int j0 = DECODE ? g / G : g, j1 = DECODE ? (g + 8) / G : g + 8;
-  uint32_t qf[8][4];
+  uint32_t qf[KS][4];
   {
     const __nv_bfloat16* r0p = nullptr;
     const __nv_bfloat16* r1p = nullptr;
     if (DECODE) {
       // rows past the live ones (G * q_count) stay zero: they never touch the rows of the positions that exist
       const int nrows = G * wk.q_count;
-      if (g < nrows) r0p = q + static_cast<size_t>(wk.q_tok0 + j0) * ldq + (kvh * G + g - j0 * G) * kD;
-      if (g + 8 < nrows) r1p = q + static_cast<size_t>(wk.q_tok0 + j1) * ldq + (kvh * G + g + 8 - j1 * G) * kD;
+      if (g < nrows) r0p = q + static_cast<size_t>(wk.q_tok0 + j0) * ldq + (kvh * G + g - j0 * G) * D;
+      if (g + 8 < nrows) r1p = q + static_cast<size_t>(wk.q_tok0 + j1) * ldq + (kvh * G + g + 8 - j1 * G) * D;
     } else {
       const int head = kvh * 4 + warp;
-      if (g < wk.q_count) r0p = q + static_cast<size_t>(wk.q_tok0 + g) * ldq + head * kD;
-      if (g + 8 < wk.q_count) r1p = q + static_cast<size_t>(wk.q_tok0 + g + 8) * ldq + head * kD;
+      if (g < wk.q_count) r0p = q + static_cast<size_t>(wk.q_tok0 + g) * ldq + head * D;
+      if (g + 8 < wk.q_count) r1p = q + static_cast<size_t>(wk.q_tok0 + g + 8) * ldq + head * D;
     }
 #pragma unroll
-    for (int ks = 0; ks < 8; ++ks) {
+    for (int ks = 0; ks < KS; ++ks) {
       const int d = ks * 16 + tq * 2;
       qf[ks][0] = r0p ? *reinterpret_cast<const uint32_t*>(r0p + d) : 0u;
       qf[ks][1] = r1p ? *reinterpret_cast<const uint32_t*>(r1p + d) : 0u;
@@ -158,9 +168,9 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
     }
   }
 
-  float o[16][4];
+  float o[2 * KS][4];
 #pragma unroll
-  for (int i = 0; i < 16; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
+  for (int i = 0; i < 2 * KS; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
   float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
   const int wo = DECODE ? warp * 16 : 0;  // this warp's token offset inside a tile
 
@@ -176,13 +186,13 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
 #pragma unroll
       for (int i = 0; i < NT; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f;
       const int mi = lane >> 3, ri = lane & 7;
-      // smem address of 16-byte chunk `chunk` (0..15 over the 128 dims) of token row `tok` of a K or V tile
+      // smem address of 16-byte chunk `chunk` (0..D/8-1 over the D dims) of token row `tok` of a K or V tile
       auto chunk_addr = [&](uint32_t base, int tok, int chunk) {
         return base + (chunk >> 3) * kHalfBytes + tok * 128 + (((chunk & 7) ^ (tok & 7)) << 4);
       };
       // ---- S = Q K^T
 #pragma unroll
-      for (int ks = 0; ks < 8; ++ks) {
+      for (int ks = 0; ks < KS; ++ks) {
 #pragma unroll
         for (int tp = 0; tp < WT / 16; ++tp) {
           const int tok = wo + tp * 16 + (mi >> 1) * 8 + ri;
@@ -229,7 +239,7 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
       l0 = l0 * a0 + ps0;
       l1 = l1 * a1 + ps1;
 #pragma unroll
-      for (int i = 0; i < 16; ++i) {
+      for (int i = 0; i < 2 * KS; ++i) {
         o[i][0] *= a0;
         o[i][1] *= a0;
         o[i][2] *= a1;
@@ -244,7 +254,7 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
         pa[2] = pack_bf16x2(s[2 * kk + 1][0], s[2 * kk + 1][1]);
         pa[3] = pack_bf16x2(s[2 * kk + 1][2], s[2 * kk + 1][3]);
 #pragma unroll
-        for (int dp = 0; dp < 8; ++dp) {
+        for (int dp = 0; dp < KS; ++dp) {
           const int tok = wo + kk * 16 + (mi & 1) * 8 + ri;
           const int chunk = dp * 2 + (mi >> 1);
           uint32_t b0, b1, b2, b3;
@@ -267,29 +277,29 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
     const int head = kvh * 4 + warp;
     const float i0 = l0 > 0.f ? 1.f / l0 : 0.f, i1 = l1 > 0.f ? 1.f / l1 : 0.f;
     if (g < wk.q_count) {
-      __nv_bfloat16* dst = out + static_cast<size_t>(wk.q_tok0 + g) * ldo + head * kD + tq * 2;
+      __nv_bfloat16* dst = out + static_cast<size_t>(wk.q_tok0 + g) * ldo + head * D + tq * 2;
 #pragma unroll
-      for (int dn = 0; dn < 16; ++dn)
+      for (int dn = 0; dn < 2 * KS; ++dn)
         *reinterpret_cast<uint32_t*>(dst + dn * 8) = pack_bf16x2(o[dn][0] * i0, o[dn][1] * i0);
     }
     if (g + 8 < wk.q_count) {
-      __nv_bfloat16* dst = out + static_cast<size_t>(wk.q_tok0 + g + 8) * ldo + head * kD + tq * 2;
+      __nv_bfloat16* dst = out + static_cast<size_t>(wk.q_tok0 + g + 8) * ldo + head * D + tq * 2;
 #pragma unroll
-      for (int dn = 0; dn < 16; ++dn)
+      for (int dn = 0; dn < 2 * KS; ++dn)
         *reinterpret_cast<uint32_t*>(dst + dn * 8) = pack_bf16x2(o[dn][2] * i1, o[dn][3] * i1);
     }
   } else {
     // merge the 4 warps' partial softmax states: row r = G * j + h of each warp tile is head kvh * G + h at query position
     // j.  The stages are free here (the loop's last barrier followed the last tile, and no gather is in flight).
-    float* so = reinterpret_cast<float*>(smem);            // [4 warps][16 rows][128]
-    float* sm = so + 4 * 16 * kD;                          // [4][16]
+    float* so = reinterpret_cast<float*>(smem);            // [4 warps][16 rows][D]
+    float* sm = so + 4 * 16 * D;                           // [4][16]
     float* sl = sm + 4 * 16;                               // [4][16]
     const int nrows = G * wk.q_count;
     if (g < nrows) {
 #pragma unroll
-      for (int dn = 0; dn < 16; ++dn) {
+      for (int dn = 0; dn < 2 * KS; ++dn) {
         float2 v = make_float2(o[dn][0], o[dn][1]);
-        *reinterpret_cast<float2*>(so + (warp * 16 + g) * kD + dn * 8 + tq * 2) = v;
+        *reinterpret_cast<float2*>(so + (warp * 16 + g) * D + dn * 8 + tq * 2) = v;
       }
       if (tq == 0) {
         sm[warp * 16 + g] = m0;
@@ -298,9 +308,9 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
     }
     if (g + 8 < nrows) {
 #pragma unroll
-      for (int dn = 0; dn < 16; ++dn) {
+      for (int dn = 0; dn < 2 * KS; ++dn) {
         float2 v = make_float2(o[dn][2], o[dn][3]);
-        *reinterpret_cast<float2*>(so + (warp * 16 + g + 8) * kD + dn * 8 + tq * 2) = v;
+        *reinterpret_cast<float2*>(so + (warp * 16 + g + 8) * D + dn * 8 + tq * 2) = v;
       }
       if (tq == 0) {
         sm[warp * 16 + g + 8] = m1;
@@ -308,8 +318,10 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
       }
     }
     __syncthreads();
-    const int d = tid;
-    for (int r = 0; r < nrows; ++r) {
+    // 128 / D rows at a time: thread tid owns dim tid % D of rows tid / D, tid / D + 128 / D, ... (at D = 128 the block's
+    // 128 threads make tid / D zero; it is spelled out so that the D = 128 code is the single-row loop)
+    const int d = D == 128 ? tid : tid % D;
+    for (int r = D == 128 ? 0 : tid / D; r < nrows; r += 128 / D) {
       const int j = r / G, h = r - j * G;
       float mm = -INFINITY;
 #pragma unroll
@@ -319,21 +331,21 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
       for (int w = 0; w < 4; ++w) {
         const float mw = sm[w * 16 + r];
         const float wgt = (mw == -INFINITY) ? 0.f : exp2f(mw - mm);
-        num += so[(w * 16 + r) * kD + d] * wgt;
+        num += so[(w * 16 + r) * D + d] * wgt;
         den += sl[w * 16 + r] * wgt;
       }
       if (parts == 1) {
-        out[static_cast<size_t>(wk.q_tok0 + j) * ldo + (kvh * G + h) * kD + d] = __float2bfloat16_rn(den > 0.f ? num / den : 0.f);
+        out[static_cast<size_t>(wk.q_tok0 + j) * ldo + (kvh * G + h) * D + d] = __float2bfloat16_rn(den > 0.f ? num / den : 0.f);
       } else {
-        // position j's slab of [position][work][kv head][part][G heads][128 acc | max | sum]: a launch whose items all
+        // position j's slab of [position][work][kv head][part][G heads][D acc | max | sum]: a launch whose items all
         // have q_count == 1 uses slab 0 only
-        const size_t slab = static_cast<size_t>(gridDim.y) * Hkv * parts * (G * (kD + 2));
-        float* dst = split_ws + j * slab + ((static_cast<size_t>(blockIdx.y) * Hkv + kvh) * parts + part) * (G * (kD + 2)) +
-                     h * (kD + 2);
+        const size_t slab = static_cast<size_t>(gridDim.y) * Hkv * parts * (G * (D + 2));
+        float* dst = split_ws + j * slab + ((static_cast<size_t>(blockIdx.y) * Hkv + kvh) * parts + part) * (G * (D + 2)) +
+                     h * (D + 2);
         dst[d] = num;
         if (d == 0) {
-          dst[kD] = mm;
-          dst[kD + 1] = den;
+          dst[D] = mm;
+          dst[D + 1] = den;
         }
       }
     }
@@ -341,26 +353,28 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
 }
 
 // out[token, head, :] = sum_p acc_p 2^(m_p - M) / sum_p l_p 2^(m_p - M) over the parts of a split decode work item
+template <int D>
 __global__ void __launch_bounds__(128)
 attn_merge_kernel(const float* __restrict__ split_ws, __nv_bfloat16* __restrict__ out, int ldo, const AttnWork* __restrict__ work,
                   int Hkv, int G, int parts) {
   griddep_enter();
   const AttnWork wk = work[blockIdx.y];
-  const int kvh = blockIdx.x, d = threadIdx.x;
-  const size_t slab = static_cast<size_t>(gridDim.y) * Hkv * parts * (G * (kD + 2));
-  for (int r = 0; r < G * wk.q_count; ++r) {
+  // 128 / D rows at a time, as in the decode kernel's epilogue
+  const int kvh = blockIdx.x, d = D == 128 ? threadIdx.x : threadIdx.x % D;
+  const size_t slab = static_cast<size_t>(gridDim.y) * Hkv * parts * (G * (D + 2));
+  for (int r = D == 128 ? 0 : threadIdx.x / D; r < G * wk.q_count; r += 128 / D) {
     const int j = r / G, h = r - j * G;
-    const float* base = split_ws + j * slab + (static_cast<size_t>(blockIdx.y) * Hkv + kvh) * parts * (G * (kD + 2));
+    const float* base = split_ws + j * slab + (static_cast<size_t>(blockIdx.y) * Hkv + kvh) * parts * (G * (D + 2));
     float mm = -INFINITY;
-    for (int p = 0; p < parts; ++p) mm = fmaxf(mm, base[(p * G + h) * (kD + 2) + kD]);
+    for (int p = 0; p < parts; ++p) mm = fmaxf(mm, base[(p * G + h) * (D + 2) + D]);
     float num = 0.f, den = 0.f;
     for (int p = 0; p < parts; ++p) {
-      const float* s = base + (p * G + h) * (kD + 2);
-      const float wgt = (s[kD] == -INFINITY) ? 0.f : exp2f(s[kD] - mm);
+      const float* s = base + (p * G + h) * (D + 2);
+      const float wgt = (s[D] == -INFINITY) ? 0.f : exp2f(s[D] - mm);
       num += s[d] * wgt;
-      den += s[kD + 1] * wgt;
+      den += s[D + 1] * wgt;
     }
-    out[static_cast<size_t>(wk.q_tok0 + j) * ldo + (kvh * G + h) * kD + d] = __float2bfloat16_rn(den > 0.f ? num / den : 0.f);
+    out[static_cast<size_t>(wk.q_tok0 + j) * ldo + (kvh * G + h) * D + d] = __float2bfloat16_rn(den > 0.f ? num / den : 0.f);
   }
 }
 
@@ -375,22 +389,26 @@ int decode_stages() {  // B200_ATTN_STAGES=2|3|4 (tiles in flight per decode CTA
   return v;
 }
 
-// One tensor map per KV-layer base pointer: the layer is viewed as [rows][128] bf16 with 256-byte rows, gathered in
-// boxes of 16 rows x 64 columns (one page-head half).  The row count is an upper bound, not the allocation size: the
-// kernel only ever addresses pages named by the block table.
+// One tensor map per (KV-layer base pointer, head size D): the layer is viewed as [rows][D] bf16 with 2 * D-byte rows,
+// gathered in boxes of 16 rows x 64 columns (one page-head half at D = 128, one page-head at D = 64).  The row count is an
+// upper bound, not the allocation size: the kernel only ever addresses pages named by the block table.  The key holds D
+// because the allocator may hand a freed layer's address to a pool of the other head size.
 }  // namespace
 
-int kv_map_for(const void* kv_layer, CUtensorMap* out) {
-  static std::unordered_map<const void*, CUtensorMap> cache;
+int kv_map_for(const void* kv_layer, CUtensorMap* out, int head_dim) {
+  struct KeyHash {
+    size_t operator()(const std::pair<const void*, int>& k) const { return std::hash<const void*>()(k.first) ^ k.second; }
+  };
+  static std::unordered_map<std::pair<const void*, int>, CUtensorMap, KeyHash> cache;
   static std::mutex mu;
   std::lock_guard<std::mutex> lk(mu);
-  auto it = cache.find(kv_layer);
+  auto it = cache.find({kv_layer, head_dim});
   if (it == cache.end()) {
     CUtensorMap tm;
     if ((reinterpret_cast<uintptr_t>(kv_layer) & 255) != 0) return -5;
-    if (int rc = tmap_encode_bf16_2d(&tm, kv_layer, 1ull << 30, kD, kD, 16, 64, 1)) return rc;
+    if (int rc = tmap_encode_bf16_2d(&tm, kv_layer, 1ull << 30, head_dim, head_dim, 16, 64, 1)) return rc;
     if (cache.size() > 4096) cache.clear();
-    it = cache.emplace(kv_layer, tm).first;
+    it = cache.emplace(std::make_pair(kv_layer, head_dim), tm).first;
   }
   *out = it->second;
   return 0;
@@ -398,38 +416,41 @@ int kv_map_for(const void* kv_layer, CUtensorMap* out) {
 
 namespace {
 
-template <bool DECODE, int S, int GC>
+template <bool DECODE, int S, int GC, int D = 128>
 int launch_attn(const CUtensorMap& tm, dim3 grid, cudaStream_t st, const __nv_bfloat16* q, int ldq, __nv_bfloat16* out,
                 int ldo, const int* block_tables, int max_blocks, const AttnWork* work, int Hkv, int G, float scale_log2,
                 float* split_ws = nullptr) {
   static std::atomic<unsigned long long> attr_done{0};
-  if (!ensure_dynamic_smem(paged_attn_kernel<DECODE, S, GC>, attn_smem_bytes<S>(), &attr_done)) return -3;
-  launch_pdl(paged_attn_kernel<DECODE, S, GC>, grid, dim3(128), attn_smem_bytes<S>(), st, tm, q, ldq, out, ldo, block_tables,
+  if (!ensure_dynamic_smem(paged_attn_kernel<DECODE, S, GC, D>, attn_smem_bytes<S, D>(), &attr_done)) return -3;
+  launch_pdl(paged_attn_kernel<DECODE, S, GC, D>, grid, dim3(128), attn_smem_bytes<S, D>(), st, tm, q, ldq, out, ldo, block_tables,
              max_blocks, work, Hkv, G, scale_log2, split_ws);
   if (cudaGetLastError() != cudaSuccess) return -2;
   if (DECODE && grid.z > 1) {
-    launch_pdl(attn_merge_kernel, dim3(grid.x, grid.y), dim3(128), 0, st, static_cast<const float*>(split_ws), out, ldo, work, Hkv,
+    launch_pdl(attn_merge_kernel<D>, dim3(grid.x, grid.y), dim3(128), 0, st, static_cast<const float*>(split_ws), out, ldo, work, Hkv,
                G, static_cast<int>(grid.z));
     if (cudaGetLastError() != cudaSuccess) return -2;
   }
   return 0;
 }
 
-template <int GC>
+// A 64-token tile is 32 KiB of K + V at D = 128 and 16 KiB at D = 64, so D = 64 keeps twice the tiles in flight: the bytes
+// in flight per CTA are the same at both head sizes for every B200_ATTN_STAGES setting.
+template <int GC, int D>
 int launch_decode(const CUtensorMap& tm, dim3 grid, cudaStream_t st, const __nv_bfloat16* q, int ldq, __nv_bfloat16* out,
                   int ldo, const int* block_tables, int max_blocks, const AttnWork* work, int Hkv, int G, float scale_log2,
                   float* split_ws) {
+  constexpr int M = 128 / D;
   switch (decode_stages()) {
-    case 3: return launch_attn<true, 3, GC>(tm, grid, st, q, ldq, out, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
-    case 4: return launch_attn<true, 4, GC>(tm, grid, st, q, ldq, out, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
-    default: return launch_attn<true, 2, GC>(tm, grid, st, q, ldq, out, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
+    case 3: return launch_attn<true, 3 * M, GC, D>(tm, grid, st, q, ldq, out, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
+    case 4: return launch_attn<true, 4 * M, GC, D>(tm, grid, st, q, ldq, out, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
+    default: return launch_attn<true, 2 * M, GC, D>(tm, grid, st, q, ldq, out, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
   }
 }
 
 }  // namespace
 
-size_t attn_split_ws_bytes(int num_work, int Hq, int parts, int max_q) {
-  return static_cast<size_t>(max_q) * num_work * Hq * parts * (kD + 2) * sizeof(float);
+size_t attn_split_ws_bytes(int num_work, int Hq, int parts, int max_q, int head_dim) {
+  return static_cast<size_t>(max_q) * num_work * Hq * parts * (head_dim + 2) * sizeof(float);
 }
 
 // Parts per decode work item such that the launch has about two CTAs per SM, each with at least two 64-token tiles.
@@ -445,21 +466,25 @@ int attn_decode_split(int num_work, int Hkv, int max_ctx, int sms) {
 
 int paged_attention(const void* q, int ldq, void* out, int ldo, const void* kv_layer, const int* block_tables,
                     int max_blocks, const AttnWork* work, int num_work, int Hq, int Hkv, float scale,
-                    int decode, cudaStream_t st, float* split_ws, int split) {
+                    int decode, cudaStream_t st, float* split_ws, int split, int head_dim) {
   if (num_work <= 0) return 0;
-  if (!attn_group_ok(Hq, Hkv) || (!decode && Hq != 4 * Hkv)) return -1;
+  if (!attn_group_ok(Hq, Hkv) || !attn_head_dim_ok(head_dim) || (!decode && (Hq != 4 * Hkv || head_dim != 128))) return -1;
   if (split > 1 && (!decode || !split_ws)) return -1;
   const int G = Hq / Hkv;
   CUtensorMap tm;
-  if (int rc = kv_map_for(kv_layer, &tm)) return rc;
+  if (int rc = kv_map_for(kv_layer, &tm, head_dim)) return rc;
   const float scale_log2 = scale * 1.4426950408889634f;
   dim3 grid(Hkv, num_work, split > 1 ? split : 1);
   const __nv_bfloat16* qq = static_cast<const __nv_bfloat16*>(q);
   __nv_bfloat16* oo = static_cast<__nv_bfloat16*>(out);
   if (!decode)
     return launch_attn<false, kPrefillStages, 4>(tm, grid, st, qq, ldq, oo, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2);
-  if (G == 4) return launch_decode<4>(tm, grid, st, qq, ldq, oo, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
-  return launch_decode<0>(tm, grid, st, qq, ldq, oo, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
+  if (head_dim == 64) {
+    if (G == 4) return launch_decode<4, 64>(tm, grid, st, qq, ldq, oo, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
+    return launch_decode<0, 64>(tm, grid, st, qq, ldq, oo, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
+  }
+  if (G == 4) return launch_decode<4, 128>(tm, grid, st, qq, ldq, oo, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
+  return launch_decode<0, 128>(tm, grid, st, qq, ldq, oo, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
 }
 
 }  // namespace b200

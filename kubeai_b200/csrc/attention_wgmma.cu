@@ -1,14 +1,16 @@
 // Chunked-prefill paged attention on the Hopper tensor cores (SURVEY.md §8a K7): for every query token of a work item,
-// softmax(q . K^T / sqrt(128)) . V over the causal prefix gathered through the sequence's block table, with G = Hq / Hkv
-// query heads per KV head (1 <= G <= 16) — the
+// softmax(q . K^T / sqrt(D)) . V over the causal prefix gathered through the sequence's block table, with head size D = 64
+// or 128 and G = Hq / Hkv query heads per KV head (1 <= G <= 16) — the
 // operation the reference backend delegates to FlashInfer/FlashAttention (vllm/model_executor/models/llama.py:223-233).
 //
 // H100 design: one CTA = one warpgroup = (work item of up to 64 query tokens, one query head h, reading KV head h / G).
-//   * Q [64 tokens][128] sits in shared memory as two 64-column halves in the 128-byte-swizzled K-major layout wgmma reads;
-//     each 64-token K tile goes to the same layout, V is transposed into [128 dims][64 tokens] (K-major for P . V).
-//   * S = Q K^T: wgmma m64n64k16 with both operands from shared-memory descriptors, fp32 accumulators in registers.
+//   * Q [64 tokens][D] sits in shared memory as D / 64 64-column halves in the 128-byte-swizzled K-major layout wgmma reads;
+//     each 64-token K tile goes to the same layout, V is transposed into [D dims][64 tokens] (K-major for P . V).
+//   * S = Q K^T: wgmma m64n64k16 (D / 16 k-steps) with both operands from shared-memory descriptors, fp32 accumulators in
+//     registers.
 //   * online softmax in registers (row max / sum over the 4 threads of a quad), P rounded to bf16 and fed to O += P V as
-//     the register A operand of wgmma (the accumulator fragment of S is the A fragment of P V), O in registers.
+//     the register A operand of wgmma m64n64k16 (the accumulator fragment of S is the A fragment of P V), one n64 column
+//     block of O per 64 dims, O in registers.
 // Tokens past the context are not read: their K / V rows are zero and their scores masked.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -25,28 +27,32 @@ namespace b200 {
 
 namespace {
 
-constexpr int kD = 128;
 constexpr int kQ = kPrefillQueryBlock;   // 64 query tokens per work item = the wgmma M tile
 constexpr int kKv = 64;                  // kv tokens per tile
 constexpr int kHalf = 64 * 128;          // [64 rows][64 bf16] swizzled: 8 KB
-constexpr int kSmem = 1024 + 3 * 2 * kHalf;   // Q, K, V^T
+template <int D>
+constexpr int smem_bytes() { return 1024 + 3 * (D / 64) * kHalf; }   // Q, K, V^T
 
 // byte offset of 16-byte chunk c of row r in a 128B-swizzled tile (base 1024-B aligned)
 __device__ __forceinline__ uint32_t swz(int r, int c) { return r * 128 + ((c ^ (r & 7)) << 4); }
 
+template <int D>
 __global__ void __launch_bounds__(128) prefill_attn_wgmma_kernel(const __nv_bfloat16* __restrict__ qkv, int qkv_rows, int ldq,
                                                                  __nv_bfloat16* __restrict__ out, int ldo,
                                                                  const __nv_bfloat16* __restrict__ kv_layer,
                                                                  const int* __restrict__ block_tables, int max_blocks,
                                                                  const AttnWork* __restrict__ work, int Hkv, int G,
                                                                  float scale_log2) {
+  static_assert(D == 64 || D == 128, "head size 64 or 128");
+  constexpr int NH = D / 64;          // 64-column halves of Q and K, n64 column blocks of O
+  constexpr int kC = D / 8, kCL = D == 128 ? 4 : 3;   // 16-byte chunks of a row, log2
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem = smem_raw + (sbase - smem_u32(smem_raw));
-  uint8_t* sq = smem;                 // two halves: dims 0..63, 64..127
-  uint8_t* sk = smem + 2 * kHalf;
-  uint8_t* sv = smem + 4 * kHalf;     // V^T: rows = dims 0..127, 64 tokens each
-  const uint32_t aq = sbase, ak = sbase + 2 * kHalf, av = sbase + 4 * kHalf;
+  uint8_t* sq = smem;                 // NH halves: dims 0..63, 64..127
+  uint8_t* sk = smem + NH * kHalf;
+  uint8_t* sv = smem + 2 * NH * kHalf;   // V^T: rows = dims 0..D-1, 64 tokens each
+  const uint32_t aq = sbase, ak = sbase + NH * kHalf, av = sbase + 2 * NH * kHalf;
 
   // work[] and block_tables were uploaded before the first kernel of the step: readable ahead of the dependency wait
   const AttnWork wk = work[blockIdx.y];
@@ -54,24 +60,24 @@ __global__ void __launch_bounds__(128) prefill_attn_wgmma_kernel(const __nv_bflo
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int* btab = block_tables + static_cast<size_t>(wk.seq) * max_blocks;
   const int kv_end = wk.q_pos0 + wk.q_count;
-  const size_t head_stride = 16 * kD, kind_stride = static_cast<size_t>(Hkv) * head_stride;
+  const size_t head_stride = 16 * D, kind_stride = static_cast<size_t>(Hkv) * head_stride;
   griddep_enter();
 
   // ---- Q tile (rows past the work item read as zero)
-  for (int i = tid; i < kQ * 16; i += 128) {
-    const int r = i >> 4, c = i & 15;
+  for (int i = tid; i < kQ * kC; i += 128) {
+    const int r = i >> kCL, c = i & (kC - 1);
     uint4 v = make_uint4(0, 0, 0, 0);
     if (r < wk.q_count && wk.q_tok0 + r < qkv_rows)
-      v = *reinterpret_cast<const uint4*>(qkv + static_cast<size_t>(wk.q_tok0 + r) * ldq + h * kD + c * 8);
+      v = *reinterpret_cast<const uint4*>(qkv + static_cast<size_t>(wk.q_tok0 + r) * ldq + h * D + c * 8);
     *reinterpret_cast<uint4*>(sq + (c >> 3) * kHalf + swz(r, c & 7)) = v;
   }
 
   // this thread's accumulator rows (wgmma D fragment): r0 and r0 + 8
   const int r0 = warp * 16 + (lane >> 2);
   const int qpos0 = wk.q_pos0 + r0, qpos1 = qpos0 + 8;
-  float o[2][32];
+  float o[NH][32];
 #pragma unroll
-  for (int j = 0; j < 2; ++j)
+  for (int j = 0; j < NH; ++j)
 #pragma unroll
     for (int i = 0; i < 32; ++i) o[j][i] = 0.f;
   float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
@@ -80,12 +86,12 @@ __global__ void __launch_bounds__(128) prefill_attn_wgmma_kernel(const __nv_bflo
   for (int t = 0; t < ntiles; ++t) {
     const int j0 = t * kKv;
     __syncthreads();   // the previous tile's wgmma reads are complete (wait_group 0 below) in every warp
-    // ---- K tile [64 tokens][128 dims] and V^T [128 dims][64 tokens]
-    for (int i = tid; i < kKv * 16; i += 128) {
-      const int r = i >> 4, c = i & 15, j = j0 + r;
+    // ---- K tile [64 tokens][D dims] and V^T [D dims][64 tokens]
+    for (int i = tid; i < kKv * kC; i += 128) {
+      const int r = i >> kCL, c = i & (kC - 1), j = j0 + r;
       uint4 kvec = make_uint4(0, 0, 0, 0), vvec = kvec;   // tokens past the context: no page to read, masked below
       if (j < kv_end) {
-        const size_t base = static_cast<size_t>(__ldg(btab + (j >> 4))) * 2 * kind_stride + kvh * head_stride + (j & 15) * kD + c * 8;
+        const size_t base = static_cast<size_t>(__ldg(btab + (j >> 4))) * 2 * kind_stride + kvh * head_stride + (j & 15) * D + c * 8;
         kvec = *reinterpret_cast<const uint4*>(kv_layer + base);
         vvec = *reinterpret_cast<const uint4*>(kv_layer + base + kind_stride);
       }
@@ -106,7 +112,7 @@ __global__ void __launch_bounds__(128) prefill_attn_wgmma_kernel(const __nv_bflo
     for (int i = 0; i < 32; ++i) s[i] = 0.f;
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < kD / 16; ++kk) {
+    for (int kk = 0; kk < D / 16; ++kk) {
       const uint32_t off = (kk >> 2) * kHalf + (kk & 3) * 32;
       wgmma_m64n64(s, gmma_desc(aq + off), gmma_desc(ak + off));
     }
@@ -150,7 +156,7 @@ __global__ void __launch_bounds__(128) prefill_attn_wgmma_kernel(const __nv_bflo
     l0 = l0 * c0 + ps0;
     l1 = l1 * c1 + ps1;
 #pragma unroll
-    for (int j = 0; j < 2; ++j)
+    for (int j = 0; j < NH; ++j)
 #pragma unroll
       for (int q = 0; q < 8; ++q) {
         o[j][q * 4 + 0] *= c0;
@@ -164,7 +170,7 @@ __global__ void __launch_bounds__(128) prefill_attn_wgmma_kernel(const __nv_bflo
 #pragma unroll
     for (int kk = 0; kk < kKv / 16; ++kk)
 #pragma unroll
-      for (int j = 0; j < 2; ++j) wgmma_m64n64_rs(o[j], pa[kk], gmma_desc(av + j * kHalf + kk * 32));
+      for (int j = 0; j < NH; ++j) wgmma_m64n64_rs(o[j], pa[kk], gmma_desc(av + j * kHalf + kk * 32));
     wgmma_commit();
     wgmma_wait<0>();
   }
@@ -177,32 +183,40 @@ __global__ void __launch_bounds__(128) prefill_attn_wgmma_kernel(const __nv_bflo
   }
   const float inv0 = l0 > 0.f ? 1.f / l0 : 0.f, inv1 = l1 > 0.f ? 1.f / l1 : 0.f;
 #pragma unroll
-  for (int j = 0; j < 2; ++j)
+  for (int j = 0; j < NH; ++j)
 #pragma unroll
     for (int q = 0; q < 8; ++q) {
       const int d = j * 64 + q * 8 + (lane & 3) * 2;
       if (r0 < wk.q_count)
-        *reinterpret_cast<uint32_t*>(out + static_cast<size_t>(wk.q_tok0 + r0) * ldo + h * kD + d) =
+        *reinterpret_cast<uint32_t*>(out + static_cast<size_t>(wk.q_tok0 + r0) * ldo + h * D + d) =
             pack_bf16x2(o[j][q * 4 + 0] * inv0, o[j][q * 4 + 1] * inv0);
       if (r0 + 8 < wk.q_count)
-        *reinterpret_cast<uint32_t*>(out + static_cast<size_t>(wk.q_tok0 + r0 + 8) * ldo + h * kD + d) =
+        *reinterpret_cast<uint32_t*>(out + static_cast<size_t>(wk.q_tok0 + r0 + 8) * ldo + h * D + d) =
             pack_bf16x2(o[j][q * 4 + 2] * inv1, o[j][q * 4 + 3] * inv1);
     }
+}
+
+template <int D>
+int launch_prefill(const void* qkv, int qkv_rows, int ldq, void* out, int ldo, const void* kv_layer, const int* block_tables,
+                   int max_blocks, const AttnWork* work, int num_work, int Hq, int Hkv, float scale, cudaStream_t st) {
+  static std::atomic<unsigned long long> attr_done{0};
+  if (!ensure_dynamic_smem(prefill_attn_wgmma_kernel<D>, smem_bytes<D>(), &attr_done)) return -3;
+  cudaError_t e = launch_pdl(prefill_attn_wgmma_kernel<D>, dim3(Hq, num_work), dim3(128), smem_bytes<D>(), st,
+                             static_cast<const __nv_bfloat16*>(qkv), qkv_rows, ldq, static_cast<__nv_bfloat16*>(out), ldo,
+                             static_cast<const __nv_bfloat16*>(kv_layer), block_tables, max_blocks, work, Hkv, Hq / Hkv,
+                             scale * 1.4426950408889634f);
+  return e == cudaSuccess ? 0 : -2;
 }
 
 }  // namespace
 
 int paged_attention_prefill_tc(const void* qkv, int qkv_rows, int ldq, void* out, int ldo, const void* kv_layer, const int* block_tables,
-                               int max_blocks, const AttnWork* work, int num_work, int Hq, int Hkv, float scale, cudaStream_t st) {
+                               int max_blocks, const AttnWork* work, int num_work, int Hq, int Hkv, float scale, cudaStream_t st,
+                               int head_dim) {
   if (num_work <= 0) return 0;
-  if (!attn_group_ok(Hq, Hkv) || qkv_rows <= 0 || ldq % 8 || ldo % 2) return -1;
-  static std::atomic<unsigned long long> attr_done{0};
-  if (!ensure_dynamic_smem(prefill_attn_wgmma_kernel, kSmem, &attr_done)) return -3;
-  cudaError_t e = launch_pdl(prefill_attn_wgmma_kernel, dim3(Hq, num_work), dim3(128), kSmem, st,
-                             static_cast<const __nv_bfloat16*>(qkv), qkv_rows, ldq, static_cast<__nv_bfloat16*>(out), ldo,
-                             static_cast<const __nv_bfloat16*>(kv_layer), block_tables, max_blocks, work, Hkv, Hq / Hkv,
-                             scale * 1.4426950408889634f);
-  return e == cudaSuccess ? 0 : -2;
+  if (!attn_group_ok(Hq, Hkv) || !attn_head_dim_ok(head_dim) || qkv_rows <= 0 || ldq % 8 || ldo % 2) return -1;
+  return head_dim == 64 ? launch_prefill<64>(qkv, qkv_rows, ldq, out, ldo, kv_layer, block_tables, max_blocks, work, num_work, Hq, Hkv, scale, st)
+                        : launch_prefill<128>(qkv, qkv_rows, ldq, out, ldo, kv_layer, block_tables, max_blocks, work, num_work, Hq, Hkv, scale, st);
 }
 
 }  // namespace b200

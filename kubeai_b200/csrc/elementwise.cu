@@ -149,12 +149,14 @@ __global__ void rmsnorm_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat1
 }
 
 // ------------------------------------------------------------------ RoPE (neox) + paged KV write
-// qkv: [T, (Hq + 2*Hkv) * 128], q and k rotated in place; k,v rows scattered to the paged cache
-// kv layout per layer: [block][2][Hkv][16][128]  (head-major inside a page: one (page,head) = 4 KiB contiguous)
+// qkv: [T, (Hq + 2*Hkv) * D], q and k rotated in place; k,v rows scattered to the paged cache; D = 64 or 128
+// kv layout per layer: [block][2][Hkv][16][D]  (head-major inside a page: one (page,head) = 32 * D bytes contiguous)
+template <int D>
 __global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ qkv, const int* __restrict__ positions,
                                const int* __restrict__ slots, const __nv_bfloat16* __restrict__ cos_sin,
                                __nv_bfloat16* __restrict__ kv, int Hq, int Hkv, int max_pos, PartialView pv) {
-  constexpr int D = 128, HALF = 64;
+  constexpr int HALF = D / 2, RT = HALF / 8, VT = D / 8;  // rotation / V-copy tasks per head
+  constexpr int RTL = D == 128 ? 3 : 2, VTL = RTL + 1;     // their log2
   const int t = blockIdx.x;
   // ---- before the dependency wait: step inputs (positions, slots), cos/sin rows and table entries (static).  The
   // first task of every thread is prepared here; later tasks (only when blockDim < tasks) look theirs up afterwards.
@@ -163,18 +165,18 @@ __global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ qkv, const int* __res
   const int slot = slots[t];
   const int ld = (Hq + 2 * Hkv) * D;
   __nv_bfloat16* row = qkv + static_cast<size_t>(t) * ld;
-  const __nv_bfloat16* cs = cos_sin + static_cast<size_t>(pos) * D;  // cos[0:64] | sin[0:64]
+  const __nv_bfloat16* cs = cos_sin + static_cast<size_t>(pos) * D;  // cos[0:D/2] | sin[0:D/2]
   const int blk = slot >> 4, off = slot & 15;
   const size_t page_stride = static_cast<size_t>(Hkv) * 16 * D;  // elements per K (or V) page over all heads
   __nv_bfloat16* kbase = kv + static_cast<size_t>(blk) * 2 * page_stride;
   __nv_bfloat16* vbase = kbase + page_stride;
 
-  const int rot_tasks = (Hq + Hkv) * (HALF / 8);  // 8 elements of x1 (and the matching 8 of x2) per task
-  const int v_tasks = Hkv * (D / 8);
+  const int rot_tasks = (Hq + Hkv) * RT;  // 8 elements of x1 (and the matching 8 of x2) per task
+  const int v_tasks = Hkv * VT;
   Vec8 co0, si0;
   int2 ent0[2] = {make_int2(0, 1), make_int2(0, 1)};
   if (static_cast<int>(threadIdx.x) < rot_tasks) {
-    const int head = threadIdx.x >> 3, c = threadIdx.x & 7;
+    const int head = threadIdx.x >> RTL, c = threadIdx.x & (RT - 1);
     co0.u = __ldg(reinterpret_cast<const uint4*>(cs + c * 8));
     si0.u = __ldg(reinterpret_cast<const uint4*>(cs + HALF + c * 8));
     if (pv.ws) {
@@ -185,7 +187,7 @@ __global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ qkv, const int* __res
   griddep_enter();
   // rotation tasks and V-copy tasks share one index space so that a 512-thread CTA gives every thread one task
   for (int task = threadIdx.x; task < rot_tasks; task += blockDim.x) {
-    const int head = task >> 3, c = task & 7;
+    const int head = task >> RTL, c = task & (RT - 1);
     const bool first = task == static_cast<int>(threadIdx.x);
     __nv_bfloat16* hp = row + head * D;
     Vec8 co, si, o1, o2;
@@ -249,7 +251,7 @@ __global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ qkv, const int* __res
     // start the V tasks where the rotation tasks ended so idle threads of the first pass take them
     for (int task = static_cast<int>((threadIdx.x + blockDim.x - rot_tasks % blockDim.x) % blockDim.x); task < v_tasks;
          task += blockDim.x) {
-      const int head = task >> 4, c = task & 15;
+      const int head = task >> VTL, c = task & (VT - 1);
       uint4 val;
       if (pv.ws) {
         float f[8];
@@ -460,13 +462,15 @@ int rmsnorm(const void* x, void* residual, const void* w, void* out, const int* 
 }
 
 int rope_kv_write(void* qkv, const int* positions, const int* slots, const void* cos_sin, void* kv_layer,
-                  int T, int Hq, int Hkv, int max_pos, cudaStream_t st, PartialView pv) {
+                  int T, int Hq, int Hkv, int max_pos, cudaStream_t st, PartialView pv, int head_dim) {
   if (T <= 0) return 0;
-  const int tasks = (Hq + Hkv) * 8 + Hkv * 16;
+  if (head_dim != 64 && head_dim != 128) return -1;
+  const int tasks = ((Hq + Hkv) * 8 + Hkv * 16) * head_dim / 128;
   // decode: one task per thread (latency); prefill bursts: 128-thread CTAs (throughput; measured 21 vs 31 us at T=2048)
   const int threads = T >= 512 ? 128 : tasks >= 512 ? 512 : tasks >= 256 ? 256 : 128;
-  launch_pdl(rope_kv_kernel, dim3(T), dim3(threads), 0, st, static_cast<__nv_bfloat16*>(qkv), positions, slots,
-             static_cast<const __nv_bfloat16*>(cos_sin), static_cast<__nv_bfloat16*>(kv_layer), Hq, Hkv, max_pos, pv);
+  launch_pdl(head_dim == 64 ? rope_kv_kernel<64> : rope_kv_kernel<128>, dim3(T), dim3(threads), 0, st,
+             static_cast<__nv_bfloat16*>(qkv), positions, slots, static_cast<const __nv_bfloat16*>(cos_sin),
+             static_cast<__nv_bfloat16*>(kv_layer), Hq, Hkv, max_pos, pv);
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 

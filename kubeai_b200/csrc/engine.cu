@@ -43,7 +43,6 @@ namespace b200 {
 
 namespace {
 
-constexpr int kD = 128;
 constexpr int kPage = 16;
 typedef __nv_bfloat16 bf16;
 
@@ -291,6 +290,22 @@ struct XMaps {
   CUtensorMap m[kGemmNumBlockN];  // token tiles 32, 64, 128, 256, 512
 };
 
+// ------------------------------------------------------------------ head size
+// The head size of a config (0 = 128); B200_ERR_INVALID unless it is 64 or 128 and the rows of q and of the whole qkv
+// projection are whole 128-row slabs, the unit of the qkv GEMM's RoPE / KV-write epilogue.  A slab holds 128 / D heads and
+// classifies each on its own, so it may hold the last k head and the first v head (an odd kv_heads at D = 64).
+int head_dim_resolve(const b200_config& c, int* D) {
+  const int d = c.head_dim ? c.head_dim : 128;
+  if (!attn_head_dim_ok(d) || (c.q_heads * d) % 128 || ((c.q_heads + 2 * c.kv_heads) * d) % 128) {
+    set_error("unsupported head_dim %d with %d query and %d KV heads (head_dim 64 or 128; q_heads * head_dim and "
+              "(q_heads + 2 * kv_heads) * head_dim must be multiples of 128, so head_dim 64 needs an even q_heads)",
+              d, c.q_heads, c.kv_heads);
+    return B200_ERR_INVALID;
+  }
+  *D = d;
+  return 0;
+}
+
 // ------------------------------------------------------------------ speculative decoding
 // The speculative settings of a config with vLLM's defaults for the lookup lengths (config/speculative.py: both unset gives
 // 5 and 5, one unset takes the other's value); B200_ERR_INVALID when out of range.  A verify item of the last token and m
@@ -372,6 +387,7 @@ int ngram_propose(const int32_t* toks, int n, int min_n, int max_n, int k, int m
 struct Engine {
   b200_config cfg;
   int L, H, Hq, Hkv, I, V, QKV;
+  int Dh = 128;   // head size: 64 or 128 (b200_config.head_dim)
   // n-gram speculative decoding: drafts per decoding sequence (0 = off) and the lookup n-gram lengths
   int spec_k = 0, spec_min = 0, spec_max = 0;
   int Tcap, Scap, max_blocks_per_seq;
@@ -502,10 +518,10 @@ struct Engine {
     int split = 1;
     if (m.nd <= kSplitMaxWork) split = std::min(attn_split_force > 0 ? attn_split_force : attn_decode_split(m.nd, Hkv, m.dmax_ctx, sms), kSplitMaxParts);
     if (split > 1) ++stats.kernel_launches;   // the merge kernel
-    return paged_attention(qkv, QKV, attn, Hq * kD, kv_l, btab, max_blocks_per_seq, dwork, m.nd, Hq, Hkv, scale, 1, stream, attn_ws, split);
+    return paged_attention(qkv, QKV, attn, Hq * Dh, kv_l, btab, max_blocks_per_seq, dwork, m.nd, Hq, Hkv, scale, 1, stream, attn_ws, split, Dh);
   }
   int prefill_attention(bf16* kv_l, const int* btab, const AttnWork* pwork, int np, float scale) {
-    return paged_attention_prefill_tc(qkv, Tcap, QKV, attn, Hq * kD, kv_l, btab, max_blocks_per_seq, pwork, np, Hq, Hkv, scale, stream);
+    return paged_attention_prefill_tc(qkv, Tcap, QKV, attn, Hq * Dh, kv_l, btab, max_blocks_per_seq, pwork, np, Hq, Hkv, scale, stream, Dh);
   }
   // one scheduler iteration = launch (schedule, pack, H2D, kernels, D2H enqueue) + complete (sync, apply) + publish
   int schedule(std::vector<Sched>& sched);
@@ -644,12 +660,12 @@ int Engine::alloc_all() {
   std::vector<Item> items;
   layers.resize(L);
   const float s_h = 1.0f / sqrtf(static_cast<float>(H)), s_i = 1.0f / sqrtf(static_cast<float>(I)),
-              s_a = 1.0f / sqrtf(static_cast<float>(Hq * kD));
+              s_a = 1.0f / sqrtf(static_cast<float>(Hq * Dh));
   items.push_back({"embed", static_cast<size_t>(V) * H, &embed, 1.0f, 0.f});
   for (int l = 0; l < L; ++l) {
     std::string p = "layers." + std::to_string(l) + ".";
     items.push_back({p + "wqkv", static_cast<size_t>(QKV) * H, &layers[l].wqkv, s_h, 0.f});
-    items.push_back({p + "wo", static_cast<size_t>(H) * Hq * kD, &layers[l].wo, s_a, 0.f});
+    items.push_back({p + "wo", static_cast<size_t>(H) * Hq * Dh, &layers[l].wo, s_a, 0.f});
     items.push_back({p + "wgu", static_cast<size_t>(2) * I * H, &layers[l].wgu, s_h, 0.f});
     items.push_back({p + "wdown", static_cast<size_t>(H) * I, &layers[l].wdown, s_i, 0.f});
     items.push_back({p + "norm1", static_cast<size_t>(H), &layers[l].norm1, 0.1f, 1.0f});
@@ -663,7 +679,7 @@ int Engine::alloc_all() {
     offs.push_back(total);
     total += align_up(it.elems * 2, 1024);
   }
-  const size_t cs_elems = static_cast<size_t>(cfg.max_model_len) * kD;
+  const size_t cs_elems = static_cast<size_t>(cfg.max_model_len) * Dh;
   const size_t cs_off = total;
   total += align_up(cs_elems * 2, 1024);
   weights_bytes = total;
@@ -689,9 +705,9 @@ int Engine::alloc_all() {
   {
     // vllm rotary_embedding/base.py:70-92: inv_freq = base^(-2i/d); cache = cos(t*f) | sin(t*f), cast to bf16
     std::vector<bf16> h(cs_elems);
-    std::vector<float> inv(kD / 2);
-    for (int i = 0; i < kD / 2; ++i)
-      inv[i] = 1.0f / powf(cfg.rope_theta, static_cast<float>(2 * i) / static_cast<float>(kD));
+    std::vector<float> inv(Dh / 2);
+    for (int i = 0; i < Dh / 2; ++i)
+      inv[i] = 1.0f / powf(cfg.rope_theta, static_cast<float>(2 * i) / static_cast<float>(Dh));
     float pos_div = 1.0f;
     if (cfg.rope_scaling_type == 1) {
       // LinearScalingRotaryEmbedding (rotary_embedding/linear_scaling_rope.py): t / factor
@@ -700,7 +716,7 @@ int Engine::alloc_all() {
       // Llama3RotaryEmbedding._compute_inv_freq (rotary_embedding/llama3_rope.py:37-54)
       const float orig = static_cast<float>(cfg.rope_original_max_pos);
       const float low_wl = orig / cfg.rope_low_freq_factor, high_wl = orig / cfg.rope_high_freq_factor;
-      for (int i = 0; i < kD / 2; ++i) {
+      for (int i = 0; i < Dh / 2; ++i) {
         const float wl = 2.0f * static_cast<float>(M_PI) / inv[i];
         if (wl < high_wl) continue;
         if (wl > low_wl || cfg.rope_low_freq_factor == cfg.rope_high_freq_factor) { inv[i] = inv[i] / cfg.rope_factor; continue; }
@@ -709,10 +725,10 @@ int Engine::alloc_all() {
       }
     }
     for (int t = 0; t < cfg.max_model_len; ++t)
-      for (int i = 0; i < kD / 2; ++i) {
+      for (int i = 0; i < Dh / 2; ++i) {
         const float f = static_cast<float>(t) / pos_div * inv[i];
-        h[static_cast<size_t>(t) * kD + i] = __float2bfloat16_rn(cosf(f));
-        h[static_cast<size_t>(t) * kD + kD / 2 + i] = __float2bfloat16_rn(sinf(f));
+        h[static_cast<size_t>(t) * Dh + i] = __float2bfloat16_rn(cosf(f));
+        h[static_cast<size_t>(t) * Dh + Dh / 2 + i] = __float2bfloat16_rn(sinf(f));
       }
     CK(cudaMemcpyAsync(cos_sin, h.data(), cs_elems * 2, cudaMemcpyHostToDevice, stream));
     CK(cudaStreamSynchronize(stream));
@@ -723,13 +739,13 @@ int Engine::alloc_all() {
   CK(cudaMalloc(&x, static_cast<size_t>(Tcap) * H * 2));
   CK(cudaMalloc(&normed, static_cast<size_t>(Tcap) * H * 2));
   CK(cudaMalloc(&qkv, static_cast<size_t>(Tcap) * QKV * 2));
-  CK(cudaMalloc(&attn, static_cast<size_t>(Tcap) * Hq * kD * 2));
+  CK(cudaMalloc(&attn, static_cast<size_t>(Tcap) * Hq * Dh * 2));
   CK(cudaMalloc(&gu, static_cast<size_t>(Tcap) * 2 * I * 2));
   CK(cudaMalloc(&act, static_cast<size_t>(Tcap) * I * 2));
   CK(cudaMalloc(&last_hidden, static_cast<size_t>(Scap) * H * 2));
   CK(cudaMalloc(&logits, static_cast<size_t>(Scap) * V * 2));
   CK(cudaMemset(normed, 0, static_cast<size_t>(Tcap) * H * 2));
-  CK(cudaMemset(attn, 0, static_cast<size_t>(Tcap) * Hq * kD * 2));
+  CK(cudaMemset(attn, 0, static_cast<size_t>(Tcap) * Hq * Dh * 2));
   CK(cudaMemset(act, 0, static_cast<size_t>(Tcap) * I * 2));
   CK(cudaMemset(last_hidden, 0, static_cast<size_t>(Scap) * H * 2));
   if (int rc = alloc_readbacks(Scap, Scap, 0)) return rc;   // the prompt-logprob records come after the KV pool
@@ -739,11 +755,11 @@ int Engine::alloc_all() {
   tensors["step.sampled"] = {sampled, static_cast<size_t>(Scap) * 4};
   tensors["step.argmax_candidates"] = {cand, static_cast<size_t>(std::min(Scap, 128)) * ((V + 127) / 128) * sizeof(float2)};
   tensors["step.logits"] = {logits, static_cast<size_t>(Scap) * V * 2};
-  CK(cudaMalloc(&attn_ws, attn_split_ws_bytes(kSplitMaxWork, Hq, kSplitMaxParts, 1 + spec_k)));
+  CK(cudaMalloc(&attn_ws, attn_split_ws_bytes(kSplitMaxWork, Hq, kSplitMaxParts, 1 + spec_k, Dh)));
   { const char* e = getenv("B200_ATTN_SPLIT"); attn_split_force = e ? atoi(e) : 0; }
   // split-K workspace and arrival counters: the largest need of any projection at any step size up to Tcap
   {
-    const int shapes[5][2] = {{QKV, H}, {H, Hq * kD}, {2 * I, H}, {H, I}, {V, H}};
+    const int shapes[5][2] = {{QKV, H}, {H, Hq * Dh}, {2 * I, H}, {H, I}, {V, H}};
     size_t ws_bytes = 1 << 20;
     int counters = 1024;
     const int t_max = std::max(Tcap, Scap);
@@ -767,7 +783,7 @@ int Engine::alloc_all() {
     return gemm_plan_init(p, W, N, K, K, gemm_ws, gemm_ws_bytes, gemm_counters, gemm_counters_cap);
   };
   for (int l = 0; l < L; ++l) {
-    if (plan(&layers[l].p_qkv, layers[l].wqkv, QKV, H) || plan(&layers[l].p_o, layers[l].wo, H, Hq * kD) ||
+    if (plan(&layers[l].p_qkv, layers[l].wqkv, QKV, H) || plan(&layers[l].p_o, layers[l].wo, H, Hq * Dh) ||
         plan(&layers[l].p_gu, layers[l].wgu, 2 * I, H) || plan(&layers[l].p_down, layers[l].wdown, H, I))
       return cuda_fail("gemm_plan_init", -2);
   }
@@ -775,7 +791,7 @@ int Engine::alloc_all() {
   const int bns[kGemmNumBlockN] = {64, 128, 256};
   for (int i = 0; i < kGemmNumBlockN; ++i) {
     if (gemm_make_x_map(&xm_normed.m[i], normed, Tcap, H, H, bns[i]) ||
-        gemm_make_x_map(&xm_attn.m[i], attn, Tcap, Hq * kD, Hq * kD, bns[i]) ||
+        gemm_make_x_map(&xm_attn.m[i], attn, Tcap, Hq * Dh, Hq * Dh, bns[i]) ||
         gemm_make_x_map(&xm_act.m[i], act, Tcap, I, I, bns[i]) ||
         gemm_make_x_map(&xm_last.m[i], last_hidden, Scap, H, H, bns[i]))
       return cuda_fail("gemm_make_x_map", -2);
@@ -791,7 +807,7 @@ int Engine::alloc_all() {
   }
 
   // ---- KV pool
-  const size_t block_bytes_layer = static_cast<size_t>(2) * Hkv * kPage * kD * 2;
+  const size_t block_bytes_layer = static_cast<size_t>(2) * Hkv * kPage * Dh * 2;
   int64_t nblocks = cfg.num_kv_blocks;
   if (nblocks <= 0) {
     size_t fr = 0, tot = 0;
@@ -808,7 +824,7 @@ int Engine::alloc_all() {
     return B200_ERR_OOM;
   }
   if (nblocks > (1 << 27)) nblocks = 1 << 27;
-  kv_layer_elems = static_cast<size_t>(nblocks) * 2 * Hkv * kPage * kD;
+  kv_layer_elems = static_cast<size_t>(nblocks) * 2 * Hkv * kPage * Dh;
   CK(cudaMalloc(&kv, kv_layer_elems * 2 * L));
   // the attention kernel gathers whole pages and masks the rows past a sequence's end: those rows must be finite
   CK(cudaMemsetAsync(kv, 0, kv_layer_elems * 2 * L, stream));
@@ -851,7 +867,8 @@ int Engine::alloc_all() {
 int Engine::init(const b200_config& c) {
   cfg = c;
   L = c.num_layers; H = c.hidden; Hq = c.q_heads; Hkv = c.kv_heads; I = c.intermediate; V = c.vocab;
-  QKV = (Hq + 2 * Hkv) * kD;
+  if (int rc = head_dim_resolve(c, &Dh)) return rc;
+  QKV = (Hq + 2 * Hkv) * Dh;
   // the constraints of every kernel the forward launches, checked here so that a bad shape fails at create time with a
   // message instead of poisoning the replica at its first step: RMSNorm rows are 256-element multiples up to 8192,
   // argmax and the partial readers use 8-element vectors, GEMM K dims are 64-element TMA boxes
@@ -902,7 +919,7 @@ int Engine::forward(const StepMeta& m, int32_t* dbuf, bool all_logits, bf16* log
   const AttnWork* dwork = reinterpret_cast<const AttnWork*>(dbuf + m.off_dwork);
   const AttnWork* pwork = reinterpret_cast<const AttnWork*>(dbuf + m.off_pwork);
   const int* btab = dbuf + m.off_btab;
-  const float scale = 1.0f / sqrtf(static_cast<float>(kD));
+  const float scale = 1.0f / sqrtf(static_cast<float>(Dh));
   int rc = 0;
   auto launched = [&](int n) { stats.kernel_launches += n; };
   // profiling: P(cls) before a launch group, Q() after it
@@ -950,11 +967,11 @@ int Engine::forward(const StepMeta& m, int32_t* dbuf, bool all_logits, bf16* log
     if (on(B200_K_GEMM_QKV)) {
       Gemm3Params p = proj(ly.p_qkv, fused ? GEMM3_EPI_ROPE_KV : GEMM3_EPI_PLAIN);
       p.out = qkv; p.ldo = QKV;
-      p.positions = pos; p.slots = slots; p.cos_sin = cos_sin; p.kv_layer = kv_l; p.Hq = Hq; p.Hkv = Hkv; p.max_pos = cfg.max_model_len;
+      p.positions = pos; p.slots = slots; p.cos_sin = cos_sin; p.kv_layer = kv_l; p.Hq = Hq; p.Hkv = Hkv; p.max_pos = cfg.max_model_len; p.head_dim = Dh;
       rc |= launch_proj(p, xm_normed, T);
     }
     Q();
-    if (!fused) { P(B200_K_ROPE); if (on(B200_K_ROPE)) rc |= rope_kv_write(qkv, pos, slots, cos_sin, kv_l, T, Hq, Hkv, cfg.max_model_len, stream); Q(); launched(1); }
+    if (!fused) { P(B200_K_ROPE); if (on(B200_K_ROPE)) rc |= rope_kv_write(qkv, pos, slots, cos_sin, kv_l, T, Hq, Hkv, cfg.max_model_len, stream, no_partials(), Dh); Q(); launched(1); }
     if (m.nd) { P(B200_K_ATTN_DECODE); if (on(B200_K_ATTN_DECODE)) rc |= decode_attention(m, kv_l, btab, dwork, scale); Q(); launched(1); }
     if (m.np) { P(B200_K_ATTN_PREFILL); if (on(B200_K_ATTN_PREFILL)) rc |= prefill_attention(kv_l, btab, pwork, m.np, scale); Q(); launched(1); }
     P(B200_K_GEMM_O); if (on(B200_K_GEMM_O)) resadd_proj(ly.p_o, xm_attn); Q();
@@ -1519,7 +1536,7 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
   }
   if (!frc && m.n_fork > 0) {   // likewise: after this step wrote the prompt's KV, before the next step writes past it
     ++stats.kernel_launches;
-    const size_t block_bytes = static_cast<size_t>(2) * Hkv * kPage * kD * 2;
+    const size_t block_bytes = static_cast<size_t>(2) * Hkv * kPage * Dh * 2;
     if (kv_copy_blocks(kv, L, static_cast<int64_t>(kv_layer_elems) * 2, static_cast<int64_t>(block_bytes), dbuf + m.off_fork,
                        dbuf + m.off_fork + m.n_fork, m.n_fork, stream))
       frc = cuda_fail("kv_copy_blocks", -2);
@@ -1846,8 +1863,9 @@ void b200_config_default(b200_config* c) {
 int b200_engine_create(const b200_config* cfg, b200_engine** out) {
   if (!cfg || !out) { set_error("null argument"); return B200_ERR_INVALID; }
   {
-    int k, mn, mx;   // checked before the device so that a bad speculative config reads the same on every host
+    int k, mn, mx, d;   // checked before the device so that a bad speculative config or head size reads the same on every host
     if (int rc = spec_resolve(*cfg, &k, &mn, &mx)) return rc;
+    if (int rc = head_dim_resolve(*cfg, &d)) return rc;
   }
   if (int rc = require_device()) return rc;
   b200_engine* e = new (std::nothrow) b200_engine();

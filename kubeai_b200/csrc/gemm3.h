@@ -39,6 +39,7 @@ struct Gemm3Params {
   const __nv_bfloat16* cos_sin;
   __nv_bfloat16* kv_layer;
   int Hq, Hkv, max_pos;
+  int head_dim;       // 64 or 128; a 128-row slab holds 128 / head_dim heads
   // ARGMAX: per (token, 128-row slab) {best logit, index as int bits}; columns >= n_valid are ignored
   float2* cand;
   int n_valid;

@@ -69,7 +69,8 @@ __device__ __forceinline__ void dispatch_width(int nw, F&& f) {
   f(std::integral_constant<int, BN>{});
 }
 
-template <int BN>
+// HD: the head size of the ROPE_KV epilogue (128, or 64 for the qkv projection of a 64-dimensional-head model)
+template <int BN, int HD>
 __global__ void __launch_bounds__(kThreads, 1) gemm_wgmma_kernel(const __grid_constant__ Gemm3Params P, int S) {
   using C = Cfg<BN>;
   extern __shared__ uint8_t smem_raw[];
@@ -315,7 +316,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_wgmma_kernel(const __grid_co
         const __nv_bfloat16 s = silu_bf16(bf16r(row[r]));
         P.out[static_cast<size_t>(t) * P.ldo + slab * 64 + r] = __float2bfloat16_rn(__bfloat162float(s) * bf16r(row[r + 64]));
       }
-    } else if (P.epi == GEMM3_EPI_ROPE_KV) {
+    } else if (P.epi == GEMM3_EPI_ROPE_KV && HD == 128) {
       // one 128-row slab = one head of the fused qkv projection
       const int head = slab;
       const size_t page_stride = static_cast<size_t>(P.Hkv) * 16 * 128;
@@ -348,6 +349,56 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_wgmma_kernel(const __grid_co
                              (static_cast<size_t>(vh) * 16 + (slot & 15)) * 128;
 #pragma unroll
         for (int e = 0; e < 4; ++e) dst[lane * 4 + e] = __float2bfloat16_rn(row[lane * 4 + e]);
+      }
+    } else if (HD == 64 && P.epi == GEMM3_EPI_ROPE_KV) {
+      // D = 64: one 128-row slab = two heads of the fused qkv projection (q heads, then k, then v); the rotation pairs
+      // rows (r, r + 32) of a head.  Heads are classified one by one, so a slab may hold the last k head and the first v
+      // head (an odd kv_heads).
+      constexpr int hd_log2 = 6, half_log2 = 5, D = 64, HALF = 32;
+      const int head0 = slab << (7 - hd_log2);           // first head of the slab
+      const size_t page_stride = static_cast<size_t>(P.Hkv) * 16 * D;
+      const int slot = head0 + (128 >> hd_log2) > P.Hq ? __ldg(P.slots + t) : 0;
+      __nv_bfloat16* kpage = P.kv_layer + static_cast<size_t>(slot >> 4) * 2 * page_stride;
+      if (head0 < P.Hq + P.Hkv) {
+        int pos = __ldg(P.positions + t);
+        pos = pos < 0 ? 0 : (pos >= P.max_pos ? P.max_pos - 1 : pos);
+        const __nv_bfloat16* cs = P.cos_sin + (static_cast<size_t>(pos) << hd_log2);
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int p = lane * 2 + e;                     // pair p of the slab's 64
+          const int head = head0 + (p >> half_log2), r = p & (HALF - 1);
+          const int ra = ((p >> half_log2) << hd_log2) + r;  // slab row of the pair's first element
+          const float a = bf16r(row[ra]), b = bf16r(row[ra + HALF]);
+          __nv_bfloat16 o1, o2;
+          if (head < P.Hq + P.Hkv) {
+            const float cc = ldbf(cs + r), sn = ldbf(cs + HALF + r);
+            // every bf16 op rounds, as in elementwise.cu rope_kv_kernel
+            const float ac = bf16r(__fmul_rn(a, cc)), bs = bf16r(__fmul_rn(b, sn));
+            const float bc = bf16r(__fmul_rn(b, cc)), as = bf16r(__fmul_rn(a, sn));
+            o1 = __float2bfloat16_rn(ac - bs);
+            o2 = __float2bfloat16_rn(bc + as);
+          } else {                                        // a v head sharing the slab with the last k head
+            o1 = __float2bfloat16_rn(a);
+            o2 = __float2bfloat16_rn(b);
+          }
+          __nv_bfloat16* dst = nullptr;
+          if (head < P.Hq) dst = P.out + static_cast<size_t>(t) * P.ldo + (head << hd_log2);
+          else if (slot >= 0)
+            dst = kpage + (head < P.Hq + P.Hkv ? 0 : page_stride) +
+                  ((static_cast<size_t>(head < P.Hq + P.Hkv ? head - P.Hq : head - P.Hq - P.Hkv) * 16 + (slot & 15)) << hd_log2);
+          if (dst) {
+            dst[r] = o1;
+            dst[r + HALF] = o2;
+          }
+        }
+      } else if (slot >= 0) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int rr = lane * 4 + e;
+          const int vh = head0 + (rr >> hd_log2) - P.Hq - P.Hkv;
+          __nv_bfloat16* dst = kpage + page_stride + ((static_cast<size_t>(vh) * 16 + (slot & 15)) << hd_log2);
+          dst[rr & (D - 1)] = __float2bfloat16_rn(row[rr]);
+        }
       }
     } else {  // GEMM3_EPI_ARGMAX: best bf16 logit of this slab, lowest index on ties
       const int nv = min(P.N, P.n_valid);
@@ -464,14 +515,14 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-template <int BN>
+template <int BN, int HD>
 int launch(const Gemm3Params& p, const Gemm3Schedule& sch, cudaStream_t st) {
   using C = Cfg<BN>;
   static std::atomic<unsigned long long> attr_done{0};
-  if (!ensure_dynamic_smem(gemm_wgmma_kernel<BN>, C::kSmem, &attr_done)) return -3;
+  if (!ensure_dynamic_smem(gemm_wgmma_kernel<BN, HD>, C::kSmem, &attr_done)) return -3;
   const int slabs = (p.N + kSlab - 1) / kSlab, ntt = (p.T + BN - 1) / BN;
   const dim3 grid = ntt > 1 ? dim3(ntt, slabs, sch.S) : dim3(slabs, 1, sch.S);   // see the kernel's CTA order
-  cudaError_t e = launch_pdl(gemm_wgmma_kernel<BN>, grid, dim3(kThreads), C::kSmem, st, p, sch.S);
+  cudaError_t e = launch_pdl(gemm_wgmma_kernel<BN, HD>, grid, dim3(kThreads), C::kSmem, st, p, sch.S);
   return e == cudaSuccess ? 0 : -4;
 }
 
@@ -586,10 +637,19 @@ int gemm3_launch(const Gemm3Params& p, const Gemm3Schedule& sch, cudaStream_t st
   if ((p.epi == GEMM3_EPI_SILU || p.epi == GEMM3_EPI_ROPE_KV) && p.N % kSlab) return -5;   // whole heads / gate-up slab pairs
   if (p.epi == GEMM3_EPI_RESADD && p.normed_out && (!p.ssq_out || !p.norm_w_out)) return -5;
   if (p.pro == GEMM3_PRO_NORM && (!p.ssq_in || !p.norm_w)) return -5;
+  if (p.epi == GEMM3_EPI_ROPE_KV && p.head_dim != 0 && p.head_dim != 64 && p.head_dim != 128) return -5;
+  if (p.epi == GEMM3_EPI_ROPE_KV && p.head_dim == 64) {
+    switch (sch.block_n) {
+      case 64: return launch<64, 64>(p, sch, st);
+      case 128: return launch<128, 64>(p, sch, st);
+      case 256: return launch<256, 64>(p, sch, st);
+      default: return -6;
+    }
+  }
   switch (sch.block_n) {
-    case 64: return launch<64>(p, sch, st);
-    case 128: return launch<128>(p, sch, st);
-    case 256: return launch<256>(p, sch, st);
+    case 64: return launch<64, 128>(p, sch, st);
+    case 128: return launch<128, 128>(p, sch, st);
+    case 256: return launch<256, 128>(p, sch, st);
     default: return -6;
   }
 }

@@ -20,8 +20,9 @@ int embed_gather(const void* table, const int* ids, void* out, int T, int H, int
 // stream-K partials of the preceding deferred GEMM (summed + rounded to bf16 on load) instead of the bf16 tensor.
 int rmsnorm(const void* x, void* residual, const void* w, void* out, const int* row_index, int rows, int H,
             float eps, cudaStream_t st, PartialView pv = no_partials());
+// head_dim D = 64 or 128: qkv rows [(Hq + 2 Hkv) * D], cos_sin rows [D], kv_layer [block][2][Hkv][16][D]
 int rope_kv_write(void* qkv, const int* positions, const int* slots, const void* cos_sin, void* kv_layer,
-                  int T, int Hq, int Hkv, int max_pos, cudaStream_t st, PartialView pv = no_partials());
+                  int T, int Hq, int Hkv, int max_pos, cudaStream_t st, PartialView pv = no_partials(), int head_dim = 128);
 // interleaved: gate/up columns alternate in 64-column blocks (engine layout) instead of [gate | up]
 int silu_mul(const void* gate_up, void* out, int T, int I, cudaStream_t st, PartialView pv = no_partials(), int interleaved = 0);
 // gate_up weight rows: logical [gate | up] <-> physical (64 gate rows, their 64 up rows, ...); dst != src
@@ -105,24 +106,28 @@ constexpr int kDecodeRows = 16;
 // the group sizes G = Hq / Hkv the attention kernels serve: Hkv divides Hq and 1 <= G <= 16
 inline bool attn_group_ok(int Hq, int Hkv) { return Hkv >= 1 && Hq % Hkv == 0 && Hq / Hkv >= 1 && Hq / Hkv <= kDecodeRows; }
 
-// Paged causal attention, head_dim 128, G = Hq / Hkv query heads per KV head (attn_group_ok), page = 16 tokens.
-//   q: rows of the fused qkv buffer (leading dim ldq), out: [T, Hq*128] (leading dim ldo)
-//   kv_layer: [block][2][Hkv][16][128];  block_tables: [num_seqs, max_blocks] int32
+// the head sizes D the attention kernels, the qkv epilogue and the KV pool serve
+inline bool attn_head_dim_ok(int D) { return D == 64 || D == 128; }
+
+// Paged causal attention, head_dim D (attn_head_dim_ok), G = Hq / Hkv query heads per KV head (attn_group_ok), page = 16 tokens.
+//   q: rows of the fused qkv buffer (leading dim ldq), out: [T, Hq*D] (leading dim ldo)
+//   kv_layer: [block][2][Hkv][16][D];  block_tables: [num_seqs, max_blocks] int32
 //   decode != 0: every work item has 1 <= q_count and G * q_count <= kDecodeRows (position j causally masked at q_pos0 + j)
-//   and the CTA's 4 warps split the KV range.  decode == 0 (the op-level prefill form) needs G == 4.
+//   and the CTA's 4 warps split the KV range.  decode == 0 (the op-level prefill form) needs G == 4 and D == 128.
 int paged_attention(const void* q, int ldq, void* out, int ldo, const void* kv_layer, const int* block_tables,
                     int max_blocks, const AttnWork* work, int num_work, int Hq, int Hkv, float scale,
-                    int decode, cudaStream_t st, float* split_ws = nullptr, int split = 1);
+                    int decode, cudaStream_t st, float* split_ws = nullptr, int split = 1, int head_dim = 128);
 // split-KV decode (few sequences): `split` CTAs per (work item, KV head) each stream a slice of the context and leave an
 // unnormalised partial per query head in split_ws (attn_split_ws_bytes, max_q = the largest q_count of the launch), merged
 // by a second tiny kernel.  attn_decode_split picks `split`.
-size_t attn_split_ws_bytes(int num_work, int Hq, int parts, int max_q = 1);
+size_t attn_split_ws_bytes(int num_work, int Hq, int parts, int max_q = 1, int head_dim = 128);
 int attn_decode_split(int num_work, int Hkv, int max_ctx, int sms);
 
 // Chunked-prefill attention on wgmma (attention_wgmma.cu): work items of up to kPrefillQueryBlock query tokens, one CTA per
 // (work item, query head); q rows are read from the fused qkv buffer [qkv_rows, ldq].
 constexpr int kPrefillQueryBlock = 64;
 int paged_attention_prefill_tc(const void* qkv, int qkv_rows, int ldq, void* out, int ldo, const void* kv_layer, const int* block_tables,
-                               int max_blocks, const AttnWork* work, int num_work, int Hq, int Hkv, float scale, cudaStream_t st);
+                               int max_blocks, const AttnWork* work, int num_work, int Hq, int Hkv, float scale, cudaStream_t st,
+                               int head_dim = 128);
 
 }  // namespace b200

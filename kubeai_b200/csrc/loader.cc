@@ -300,13 +300,45 @@ int b200_config_from_hf(const char* dir, b200_config* cfg) {
     set_error("shape not supported by the kernels (hidden %% 256 == 0 and <= 8192, vocab %% 8 == 0, intermediate %% 64 == 0)");
     return B200_ERR_INVALID;
   }
+  // HF Llama takes an explicit head_dim (Llama-3.2-1B: 64 with hidden 2048 and 32 heads); hidden / q_heads otherwise
   const int head_dim = static_cast<int>(num("head_dim", cfg->q_heads ? cfg->hidden / cfg->q_heads : 0));
-  if (head_dim != 128) { set_error("head_dim %d is not supported (kernels are specialised for 128)", head_dim); return B200_ERR_INVALID; }
+  if (head_dim != 64 && head_dim != 128) {
+    set_error("head_dim %d is not supported (the kernels serve 64 and 128)", head_dim);
+    return B200_ERR_INVALID;
+  }
   if (cfg->kv_heads < 1 || cfg->q_heads % cfg->kv_heads || cfg->q_heads / cfg->kv_heads > 16) {
     set_error("GQA ratio %d:%d is not supported (kv_heads must divide q_heads, with 1 to 16 query heads per KV head)",
               cfg->q_heads, cfg->kv_heads);
     return B200_ERR_INVALID;
   }
+  if ((cfg->q_heads * head_dim) % 128) {
+    set_error("head_dim %d with %d query heads is not supported (q_heads * head_dim must be a multiple of 128: head_dim 64 "
+              "needs an even q_heads)", head_dim, cfg->q_heads);
+    return B200_ERR_INVALID;
+  }
+  // The head size is not a free parameter of the weights: the first layer's q / k projections have q_heads * head_dim and
+  // kv_heads * head_dim rows.  A config.json that contradicts the checkpoint beside it (an edited head_dim, or a config
+  // written for other weights) is refused here, before an engine of the wrong shape is built.  A directory without
+  // safetensors (config only) is not checked.
+  {
+    Checkpoint ck;
+    std::string err;
+    if (ck.open_path(dir, &err)) {
+      auto rows = [&](const char* name) -> int64_t {
+        auto it = ck.index.find(name);
+        return it == ck.index.end() || it->second.second->shape.size() != 2 ? -1 : it->second.second->shape[0];
+      };
+      const int64_t qr = rows("model.layers.0.self_attn.q_proj.weight"), kr = rows("model.layers.0.self_attn.k_proj.weight");
+      if ((qr >= 0 && qr != static_cast<int64_t>(cfg->q_heads) * head_dim) ||
+          (kr >= 0 && kr != static_cast<int64_t>(cfg->kv_heads) * head_dim)) {
+        set_error("head_dim %d does not match the checkpoint: layer 0 has q_proj / k_proj of %lld / %lld rows, not "
+                  "q_heads * head_dim = %d / kv_heads * head_dim = %d", head_dim, static_cast<long long>(qr),
+                  static_cast<long long>(kr), cfg->q_heads * head_dim, cfg->kv_heads * head_dim);
+        return B200_ERR_INVALID;
+      }
+    }
+  }
+  cfg->head_dim = head_dim;
   if (const JVal* e = root.get("eos_token_id"); e && e->type == JVal::Num) cfg->eos_token_id = static_cast<int>(e->num);
   return 0;
 }

@@ -49,16 +49,17 @@ EPI_PLAIN, EPI_RESADD, EPI_SILU, EPI_ROPE_KV, EPI_ARGMAX = 0, 1, 2, 3, 4
 
 def gemm3(x, w, T=None, pro=PRO_NONE, epi=EPI_PLAIN, force=0, ssq_in=None, norm_w=None, eps=1e-5, out=None, ssq_out=None,
           positions=None, slots=None, cos_sin=None, kv_layer=None, q_heads=0, kv_heads=0, argmax_out=None, n_valid=0,
-          normed_out=None, norm_w_out=None):
+          normed_out=None, norm_w_out=None, head_dim=0):
     """The fused projection GEMM (b200_op_gemm3).  x: [rows >= T, K] activations (or the residual for PRO_NORM),
     w: [N, K].  Returns (out, schedule) with schedule = (K-splits per tile, rule that chose them: 0 given by `force`,
-    1 device-filling for one token tile, 2 device-filling over several token tiles (T > 128), CTAs)."""
+    1 device-filling for one token tile, 2 device-filling over several token tiles (T > 128), CTAs).  head_dim (EPI_ROPE_KV):
+    64 or 128, 0 = 128."""
     from ._lib import Gemm3Args
     _chk(x), _chk(w)
     T = x.shape[0] if T is None else T
     N, K = w.shape
     a = Gemm3Args(N=N, T=T, K=K, x_rows=x.shape[0], pro=pro, epi=epi, force=force, w=w.data_ptr(), x=x.data_ptr(), eps=eps,
-                  q_heads=q_heads, kv_heads=kv_heads, n_valid=n_valid)
+                  q_heads=q_heads, kv_heads=kv_heads, n_valid=n_valid, head_dim=head_dim)
     if pro == PRO_NORM:
         _chk(norm_w), _chk(ssq_in, torch.float32)
         a.ssq_in, a.ssq_slabs, a.norm_w = ssq_in.data_ptr(), ssq_in.shape[1], norm_w.data_ptr()
@@ -106,10 +107,14 @@ def rmsnorm(x, w, eps, residual=None, row_index=None):
     return out
 
 
-def rope_kvwrite(qkv, positions, slots, cos_sin, kv_layer, q_heads, kv_heads):
+def rope_kvwrite(qkv, positions, slots, cos_sin, kv_layer, q_heads, kv_heads, head_dim=None):
+    """head_dim None: b200_op_rope_kvwrite (D = 128); 64 or 128: b200_op_rope_kvwrite_hd."""
     _chk(qkv), _chk(positions, torch.int32), _chk(slots, torch.int32), _chk(cos_sin), _chk(kv_layer)
-    check(lib().b200_op_rope_kvwrite(_p(qkv), _p(positions), _p(slots), _p(cos_sin), _p(kv_layer), qkv.shape[0],
-                                     q_heads, kv_heads, cos_sin.shape[0], _stream()))
+    args = (_p(qkv), _p(positions), _p(slots), _p(cos_sin), _p(kv_layer), qkv.shape[0], q_heads, kv_heads, cos_sin.shape[0])
+    if head_dim is None:
+        check(lib().b200_op_rope_kvwrite(*args, _stream()))
+    else:
+        check(lib().b200_op_rope_kvwrite_hd(*args, head_dim, _stream()))
 
 
 def silu_mul(gu):
@@ -213,33 +218,41 @@ def logprobs_rank(logits, tokens, top_n):
     return lp, rank, top_ids, top_lp
 
 
-def paged_attn(qkv, kv_layer, block_tables, work, q_heads, kv_heads, decode: bool, out=None, split: int = 0):
-    """qkv: [T, (Hq+2Hkv)*128] (q read from it), work: int32 [n, 4] = (q_tok0, q_count, q_pos0, seq).
-    split >= 1 (decode only): split-KV form with that many CTAs per (work item, KV head)."""
+def paged_attn(qkv, kv_layer, block_tables, work, q_heads, kv_heads, decode: bool, out=None, split: int = 0, head_dim=None):
+    """qkv: [T, (Hq+2Hkv)*D] (q read from it), work: int32 [n, 4] = (q_tok0, q_count, q_pos0, seq).
+    split >= 1 (decode only): split-KV form with that many CTAs per (work item, KV head).
+    head_dim None: the entry points without _hd (D = 128); 64 or 128: their _hd siblings."""
     _chk(qkv), _chk(kv_layer), _chk(block_tables, torch.int32), _chk(work, torch.int32)
     T = qkv.shape[0]
+    D = 128 if head_dim is None else head_dim
     if out is None:
-        out = torch.zeros(T, q_heads * 128, dtype=torch.bfloat16, device=qkv.device)
+        out = torch.zeros(T, q_heads * D, dtype=torch.bfloat16, device=qkv.device)
+    args = (_p(qkv), qkv.shape[1], _p(out), out.shape[1], _p(kv_layer), _p(block_tables), block_tables.shape[1], _p(work),
+            work.shape[0], q_heads, kv_heads, D ** -0.5)
+    hd = () if head_dim is None else (head_dim,)
     if split:
         assert decode
-        check(lib().b200_op_paged_attn_decode_split(_p(qkv), qkv.shape[1], _p(out), out.shape[1], _p(kv_layer), _p(block_tables),
-                                                    block_tables.shape[1], _p(work), work.shape[0], q_heads, kv_heads,
-                                                    128 ** -0.5, split, _stream()))
+        fn = lib().b200_op_paged_attn_decode_split if head_dim is None else lib().b200_op_paged_attn_decode_split_hd
+        check(fn(*args, split, *hd, _stream()))
         return out
-    check(lib().b200_op_paged_attn(_p(qkv), qkv.shape[1], _p(out), out.shape[1], _p(kv_layer), _p(block_tables),
-                                   block_tables.shape[1], _p(work), work.shape[0], q_heads, kv_heads,
-                                   128 ** -0.5, 1 if decode else 0, _stream()))
+    fn = lib().b200_op_paged_attn if head_dim is None else lib().b200_op_paged_attn_hd
+    check(fn(*args, 1 if decode else 0, *hd, _stream()))
     return out
 
 
-def paged_attn_prefill_tc(qkv, kv_layer, block_tables, work, q_heads, kv_heads, out=None):
-    """wgmma chunked-prefill attention; work: int32 [n, 4] = (q_tok0, q_count <= 64, q_pos0, seq)."""
+def paged_attn_prefill_tc(qkv, kv_layer, block_tables, work, q_heads, kv_heads, out=None, head_dim=None):
+    """wgmma chunked-prefill attention; work: int32 [n, 4] = (q_tok0, q_count <= 64, q_pos0, seq).  head_dim as paged_attn."""
     _chk(qkv), _chk(kv_layer), _chk(block_tables, torch.int32), _chk(work, torch.int32)
     T = qkv.shape[0]
+    D = 128 if head_dim is None else head_dim
     if out is None:
-        out = torch.zeros(T, q_heads * 128, dtype=torch.bfloat16, device=qkv.device)
-    check(lib().b200_op_paged_attn_prefill_tc(_p(qkv), T, qkv.shape[1], _p(out), out.shape[1], _p(kv_layer), _p(block_tables),
-                                              block_tables.shape[1], _p(work), work.shape[0], q_heads, kv_heads, 128 ** -0.5, _stream()))
+        out = torch.zeros(T, q_heads * D, dtype=torch.bfloat16, device=qkv.device)
+    args = (_p(qkv), T, qkv.shape[1], _p(out), out.shape[1], _p(kv_layer), _p(block_tables), block_tables.shape[1], _p(work),
+            work.shape[0], q_heads, kv_heads, D ** -0.5)
+    if head_dim is None:
+        check(lib().b200_op_paged_attn_prefill_tc(*args, _stream()))
+    else:
+        check(lib().b200_op_paged_attn_prefill_tc_hd(*args, head_dim, _stream()))
     return out
 
 
