@@ -6,6 +6,7 @@
 //
 //   b200serve --gpus 8 --model llama-3-8b [--model-dir /models/llama-3-8b] [--strategy PrefixHash] [--port 8000]
 //             [--speculative-config '{"method": "ngram", "num_speculative_tokens": 3, "prompt_lookup_max": 4}']
+//             [--runner generate|pooling]   (default: pooling for a LlamaModel / MistralModel directory, else generate)
 #include <signal.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -27,6 +28,7 @@ int main(int argc, char** argv) {
   unsigned long long seed = 0;
   bool greedy_only = false;
   std::string spec_json;   // vLLM's --speculative-config; speculation stays off without it
+  std::string runner;      // vLLM's --runner: generate | pooling; default from the checkpoint's architecture
   for (int i = 1; i < argc; ++i) {
     std::string a = argv[i];
     auto next = [&]() -> const char* { return i + 1 < argc ? argv[++i] : ""; };
@@ -45,6 +47,7 @@ int main(int argc, char** argv) {
     else if (a == "--seed") seed = strtoull(next(), nullptr, 10);
     else if (a == "--greedy-only") greedy_only = true;   // refuse temperature >= 1e-5 with a 400
     else if (a == "--speculative-config") spec_json = next();
+    else if (a == "--runner") runner = next();
     else { fprintf(stderr, "unknown flag %s\n", a.c_str()); return 2; }
   }
   b200_config cfg;
@@ -55,6 +58,9 @@ int main(int argc, char** argv) {
   cfg.max_batched_tokens = budget;
   cfg.kv_fraction = static_cast<float>(kv_fraction);
   cfg.seed = seed;
+  if (runner == "generate") cfg.runner = B200_RUNNER_GENERATE;
+  else if (runner == "pooling") cfg.runner = B200_RUNNER_POOLING;
+  else if (!runner.empty()) { fprintf(stderr, "--runner must be generate or pooling, got %s\n", runner.c_str()); return 2; }
   if (!spec_json.empty() && b200_speculative_config_parse(spec_json.c_str(), &cfg)) { fprintf(stderr, "%s\n", b200_last_error()); return 2; }
   std::vector<b200_engine*> engines;
   for (int g = 0; g < gpus; ++g) {
@@ -82,12 +88,19 @@ int main(int argc, char** argv) {
   if (b200_server_create(&sc, engines.data(), gpus, &srv)) { fprintf(stderr, "server: %s\n", b200_last_error()); return 1; }
   // the checkpoint's tokenizer + Llama-3 chat template when there is one; the synthetic tokenizer otherwise
   b200_tokenizer* tokenizer = nullptr;
+  const bool explicit_tokenizer = !tokenizer_path.empty();
   if (tokenizer_path.empty() && !model_dir.empty()) {
     const std::string cand = model_dir + "/tokenizer.json";
     if (FILE* f = fopen(cand.c_str(), "rb")) { fclose(f); tokenizer_path = cand; }
   }
+  if (!tokenizer_path.empty() && cfg.runner == B200_RUNNER_POOLING && !explicit_tokenizer &&
+      b200_tokenizer_load(tokenizer_path.c_str(), &tokenizer)) {
+    // an embedding checkpoint whose tokenizer is not of the Llama-3 pipeline is served through token-id inputs
+    fprintf(stderr, "[b200serve] %s not loaded (%s): token-id inputs only\n", tokenizer_path.c_str(), b200_last_error());
+    tokenizer_path.clear();
+  }
   if (!tokenizer_path.empty()) {
-    if (b200_tokenizer_load(tokenizer_path.c_str(), &tokenizer) || b200_server_set_tokenizer(srv, tokenizer)) { fprintf(stderr, "tokenizer: %s\n", b200_last_error()); return 1; }
+    if ((!tokenizer && b200_tokenizer_load(tokenizer_path.c_str(), &tokenizer)) || b200_server_set_tokenizer(srv, tokenizer)) { fprintf(stderr, "tokenizer: %s\n", b200_last_error()); return 1; }
     fprintf(stderr, "[b200serve] tokenizer %s (%d ids)\n", tokenizer_path.c_str(), b200_tokenizer_vocab_size(tokenizer));
   }
   int bound = 0;

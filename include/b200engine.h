@@ -77,7 +77,17 @@ typedef struct {
    * an even q_heads), otherwise B200_ERR_INVALID at b200_engine_create.  The KV pool holds 2 * kv_heads * 16 * D bf16 per
    * page and layer, so D = 64 fits twice the tokens in the same memory. */
   int32_t head_dim;
+  /* what the engine runs (vLLM's --runner): 0 = generate (b200_submit / b200_submit_n), 1 = pooling (b200_submit_embed: each
+   * request is a prompt whose last position's final-normed hidden state, L2-normalised on request, is its embedding; no
+   * lm_head is allocated or loaded, and num_speculative_tokens must be 0).  b200_config_from_hf sets 1 for a LlamaModel /
+   * MistralModel checkpoint and 0 for a *ForCausalLM one; a caller may set 1 on a ForCausalLM checkpoint. */
+  int32_t runner;
+  /* sliding-window attention span of the checkpoint (Mistral's sliding_window), 0 = none.  The kernels attend to the whole
+   * context, which inside the window is the same attention: b200_engine_create refuses max_model_len > sliding_window. */
+  int32_t sliding_window;
 } b200_config;
+
+enum { B200_RUNNER_GENERATE = 0, B200_RUNNER_POOLING = 1 };
 
 /* drafts per step at most: a verify item's G query heads times its 1 + m positions share decode attention's 16-row tile,
  * so 3 drafts fill it at G = 4 and fewer fit at larger G (k_max(G) above) */
@@ -171,6 +181,16 @@ int b200_submit(b200_engine* e, const int32_t* prompt_ids, int32_t n, const b200
  * "n must be 1 when using greedy sampling").  B200_ERR_INVALID otherwise.  n = 1 is b200_submit. */
 int b200_submit_n(b200_engine* e, const int32_t* prompt_ids, int32_t n_prompt, const b200_sampling* sp, int32_t n,
                   uint64_t* req_ids);
+/* Pooling runner only (b200_submit and b200_submit_n are refused there, and this call by a generate runner, with
+ * B200_ERR_INVALID): one embedding request of 1..max_model_len prompt ids.  It is scheduled, chunked, prefix-cached and
+ * preempted like any prompt, and finishes (B200_FINISH_STOP) at the step that computes its last position.  normalize != 0:
+ * the vector is L2-normalised in fp32 (vLLM's embed default), else it is the fp32 of the bf16 final-normed hidden row.
+ * b200_wait, b200_abort and b200_release work on it as on any request. */
+int b200_submit_embed(b200_engine* e, const int32_t* ids, int32_t n, int32_t normalize, uint64_t* req_id);
+/* The embedding of a b200_submit_embed request: *finished gets a B200_FINISH_* code or 0, and once it is B200_FINISH_STOP
+ * out[0..dim) gets the vector (dim must be the model's hidden size, else B200_ERR_INVALID).  usage: prompt and cached
+ * tokens, completion_tokens 0. */
+int b200_poll_embedding(b200_engine* e, uint64_t req_id, float* out, int32_t dim, int32_t* finished, b200_usage* usage);
 /* Drain newly generated token ids (at most cap).  *finished gets a B200_FINISH_* code or 0. */
 int b200_poll(b200_engine* e, uint64_t req_id, int32_t* out_ids, int32_t cap, int32_t* n_out, int32_t* finished,
               b200_usage* usage);
@@ -488,6 +508,12 @@ int b200_op_gemm3(const b200_gemm3_args* a, void* stream, int32_t* schedule_out)
 int b200_op_embed(const void* table, const int32_t* ids, void* out, int32_t T, int32_t H, int32_t vocab, void* stream);
 int b200_op_rmsnorm(const void* x, void* residual, const void* w, void* out, const int32_t* row_index, int32_t rows,
                     int32_t H, float eps, void* stream);
+/* Last-token pooling's tail, as a pooling engine runs it on its pooled rows: out[s] (fp32 [rows, H], device) = the final
+ * RMSNorm (weight w, eps) of bf16 row row_index[s] of hidden, bit-identical in bf16 to b200_op_rmsnorm over the same rows,
+ * then, when flags[s] != 0, divided by max(sqrt(sum of its squares), 1e-12) in fp32 (F.normalize).  H % 256 == 0 and
+ * H <= 8192; row_index and flags are device int32 [rows]. */
+int b200_op_pool_rows(const void* hidden, const void* w, const int32_t* row_index, const int32_t* flags, int32_t rows,
+                      int32_t H, float eps, float* out, void* stream);
 int b200_op_rope_kvwrite(void* qkv, const int32_t* positions, const int32_t* slots, const void* cos_sin,
                          void* kv_layer, int32_t T, int32_t q_heads, int32_t kv_heads, int32_t max_pos, void* stream);
 /* b200_op_rope_kvwrite at head size head_dim = 64 or 128: qkv rows of (q_heads + 2 * kv_heads) * head_dim, cos_sin rows of

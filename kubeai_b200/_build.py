@@ -25,6 +25,7 @@ SOURCES = [
     "sampling.cu",
     "penalties.cu",
     "kv_fork.cu",
+    "pooling.cu",
     "abi_ops.cu",
     "engine.cu",
     "router.cc",

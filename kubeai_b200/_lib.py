@@ -30,7 +30,7 @@ class Config(C.Structure):
         ("rope_scaling_type", C.c_int32), ("rope_factor", C.c_float), ("rope_low_freq_factor", C.c_float),
         ("rope_high_freq_factor", C.c_float), ("rope_original_max_pos", C.c_int32),
         ("num_speculative_tokens", C.c_int32), ("prompt_lookup_min", C.c_int32), ("prompt_lookup_max", C.c_int32),
-        ("head_dim", C.c_int32),
+        ("head_dim", C.c_int32), ("runner", C.c_int32), ("sliding_window", C.c_int32),
     ]
 
 
@@ -143,6 +143,8 @@ SYMBOLS = {
     "b200_poll": (C.c_int, [_vp, _u64, _pi32, _i32, _pi32, _pi32, C.POINTER(Usage)]),
     "b200_poll_logprobs": (C.c_int, [_vp, _u64, _pi32, _vp, _pi32, _vp, _i32, _pi32, _pi32, C.POINTER(Usage)]),
     "b200_poll_prompt_logprobs": (C.c_int, [_vp, _u64, _vp, _pi32, _pi32, _vp, _i32, _pi32]),
+    "b200_submit_embed": (C.c_int, [_vp, _pi32, _i32, _i32, C.POINTER(_u64)]),
+    "b200_poll_embedding": (C.c_int, [_vp, _u64, _vp, _i32, _pi32, C.POINTER(Usage)]),
     "b200_submit_n": (C.c_int, [_vp, _pi32, _i32, C.POINTER(Sampling), _i32, C.POINTER(_u64)]),
     "b200_wait": (C.c_int, [_vp, _u64, _i64]),
     "b200_wait_any": (C.c_int, [_vp, C.POINTER(_u64), _i32, _i64]),
@@ -206,6 +208,7 @@ SYMBOLS = {
     "b200_op_gemm3": (C.c_int, [C.POINTER(Gemm3Args), _vp, _pi32]),
     "b200_op_embed": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "b200_op_rmsnorm": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _f, _vp]),
+    "b200_op_pool_rows": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _f, _vp, _vp]),
     "b200_op_rope_kvwrite": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
     "b200_op_rope_kvwrite_hd": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
     "b200_op_silu_mul": (C.c_int, [_vp, _vp, _i32, _i32, _vp]),

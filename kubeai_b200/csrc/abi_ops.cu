@@ -222,6 +222,17 @@ int b200_op_rmsnorm(const void* x, void* residual, const void* w, void* out, con
   return rc ? cuda_fail("rmsnorm", rc) : 0;
 }
 
+int b200_op_pool_rows(const void* hidden, const void* w, const int32_t* row_index, const int32_t* flags, int32_t rows,
+                      int32_t H, float eps, float* out, void* stream) {
+  if (int rc = require_device()) return rc;
+  if (rows < 0 || H % 256 || H <= 0 || H > 8192 || (rows > 0 && (!hidden || !w || !row_index || !flags || !out))) {
+    set_error("b200_op_pool_rows: bad arguments (rows %d, H %d: H %% 256 == 0 and <= 8192)", rows, H);
+    return B200_ERR_INVALID;
+  }
+  int rc = pool_rows(hidden, nullptr, w, row_index, flags, rows, H, eps, out, static_cast<cudaStream_t>(stream));
+  return rc ? cuda_fail("pool_rows", rc) : 0;
+}
+
 int b200_op_rope_kvwrite(void* qkv, const int32_t* positions, const int32_t* slots, const void* cos_sin,
                          void* kv_layer, int32_t T, int32_t q_heads, int32_t kv_heads, int32_t max_pos,
                          void* stream) {

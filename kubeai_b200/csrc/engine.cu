@@ -222,6 +222,11 @@ struct Seq {
   std::shared_ptr<WaitGroup> group;
   // speculative decoding (engine thread): the drafts proposed for the step being launched (Sched::n_draft of them)
   std::vector<int32_t> draft;
+  // pooling runner (b200_submit_embed): the request's last position is pooled, L2-normalised when `normalize`; its vector
+  // is written by the engine thread before the finish code is published, and read by API threads once finished
+  bool embed = false;
+  bool normalize = true;
+  std::vector<float> embedding;
   void notify_group() {
     if (!group) return;
     { std::lock_guard<std::mutex> lk(group->m); ++group->gen; }
@@ -279,6 +284,9 @@ struct StepMeta {
   // packed only when n_fork > 0
   int off_fork = -1;
   int n_fork = 0;
+  // pooled rows (pooling runner): E step token indices, then their E normalise flags; packed only when E > 0
+  int off_pool = -1;
+  int E = 0;
   int words = 0;
   int64_t kv_tokens = 0;
   int out_tokens = 0;  // sampled rows that produce a generated token
@@ -388,6 +396,7 @@ struct Engine {
   b200_config cfg;
   int L, H, Hq, Hkv, I, V, QKV;
   int Dh = 128;   // head size: 64 or 128 (b200_config.head_dim)
+  bool pooling = false;   // b200_config.runner == B200_RUNNER_POOLING: no lm_head, pooled rows instead of sampled ones
   // n-gram speculative decoding: drafts per decoding sequence (0 = off) and the lookup n-gram lengths
   int spec_k = 0, spec_min = 0, spec_max = 0;
   int Tcap, Scap, max_blocks_per_seq;
@@ -419,8 +428,9 @@ struct Engine {
   int *lp_ids_dev = nullptr, *plp_ids_dev = nullptr, *plp_rank_dev = nullptr;
   int32_t *sampled_host = nullptr, *lp_ids_host = nullptr, *plp_ids_host = nullptr, *plp_rank_host = nullptr;
   float *lp_host = nullptr, *plp_f_host = nullptr;
+  float *pooled = nullptr, *pooled_host = nullptr;   // per pooled row its fp32 vector [H] (pooling runner)
   template <class F>
-  void for_each_readback(size_t S, size_t n_lp, size_t n_plp, F fn) {
+  void for_each_readback(size_t S, size_t n_lp, size_t n_plp, size_t E, F fn) {
     const size_t rec = (1 + kMaxLogprobs) * sizeof(float), ids = kMaxLogprobs * sizeof(int32_t);
     fn(sampled, sampled_host, S * sizeof(int32_t));
     fn(lp_dev, lp_host, n_lp * rec);
@@ -428,8 +438,9 @@ struct Engine {
     fn(plp_f_dev, plp_f_host, n_plp * rec);
     fn(plp_ids_dev, plp_ids_host, n_plp * ids);
     fn(plp_rank_dev, plp_rank_host, n_plp * sizeof(int32_t));
+    fn(pooled, pooled_host, E * H * sizeof(float));
   }
-  int alloc_readbacks(int S, int n_lp, int n_plp);
+  int alloc_readbacks(int S, int n_lp, int n_plp, int E);
   // record i of the token (prompt = false) or prompt-logprob readbacks
   LogprobRecord read_record(bool prompt, int i) const {
     const float* src = (prompt ? plp_f_host : lp_host) + static_cast<size_t>(i) * (1 + kMaxLogprobs);
@@ -546,6 +557,7 @@ struct Engine {
   std::vector<int> lp_rows_, lp_n_;      // logprobs rows (indices into rows_) and their N
   std::vector<PenaltyRow> pen_;          // rows with logits edits
   std::vector<int> fork_src_, fork_dst_; // the step's fork page copies
+  std::vector<int> pool_rows_, pool_flags_;   // pooled rows: step token index, normalise flag
   std::vector<int32_t> draft_tmp_;
   void add_drafts(std::vector<Sched>& sched, int* budget);
   int admit_edits(Seq& s);
@@ -619,7 +631,7 @@ Engine::~Engine() {
   for (auto p : stage_dev)
     if (p) cudaFree(p);
   if (stage_host) cudaFreeHost(stage_host);
-  for_each_readback(0, 0, 0, [](auto* dev, auto* host, size_t) {
+  for_each_readback(0, 0, 0, 0, [](auto* dev, auto* host, size_t) {
     if (dev) cudaFree(dev);
     if (host) cudaFreeHost(host);
   });
@@ -637,10 +649,10 @@ static uint64_t splitmix64(uint64_t* state) {
   return z ^ (z >> 31);
 }
 
-// the readbacks of up to S sampled, n_lp logprobs and n_plp prompt-logprob rows that are not allocated yet
-int Engine::alloc_readbacks(int S, int n_lp, int n_plp) {
+// the readbacks of up to S sampled, n_lp logprobs, n_plp prompt-logprob and E pooled rows that are not allocated yet
+int Engine::alloc_readbacks(int S, int n_lp, int n_plp, int E) {
   cudaError_t ce = cudaSuccess;
-  for_each_readback(S, n_lp, n_plp, [&](auto*& dev, auto*& host, size_t bytes) {
+  for_each_readback(S, n_lp, n_plp, E, [&](auto*& dev, auto*& host, size_t bytes) {
     if (bytes == 0 || dev || ce != cudaSuccess) return;
     ce = cudaMalloc(&dev, bytes);
     if (ce == cudaSuccess) ce = cudaMallocHost(&host, bytes);
@@ -672,7 +684,8 @@ int Engine::alloc_all() {
     items.push_back({p + "norm2", static_cast<size_t>(H), &layers[l].norm2, 0.1f, 1.0f});
   }
   items.push_back({"final_norm", static_cast<size_t>(H), &final_norm, 0.1f, 1.0f});
-  items.push_back({"lm_head", static_cast<size_t>(V) * H, &lm_head, s_h * (cfg.init_scale > 0 ? cfg.init_scale : 4.0f), 0.f});
+  if (!pooling)   // a pooling engine never runs the lm_head
+    items.push_back({"lm_head", static_cast<size_t>(V) * H, &lm_head, s_h * (cfg.init_scale > 0 ? cfg.init_scale : 4.0f), 0.f});
   size_t total = 0;
   std::vector<size_t> offs;
   for (auto& it : items) {
@@ -748,7 +761,8 @@ int Engine::alloc_all() {
   CK(cudaMemset(attn, 0, static_cast<size_t>(Tcap) * Hq * Dh * 2));
   CK(cudaMemset(act, 0, static_cast<size_t>(Tcap) * I * 2));
   CK(cudaMemset(last_hidden, 0, static_cast<size_t>(Scap) * H * 2));
-  if (int rc = alloc_readbacks(Scap, Scap, 0)) return rc;   // the prompt-logprob records come after the KV pool
+  // the prompt-logprob records come after the KV pool; a pooling step pools at most one row per sequence
+  if (int rc = alloc_readbacks(Scap, Scap, 0, pooling ? cfg.max_num_seqs : 0)) return rc;
   CK(cudaMalloc(&cand, static_cast<size_t>(std::min(Scap, 128)) * ((V + 127) / 128) * sizeof(float2)));
   // outputs of the last step, readable by name (b200_engine_tensor_read): sampled ids int32 [S]; the lm_head's per-slab
   // {best logit, index} candidates float2 [S][ceil(V / 128)] when the step sampled through them, else bf16 logits [S][V]
@@ -787,7 +801,7 @@ int Engine::alloc_all() {
         plan(&layers[l].p_gu, layers[l].wgu, 2 * I, H) || plan(&layers[l].p_down, layers[l].wdown, H, I))
       return cuda_fail("gemm_plan_init", -2);
   }
-  if (plan(&p_lm, lm_head, V, H)) return cuda_fail("gemm_plan_init(lm_head)", -2);
+  if (!pooling && plan(&p_lm, lm_head, V, H)) return cuda_fail("gemm_plan_init(lm_head)", -2);
   const int bns[kGemmNumBlockN] = {64, 128, 256};
   for (int i = 0; i < kGemmNumBlockN; ++i) {
     if (gemm_make_x_map(&xm_normed.m[i], normed, Tcap, H, H, bns[i]) ||
@@ -846,7 +860,7 @@ int Engine::alloc_all() {
   CK(cudaMalloc(&prompt_hidden, static_cast<size_t>(plp_G) * H * 2));
   CK(cudaMalloc(&prompt_logits, static_cast<size_t>(plp_G) * V * 2));
   CK(cudaMemset(prompt_hidden, 0, static_cast<size_t>(plp_G) * H * 2));
-  if (int rc = alloc_readbacks(Scap, Scap, Tcap)) return rc;
+  if (int rc = alloc_readbacks(Scap, Scap, Tcap, pooling ? cfg.max_num_seqs : 0)) return rc;
   // bf16 logits [plp_G, V] of the last group of prompt-logprob rows of the last step
   tensors["step.prompt_logits"] = {prompt_logits, static_cast<size_t>(plp_G) * V * 2};
   for (int i = 0; i < kGemmNumBlockN; ++i)
@@ -868,6 +882,7 @@ int Engine::init(const b200_config& c) {
   cfg = c;
   L = c.num_layers; H = c.hidden; Hq = c.q_heads; Hkv = c.kv_heads; I = c.intermediate; V = c.vocab;
   if (int rc = head_dim_resolve(c, &Dh)) return rc;
+  pooling = c.runner == B200_RUNNER_POOLING;
   QKV = (Hq + 2 * Hkv) * Dh;
   // the constraints of every kernel the forward launches, checked here so that a bad shape fails at create time with a
   // message instead of poisoning the replica at its first step: RMSNorm rows are 256-element multiples up to 8192,
@@ -1031,6 +1046,16 @@ int Engine::forward(const StepMeta& m, int32_t* dbuf, bool all_logits, bf16* log
       Q();
       launched(1);
     }
+  }
+  // pooled rows: the gathered final norm and the L2 normalisation in one launch, into the pooled readback.  Only scratch
+  // is written, so a replay changes nothing a later step reads.
+  if (!all_logits && m.E > 0) {
+    const int* prow = dbuf + m.off_pool;
+    P(B200_K_NORM);
+    if (!x_pending) rc |= pool_rows(res, nullptr, final_norm, prow, prow + m.E, m.E, H, cfg.rms_eps, pooled, stream);
+    else rc |= pool_rows(x, res, final_norm, prow, prow + m.E, m.E, H, cfg.rms_eps, pooled, stream);
+    Q();
+    launched(1);
   }
   // prompt-logprob rows, plp_G at a time: gathered final norm (the residual is not written back, so the rows can be read
   // again), plain lm_head into the scratch, then the ranked log-softmax into the step's records.  Only scratch is
@@ -1372,6 +1397,8 @@ int Engine::pack(const std::vector<Sched>& sched, StepMeta* mp) {
   plp_n_.clear();
   fork_src_.clear();
   fork_dst_.clear();
+  pool_rows_.clear();
+  pool_flags_.clear();
   int32_t* h = stage_host;
   m.off_ids = 0; m.off_pos = m.T; m.off_slots = 2 * m.T;
   int tok = 0;
@@ -1403,7 +1430,11 @@ int Engine::pack(const std::vector<Sched>& sched, StepMeta* mp) {
       ++m.npre_seq;
     }
     m.kv_tokens += p0 + n;  // unique K/V tokens this sequence streams from HBM (query tiles re-read them from L2)
-    if (p0 + n - nd == static_cast<int>(s.toks.size())) {
+    if (s.embed && p0 + n == static_cast<int>(s.toks.size())) {
+      // the chunk that completes an embedding request's prompt: its last position is pooled
+      pool_rows_.push_back(tok + n - 1);
+      pool_flags_.push_back(s.normalize ? 1 : 0);
+    } else if (p0 + n - nd == static_cast<int>(s.toks.size())) {
       // row j (0..nd) of a verify is drawn as the token with index n_generated + j: accepting draft j exactly when it
       // equals row j's token gives the stream the non-speculative steps would
       for (int j = 0; j <= nd; ++j) add_row(s, tok + n - 1 - nd + j, s.n_generated + j);
@@ -1433,6 +1464,7 @@ int Engine::pack(const std::vector<Sched>& sched, StepMeta* mp) {
   m.n_lp = static_cast<int>(lp_rows_.size());
   m.n_plp = static_cast<int>(plp_tok_.size());
   m.n_fork = static_cast<int>(fork_src_.size());
+  m.E = static_cast<int>(pool_rows_.size());
   bool any_sampled = false, any_minp = false;   // (submit zeroes min_p for greedy requests)
   for (auto& r : samp_) {
     any_sampled |= r.temperature >= 1e-5f;
@@ -1477,6 +1509,10 @@ int Engine::pack(const std::vector<Sched>& sched, StepMeta* mp) {
     m.off_fork = put(fork_src_);
     put(fork_dst_);
   }
+  if (m.E > 0) {
+    m.off_pool = put(pool_rows_);
+    put(pool_flags_);
+  }
   m.words = w;
   if (w > step_words_cap) {
     set_error("step staging overflow (%d > %d words)", w, step_words_cap);
@@ -1500,7 +1536,8 @@ int Engine::step_words_bound() const {
          + seqs * max_blocks_per_seq              // block tables
          + 7 * Scap + 8 * Scap + 2 * Scap         // SampleRows, PenaltyRows, logprobs rows (row, N): at most one each per row
          + 3 * Tcap                               // prompt-logprob rows (token, target, N): at most one per token
-         + 2 * seqs;                              // fork page copies (source, destination): at most one per member
+         + 2 * seqs                               // fork page copies (source, destination): at most one per member
+         + (pooling ? 2 * seqs : 0);              // pooled rows (token, flag): at most one per sequence
 }
 
 // launch(): schedule, pack, then enqueue the H2D copy of the step's inputs, the kernels and the D2H of its outputs.
@@ -1545,7 +1582,7 @@ int Engine::launch(InFlight* f, StepMeta* mp) {
   if (frc) return frc;
   CK(cudaEventRecord(ev1, stream));
   cudaError_t readback = cudaSuccess;
-  for_each_readback(m.S, m.n_lp, m.n_plp, [&](auto* dev, auto* host, size_t bytes) {
+  for_each_readback(m.S, m.n_lp, m.n_plp, m.E, [&](auto* dev, auto* host, size_t bytes) {
     if (bytes > 0 && readback == cudaSuccess) readback = cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, stream);
   });
   CK(readback);
@@ -1563,7 +1600,7 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
   float ms = 0.f;
   cudaEventElapsedTime(&ms, ev0, ev1);
 
-  int ri = 0, li = 0, pi = 0;
+  int ri = 0, li = 0, pi = 0, ei = 0;
   int64_t gen = 0;
   int step_accepted = 0, step_verifies = 0;
   int64_t step_accepted_pos[B200_MAX_SPEC_TOKENS] = {};
@@ -1588,6 +1625,18 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
     for (int k = 0; k < n_plp; ++k, ++pi) pending_plp.push_back({read_record(true, pi), plp_rank_host[pi]});
     if (!samples) {
       if (n_plp > 0) pending_pub.push_back({sp, 0, false, 0, -1, plp0, n_plp});
+      continue;
+    }
+    if (s.embed) {   // pooled rows come back in step order; the request finishes with its vector
+      const float* v = pooled_host + static_cast<size_t>(ei++) * H;
+      {
+        std::lock_guard<std::mutex> lk(s.m);
+        s.embedding.assign(v, v + H);
+      }
+      pending_pub.push_back({sp, 0, false, B200_FINISH_STOP});
+      release_blocks(s);
+      s.leaving = true;
+      any_done = true;
       continue;
     }
     // the sampled token of `q` (the next row), its finish code and its logprobs record
@@ -1703,7 +1752,7 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
     stats.total_device_us += ms * 1000.0;
     stats.last_step_tokens = m.T;
     stats.h2d_bytes += static_cast<int64_t>(m.words) * 4;
-    for_each_readback(m.S, m.n_lp, m.n_plp, [&](auto*, auto*, size_t bytes) { stats.d2h_bytes += static_cast<int64_t>(bytes); });
+    for_each_readback(m.S, m.n_lp, m.n_plp, m.E, [&](auto*, auto*, size_t bytes) { stats.d2h_bytes += static_cast<int64_t>(bytes); });
     stats.running = static_cast<int>(running.size());
     stats.waiting = static_cast<int>(waiting.size());
     stats.kv_blocks_free = pool.free_count();
@@ -1867,6 +1916,20 @@ int b200_engine_create(const b200_config* cfg, b200_engine** out) {
     if (int rc = spec_resolve(*cfg, &k, &mn, &mx)) return rc;
     if (int rc = head_dim_resolve(*cfg, &d)) return rc;
   }
+  if (cfg->runner != B200_RUNNER_GENERATE && cfg->runner != B200_RUNNER_POOLING) {
+    set_error("runner must be 0 (generate) or 1 (pooling), got %d", cfg->runner);
+    return B200_ERR_INVALID;
+  }
+  if (cfg->runner == B200_RUNNER_POOLING && cfg->num_speculative_tokens > 0) {
+    set_error("speculative decoding (num_speculative_tokens=%d) needs the generate runner", cfg->num_speculative_tokens);
+    return B200_ERR_INVALID;
+  }
+  // sliding-window attention is not implemented: inside the window it is full attention, which the kernels compute exactly
+  if (cfg->sliding_window < 0 || (cfg->sliding_window > 0 && cfg->max_model_len > cfg->sliding_window)) {
+    set_error("max_model_len %d exceeds sliding_window %d: attention beyond the sliding window is not supported (lower "
+              "max_model_len to at most %d)", cfg->max_model_len, cfg->sliding_window, cfg->sliding_window);
+    return B200_ERR_INVALID;
+  }
   if (int rc = require_device()) return rc;
   b200_engine* e = new (std::nothrow) b200_engine();
   if (!e) { set_error("host OOM"); return B200_ERR_OOM; }
@@ -1892,6 +1955,7 @@ static int submit_impl(b200_engine* e, const int32_t* prompt_ids, int32_t n, con
                        uint64_t* req_ids) {
   if (!e || !prompt_ids || n <= 0 || !req_ids) { set_error("b200_submit: bad arguments"); return B200_ERR_INVALID; }
   Engine& g = e->impl;
+  if (g.pooling) { set_error("this engine runs the pooling runner: submit embedding requests with b200_submit_embed"); return B200_ERR_INVALID; }
   // vLLM's SamplingParams._verify_args / _verify_greedy_sampling; every member runs at once, so max_num_seqs bounds n
   if (members < 1) { set_error("n must be at least 1, got %d.", members); return B200_ERR_INVALID; }
   if (members > g.cfg.max_num_seqs) { set_error("n (%d) exceeds max_num_seqs %d", members, g.cfg.max_num_seqs); return B200_ERR_INVALID; }
@@ -1967,6 +2031,56 @@ static int submit_impl(b200_engine* e, const int32_t* prompt_ids, int32_t n, con
     g.incoming.push_back(group[0]);
   }
   g.cv_work_.notify_one();
+  return 0;
+}
+
+int b200_submit_embed(b200_engine* e, const int32_t* ids, int32_t n, int32_t normalize, uint64_t* req_id) {
+  if (!e || !ids || n <= 0 || !req_id) { set_error("b200_submit_embed: bad arguments"); return B200_ERR_INVALID; }
+  Engine& g = e->impl;
+  if (!g.pooling) { set_error("this engine runs the generate runner: embedding requests need an engine created with runner = pooling"); return B200_ERR_INVALID; }
+  if (n > g.cfg.max_model_len) { set_error("prompt (%d tokens) exceeds max_model_len %d", n, g.cfg.max_model_len); return B200_ERR_INVALID; }
+  for (int i = 0; i < n; ++i)
+    if (ids[i] < 0 || ids[i] >= g.V) { set_error("token id %d out of range [0, %d)", ids[i], g.V); return B200_ERR_INVALID; }
+  auto s = std::make_shared<Seq>();
+  s->toks.assign(ids, ids + n);
+  s->n_prompt = n;
+  s->arrival_key = xxh64(ids, static_cast<size_t>(n) * sizeof(int32_t), 0);
+  s->max_tokens = 0;
+  s->embed = true;
+  s->normalize = normalize != 0;
+  {
+    std::lock_guard<std::mutex> lk(g.mu_);
+    if (g.fatal) { set_error("engine is in a failed state"); return B200_ERR_CUDA; }
+    s->id = g.next_id++;
+    g.requests[s->id] = s;
+    *req_id = s->id;
+    g.incoming.push_back(s);
+  }
+  g.cv_work_.notify_one();
+  return 0;
+}
+
+int b200_poll_embedding(b200_engine* e, uint64_t req_id, float* out, int32_t dim, int32_t* finished, b200_usage* usage) {
+  if (!e || !finished) { set_error("b200_poll_embedding: bad arguments"); return B200_ERR_INVALID; }
+  Engine& g = e->impl;
+  std::shared_ptr<Seq> s;
+  {
+    std::lock_guard<std::mutex> lk(g.mu_);
+    auto it = g.requests.find(req_id);
+    if (it != g.requests.end()) s = it->second;
+  }
+  if (!s) { set_error("unknown request %llu", static_cast<unsigned long long>(req_id)); return B200_ERR_NOT_FOUND; }
+  if (!s->embed) { set_error("request %llu is not an embedding request", static_cast<unsigned long long>(req_id)); return B200_ERR_INVALID; }
+  if (dim != g.H || !out) { set_error("b200_poll_embedding: dim %d != hidden size %d", dim, g.H); return B200_ERR_INVALID; }
+  std::lock_guard<std::mutex> lk(s->m);
+  *finished = s->finished;
+  if (s->finished == B200_FINISH_STOP) memcpy(out, s->embedding.data(), static_cast<size_t>(g.H) * sizeof(float));
+  if (usage) {
+    const int nc = s->n_cached.load();
+    usage->prompt_tokens = s->n_prompt;
+    usage->cached_tokens = nc < 0 ? 0 : nc;
+    usage->completion_tokens = 0;
+  }
   return 0;
 }
 
@@ -2346,6 +2460,9 @@ int b200_engine_read_logits(b200_engine* e, void* host_logits_bf16, int32_t rows
 
 }  // extern "C"
 
+int b200::engine_runner(const b200_engine* e) { return e->impl.pooling ? B200_RUNNER_POOLING : B200_RUNNER_GENERATE; }
+int b200::engine_hidden(const b200_engine* e) { return e->impl.H; }
+
 int b200::engine_relayout_gate_up(b200_engine* e, const char* name) {
   uint64_t nb = 0; void* p = nullptr;
   if (int rc = b200_engine_tensor_info(e, name, &nb, &p)) return rc;
@@ -2367,6 +2484,7 @@ int b200_engine_forward_logits(b200_engine* e, const int32_t* ids, int32_t n, vo
   if (!e || !ids || n <= 0 || !host_logits_bf16) { set_error("bad arguments"); return B200_ERR_INVALID; }
   Engine& g = e->impl;
   if (!g.cfg.manual_step) { set_error("forward_logits needs manual_step"); return B200_ERR_INVALID; }
+  if (g.pooling) { set_error("forward_logits needs the lm_head, which a pooling engine does not have"); return B200_ERR_INVALID; }
   if (n > g.Tcap || n > g.cfg.max_model_len) { set_error("too many tokens"); return B200_ERR_INVALID; }
   cudaSetDevice(g.cfg.device);
   // one greedy prompt from position 0, packed as a step and staged in the scratch ring slot: the recorded steps stay

@@ -11,4 +11,7 @@ namespace b200 {
 // The gate_up weight named `name` was just filled in logical order ([gate rows | up rows]) through its device pointer:
 // move it to the engine's physical layout (64-row gate/up blocks interleaved).  Used by the checkpoint loader.
 int engine_relayout_gate_up(b200_engine* e, const char* name);
+// b200_config.runner and hidden size of an engine (the serving shell routes and sizes embeddings by them)
+int engine_runner(const b200_engine* e);
+int engine_hidden(const b200_engine* e);
 }

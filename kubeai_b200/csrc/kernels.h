@@ -20,6 +20,11 @@ int embed_gather(const void* table, const int* ids, void* out, int T, int H, int
 // stream-K partials of the preceding deferred GEMM (summed + rounded to bf16 on load) instead of the bf16 tensor.
 int rmsnorm(const void* x, void* residual, const void* w, void* out, const int* row_index, int rows, int H,
             float eps, cudaStream_t st, PartialView pv = no_partials());
+// Last-token pooling (pooling.cu): out[s] (fp32 [rows, H]) = the final RMSNorm of row row_index[s] of x (+ residual, as
+// rmsnorm with a row_index), bit-identical in bf16 to rmsnorm over the same rows, then L2-normalised in fp32 when
+// flags[s] != 0.  H % 256 == 0 and H <= 8192; row_index and flags are device int arrays [rows].
+int pool_rows(const void* x, const void* residual, const void* w, const int* row_index, const int* flags, int rows, int H,
+              float eps, float* out, cudaStream_t st);
 // head_dim D = 64 or 128: qkv rows [(Hq + 2 Hkv) * D], cos_sin rows [D], kv_layer [block][2][Hkv][16][D]
 int rope_kv_write(void* qkv, const int* positions, const int* slots, const void* cos_sin, void* kv_layer,
                   int T, int Hq, int Hkv, int max_pos, cudaStream_t st, PartialView pv = no_partials(), int head_dim = 128);

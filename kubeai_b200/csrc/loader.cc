@@ -282,10 +282,56 @@ int b200_config_from_hf(const char* dir, b200_config* cfg) {
       return B200_ERR_INVALID;
     }
   }
-  // architecture switches the kernels do not implement are refused, not ignored
-  if (const JVal* mt = root.get("model_type"); mt && mt->type == JVal::Str && mt->str != "llama") {
-    set_error("model_type \"%s\" is not supported (llama)", mt->str.c_str());
+  // architecture switches the kernels do not implement are refused, not ignored.  Mistral is the Llama block with an
+  // optional sliding window, which b200_engine_create bounds max_model_len by.
+  if (const JVal* mt = root.get("model_type"); mt && mt->type == JVal::Str && mt->str != "llama" && mt->str != "mistral") {
+    set_error("model_type \"%s\" is not supported (llama, mistral)", mt->str.c_str());
     return B200_ERR_INVALID;
+  }
+  int sliding_window = 0;
+  if (const JVal* sw = root.get("sliding_window"); sw && sw->type == JVal::Num) {
+    if (!(sw->num >= 1 && sw->num <= 2147483647.0)) {
+      set_error("sliding_window %g is not a positive integer", sw->num);
+      return B200_ERR_INVALID;
+    }
+    sliding_window = static_cast<int>(sw->num);
+  }
+  // the runner (vLLM's --runner auto): a base model (LlamaModel, MistralModel) has no lm_head and serves embeddings
+  int runner = cfg->runner;
+  if (const JVal* ar = root.get("architectures"); ar && ar->type == JVal::Arr && !ar->arr.empty() && ar->arr[0].type == JVal::Str) {
+    const std::string& a = ar->arr[0].str;
+    if (a == "LlamaModel" || a == "MistralModel") runner = B200_RUNNER_POOLING;
+    else if (a.size() > 11 && a.compare(a.size() - 11, 11, "ForCausalLM") == 0) runner = B200_RUNNER_GENERATE;
+  }
+  // the pooling type a sentence-transformers checkpoint declares (modules.json, then <Pooling module>/config.json, as
+  // vLLM's get_pooling_config reads them), checked when the checkpoint pools: none declared = last token, the only mode
+  // the engine serves; any other mode, alone or beside last token, is refused
+  if (runner == B200_RUNNER_POOLING) {
+    std::string mods;
+    JVal mroot;
+    std::string merr;
+    if (read_text(std::string(dir) + "/modules.json", &mods) && JParser(mods.data(), mods.size()).parse(&mroot, &merr) &&
+        mroot.type == JVal::Arr) {
+      for (auto& mod : mroot.arr) {
+        const JVal* ty = mod.get("type");
+        const JVal* path = mod.get("path");
+        if (!ty || ty->type != JVal::Str || ty->str != "sentence_transformers.models.Pooling" || !path || path->type != JVal::Str) continue;
+        std::string ptxt;
+        JVal proot;
+        if (!read_text(std::string(dir) + "/" + path->str + "/config.json", &ptxt) ||
+            !JParser(ptxt.data(), ptxt.size()).parse(&proot, &merr) || proot.type != JVal::Obj)
+          continue;
+        for (auto& kv : proot.obj) {
+          if (kv.first.rfind("pooling_mode_", 0) != 0 || kv.second.type != JVal::Bool || !kv.second.b) continue;
+          const std::string mode = kv.first.substr(13);
+          if (mode != "lasttoken") {
+            set_error("pooling mode \"%s\" (%s/config.json) is not supported: the engine serves last-token pooling only",
+                      mode.c_str(), path->str.c_str());
+            return B200_ERR_INVALID;
+          }
+        }
+      }
+    }
   }
   if (const JVal* ha = root.get("hidden_act"); ha && ha->type == JVal::Str && ha->str != "silu") {
     set_error("hidden_act \"%s\" is not supported (silu)", ha->str.c_str());
@@ -328,7 +374,10 @@ int b200_config_from_hf(const char* dir, b200_config* cfg) {
         auto it = ck.index.find(name);
         return it == ck.index.end() || it->second.second->shape.size() != 2 ? -1 : it->second.second->shape[0];
       };
-      const int64_t qr = rows("model.layers.0.self_attn.q_proj.weight"), kr = rows("model.layers.0.self_attn.k_proj.weight");
+      // HF writes a *ForCausalLM's tensors under "model." and a base model's (LlamaModel, MistralModel) without it
+      const char* pre = ck.index.count("model.layers.0.self_attn.q_proj.weight") ? "model." : "";
+      const int64_t qr = rows((std::string(pre) + "layers.0.self_attn.q_proj.weight").c_str()),
+                    kr = rows((std::string(pre) + "layers.0.self_attn.k_proj.weight").c_str());
       if ((qr >= 0 && qr != static_cast<int64_t>(cfg->q_heads) * head_dim) ||
           (kr >= 0 && kr != static_cast<int64_t>(cfg->kv_heads) * head_dim)) {
         set_error("head_dim %d does not match the checkpoint: layer 0 has q_proj / k_proj of %lld / %lld rows, not "
@@ -339,6 +388,8 @@ int b200_config_from_hf(const char* dir, b200_config* cfg) {
     }
   }
   cfg->head_dim = head_dim;
+  cfg->runner = runner;
+  cfg->sliding_window = sliding_window;
   if (const JVal* e = root.get("eos_token_id"); e && e->type == JVal::Num) cfg->eos_token_id = static_cast<int>(e->num);
   return 0;
 }
@@ -359,17 +410,18 @@ int b200_engine_load_safetensors(b200_engine* e, const char* path) {
   const int64_t V = static_cast<int64_t>(nb / 2) / H;
   int rc;
 #define LD(hfname, row0, rows, cols) if ((rc = copy_rows(ck, hfname, p, nb, row0, rows, cols, &err))) { set_error("%s", err.c_str()); return rc; }
-  LD("model.embed_tokens.weight", 0, V, H);
+  // a *ForCausalLM checkpoint names its tensors "model.<name>", a base model (LlamaModel, MistralModel) "<name>"
+  const std::string pre = ck.index.count("model.embed_tokens.weight") ? "model." : "";
+  LD(pre + "embed_tokens.weight", 0, V, H);
   if (dev("final_norm", &p, &nb)) return B200_ERR_NOT_FOUND;
-  LD("model.norm.weight", 0, 1, H);
-  if (dev("lm_head", &p, &nb)) return B200_ERR_NOT_FOUND;
-  {
+  LD(pre + "norm.weight", 0, 1, H);
+  if (b200_engine_tensor_info(e, "lm_head", &nb, &p) == 0) {   // a pooling engine has no lm_head
     // tie_word_embeddings: checkpoints without lm_head.weight reuse the embedding matrix
-    const std::string head = ck.index.count("lm_head.weight") ? "lm_head.weight" : "model.embed_tokens.weight";
+    const std::string head = ck.index.count("lm_head.weight") ? "lm_head.weight" : pre + "embed_tokens.weight";
     LD(head, 0, V, H);
   }
   for (int l = 0;; ++l) {
-    const std::string ep = "layers." + std::to_string(l) + ".", hp = "model.layers." + std::to_string(l) + ".";
+    const std::string ep = "layers." + std::to_string(l) + ".", hp = pre + "layers." + std::to_string(l) + ".";
     if (dev(ep + "wqkv", &p, &nb)) break;  // no more layers in the engine
     auto qit = ck.index.find(hp + "self_attn.q_proj.weight"), kit = ck.index.find(hp + "self_attn.k_proj.weight");
     if (qit == ck.index.end() || kit == ck.index.end() || qit->second.second->shape.size() != 2) { set_error("missing %sself_attn.{q,k}_proj.weight", hp.c_str()); return B200_ERR_NOT_FOUND; }

@@ -53,6 +53,8 @@ struct Server {
   bool edits = false;      // b200_server_config.enable_logits_processors: serve penalties, min_p, min_tokens, logit_bias
   bool prompt_lp = false;  // b200_server_config.enable_prompt_logprobs: serve prompt_logprobs and completions echo
   int max_n = 0;           // b200_server_config.max_n: >= 2 serves n up to it (else n > 1 is a 400)
+  bool pooling = false;    // the replicas run the pooling runner: /v1/embeddings is served, the generation routes are not
+  int hidden = 0;          // embedding size (pooling)
   // optional real tokenizer (b200_server_set_tokenizer): a checkpoint's tokenizer.json instead of the synthetic byte/word ids
   const b200_tokenizer* real_tok = nullptr;
 
@@ -156,6 +158,7 @@ int send_error(Writer& w, int status, const std::string& msg) {
 
 struct ParsedRequest {
   bool chat = true;
+  bool embed = false;   // /v1/embeddings (the reference's EmbeddingRequest: no Prefix)
   std::string requested_model, model, adapter, prefix;
   std::vector<std::pair<std::string, std::string>> messages;
   std::vector<int32_t> prompt_ids;  // completions with token-id prompt
@@ -204,6 +207,7 @@ int parse_request(Server& sv, const std::string& path, const std::string& ctype,
   }
   if (path == "/v1/chat/completions") pr->chat = true;
   else if (path == "/v1/completions") pr->chat = false;
+  else if (path == "/v1/embeddings") pr->embed = true;
   else {
     *err = "bad request: reading model from body: unknown path: \"" + path + "\"";
     return 400;
@@ -229,6 +233,7 @@ int parse_request(Server& sv, const std::string& path, const std::string& ctype,
     *err = "model not found: \"" + pr->requested_model + "\"";
     return 404;
   }
+  if (pr->embed) return 0;   // its fields are read by serve_embeddings
   if (pr->chat) {
     const JVal* msgs = root.get("messages");
     if (msgs && msgs->type == JVal::Arr) {
@@ -921,6 +926,225 @@ static int serve_inference(Server& sv, const std::string& path, const std::strin
   }
 }
 
+// Standard base64 with padding (RFC 4648 §4), as Python's base64.b64encode gives.
+static std::string base64(const uint8_t* p, size_t n) {
+  static const char* a = "ABCDEFGHIJKLMNOPQRSTUVWXYZabcdefghijklmnopqrstuvwxyz0123456789+/";
+  std::string o;
+  o.reserve((n + 2) / 3 * 4);
+  for (size_t i = 0; i < n; i += 3) {
+    const uint32_t v = (static_cast<uint32_t>(p[i]) << 16) | (i + 1 < n ? static_cast<uint32_t>(p[i + 1]) << 8 : 0) |
+                       (i + 2 < n ? p[i + 2] : 0);
+    o += a[(v >> 18) & 63];
+    o += a[(v >> 12) & 63];
+    o += i + 1 < n ? a[(v >> 6) & 63] : '=';
+    o += i + 2 < n ? a[v & 63] : '=';
+  }
+  return o;
+}
+
+// The embedding inputs and options of a /v1/embeddings body (vLLM 0.22's EmbeddingCompletionRequest).  Returns 0 or 400
+// with *err set.  Every field the engine does not implement is refused, never dropped.
+struct EmbedRequest {
+  std::vector<std::vector<int32_t>> inputs;
+  bool base64 = false;
+  bool normalize = true;
+};
+static int parse_embed_body(const Server& sv, const char* body, size_t len, EmbedRequest* er, std::string* err) {
+  JVal root;
+  std::string jerr;
+  if (!JParser(body, len).parse(&root, &jerr) || root.type != JVal::Obj) { *err = "bad request: expected a JSON object"; return 400; }
+  auto bad = [&](const std::string& m) { *err = "bad request: " + m; return 400; };
+  auto present = [&](const char* k) { const JVal* v = root.get(k); return v && v->type != JVal::Null; };
+  if (present("dimensions"))
+    return bad("Model \"" + sv.model + "\" does not support matryoshka representation, changing output dimensions will lead to poor results.");
+  if (const JVal* v = root.get("embed_dtype"); v && v->type != JVal::Null && !(v->type == JVal::Str && v->str == "float32"))
+    return bad("embed_dtype other than float32 is not supported by this engine");
+  if (const JVal* v = root.get("endianness"); v && v->type != JVal::Null &&
+      !(v->type == JVal::Str && (v->str == "native" || v->str == "little")))
+    return bad("endianness other than native or little is not supported by this engine");
+  if (present("truncate_prompt_tokens")) return bad("truncate_prompt_tokens is not supported by this engine");
+  if (present("messages")) return bad("chat-form embeddings (messages) are not supported by this engine");
+  if (const JVal* v = root.get("encoding_format"); v && v->type != JVal::Null) {
+    if (v->type == JVal::Str && v->str == "base64") er->base64 = true;
+    else if (!(v->type == JVal::Str && v->str == "float")) return bad("encoding_format must be \"float\" or \"base64\"");
+  }
+  if (const JVal* v = root.get("use_activation"); v && v->type != JVal::Null) {
+    if (v->type != JVal::Bool) return bad("use_activation must be a boolean or null");
+    er->normalize = v->b;
+  }
+  bool special = true;
+  if (const JVal* v = root.get("add_special_tokens"); v && v->type != JVal::Null) {
+    if (v->type != JVal::Bool) return bad("add_special_tokens must be a boolean");
+    special = v->b;
+  }
+  auto text_ids = [&](const std::string& s, std::vector<int32_t>* ids) {
+    if (sv.real_tok) {
+      if (special && tokenizer_bos(sv.real_tok) >= 0) ids->push_back(tokenizer_bos(sv.real_tok));
+      std::vector<int32_t> buf(s.size() + 16);
+      int64_t n = b200_tokenizer_encode(sv.real_tok, s.data(), s.size(), 1, buf.data(), buf.size());
+      if (n > static_cast<int64_t>(buf.size())) {
+        buf.resize(static_cast<size_t>(n));
+        n = b200_tokenizer_encode(sv.real_tok, s.data(), s.size(), 1, buf.data(), buf.size());
+      }
+      if (n > 0) ids->insert(ids->end(), buf.begin(), buf.begin() + n);
+    } else {
+      sv.tok.encode(s, ids);
+    }
+  };
+  auto id_list = [&](const JVal& a, std::vector<int32_t>* ids) {
+    for (auto& e : a.arr) {
+      if (e.type != JVal::Num || e.num != std::floor(e.num) || !(e.num >= 0 && e.num < sv.tok.vocab)) return false;
+      ids->push_back(static_cast<int32_t>(e.num));
+    }
+    return true;
+  };
+  const JVal* in = root.get("input");
+  if (!in || in->type == JVal::Null) return bad("input is required");
+  const std::string shape = "input must be a string, a list of strings, a list of token ids or a list of token id lists";
+  if (in->type == JVal::Str) {
+    er->inputs.emplace_back();
+    text_ids(in->str, &er->inputs.back());
+  } else if (in->type == JVal::Arr) {
+    if (in->arr.empty()) return bad("input must not be empty");
+    const JVal::Type t0 = in->arr[0].type;
+    for (auto& e : in->arr)
+      if (e.type != t0) return bad(shape);
+    if (t0 == JVal::Num) {
+      er->inputs.emplace_back();
+      if (!id_list(*in, &er->inputs.back())) return bad("token ids must be integers in [0, " + std::to_string(sv.tok.vocab) + ")");
+    } else if (t0 == JVal::Str) {
+      for (auto& e : in->arr) {
+        er->inputs.emplace_back();
+        text_ids(e.str, &er->inputs.back());
+      }
+    } else if (t0 == JVal::Arr) {
+      for (auto& e : in->arr) {
+        er->inputs.emplace_back();
+        if (!id_list(e, &er->inputs.back())) return bad("token ids must be integers in [0, " + std::to_string(sv.tok.vocab) + ")");
+      }
+    } else {
+      return bad(shape);
+    }
+  } else {
+    return bad(shape);
+  }
+  for (auto& ids : er->inputs) {
+    if (ids.empty()) return bad("input must not be empty");
+    // vLLM 0.22 renderers/params.py _token_len_check, with the 0 output tokens of a pooling request; it says "at least"
+    // when the count is max_model_len + 1, the length its tokenizer truncates a longer text to
+    if (static_cast<int>(ids.size()) > sv.max_model_len) {
+      const std::string n = (static_cast<int>(ids.size()) == sv.max_model_len + 1 ? "at least " : "") + std::to_string(ids.size());
+      return bad("This model's maximum context length is " + std::to_string(sv.max_model_len) +
+                 " tokens. However, you requested 0 output tokens and your prompt contains " + n +
+                 " input tokens, for a total of " + n + " tokens. Please reduce the length of the input prompt or the number "
+                 "of requested output tokens.");
+    }
+  }
+  return 0;
+}
+
+// /v1/embeddings on a pooling server: every input is one engine request, all submitted before any is waited on; the
+// response is vLLM's EmbeddingResponse with data in input order.  Retries follow serve_inference.  The response is one
+// write at the end, and the writer reports a client that went away only when a write fails: as for a non-streaming
+// completion, such a client is noticed at that write (status 499), after its requests finished and were released.
+static int serve_embeddings(Server& sv, const std::string& path, const std::string& ctype, const char* body, size_t len,
+                            Writer& w) {
+  ParsedRequest pr;
+  std::string err;
+  if (int st = parse_request(sv, path, ctype, body, len, &pr, &err)) return send_error(w, st, err);
+  EmbedRequest er;
+  if (int st = parse_embed_body(sv, body, len, &er, &err)) return send_error(w, st, err);
+  {
+    std::lock_guard<std::mutex> lk(sv.mmu);
+    ++sv.active[pr.requested_model];
+  }
+  sv.requests_total.fetch_add(1);
+  struct Dec {
+    Server& s;
+    std::string m;
+    ~Dec() {
+      std::lock_guard<std::mutex> lk(s.mmu);
+      --s.active[m];
+    }
+  } dec{sv, pr.requested_model};
+  const size_t n_in = er.inputs.size();
+  std::vector<uint64_t> tokens_held;
+  auto release_all = [&] {
+    for (auto t : tokens_held) b200_router_done(sv.router, t);
+    tokens_held.clear();
+  };
+  for (int attempt = 0;; ++attempt) {
+    char addr[64];
+    uint64_t ep_token = 0;
+    if (b200_router_pick(sv.router, sv.strategy, pr.adapter.c_str(), "", 0, sv.mean_load_pct, 30ll * 1000 * 1000, addr,
+                         sizeof(addr), &ep_token)) {
+      release_all();
+      sv.errors_total.fetch_add(1);
+      return send_error(w, 504, "request timeout while finding host");
+    }
+    tokens_held.push_back(ep_token);
+    const int replica = atoi(addr + 4);  // "gpu:<i>"
+    b200_engine* eng = sv.replicas[replica];
+    bool failed = false;
+    if (sv.faults[replica]->load() < 0) failed = true;
+    else if (sv.faults[replica]->load() > 0 && sv.faults[replica]->fetch_sub(1) > 0) failed = true;
+    std::vector<uint64_t> rids;
+    for (size_t i = 0; i < n_in && !failed; ++i) {
+      uint64_t rid = 0;
+      if (b200_submit_embed(eng, er.inputs[i].data(), static_cast<int>(er.inputs[i].size()), er.normalize ? 1 : 0, &rid)) failed = true;
+      else rids.push_back(rid);
+    }
+    std::vector<float> vecs(n_in * static_cast<size_t>(sv.hidden));
+    std::vector<b200_usage> usage(n_in);
+    std::vector<int> fin(n_in, 0);
+    for (size_t i = 0; i < rids.size() && !failed;) {
+      if (fin[i]) { ++i; continue; }
+      b200_wait(eng, rids[i], 200000);
+      if (b200_poll_embedding(eng, rids[i], vecs.data() + i * sv.hidden, sv.hidden, &fin[i], &usage[i])) failed = true;
+      else if (fin[i] && fin[i] != B200_FINISH_STOP) failed = true;
+    }
+    for (auto r : rids) b200_release(eng, r);   // releasing an unfinished request (a failed attempt) aborts it
+    if (failed) {
+      if (b200_engine_is_failed(eng) || sv.faults[replica]->load() < 0) sv.drop_replica(replica);
+      if (attempt < sv.max_retries) {
+        sv.retries_total.fetch_add(1);
+        continue;
+      }
+      release_all();
+      sv.errors_total.fetch_add(1);
+      return send_error(w, 502, "proxy: exceeded retries");
+    }
+    release_all();
+    int prompt_tokens = 0;
+    for (auto& u : usage) prompt_tokens += u.prompt_tokens;
+    std::string out = "{\"id\":\"embd-" + hex_id(32) + "\",\"object\":\"list\",\"created\":" +
+                      std::to_string(static_cast<long>(time(nullptr))) + ",\"model\":" + json_str(pr.requested_model) + ",\"data\":[";
+    char num[32];
+    for (size_t i = 0; i < n_in; ++i) {
+      out += (i ? ",{\"index\":" : "{\"index\":") + std::to_string(i) + ",\"object\":\"embedding\",\"embedding\":";
+      const float* v = vecs.data() + i * sv.hidden;
+      if (er.base64) {
+        // the little-endian fp32 bytes (vLLM's float32 embed_dtype at native endianness on x86 / aarch64)
+        out += "\"" + base64(reinterpret_cast<const uint8_t*>(v), static_cast<size_t>(sv.hidden) * sizeof(float)) + "\"";
+      } else {
+        out += "[";
+        for (int k = 0; k < sv.hidden; ++k) {
+          snprintf(num, sizeof(num), "%.9g", static_cast<double>(v[k]));   // 9 significant digits round-trip an fp32
+          out += (k ? "," : "");
+          out += num;
+        }
+        out += "]";
+      }
+      out += "}";
+    }
+    out += "],\"usage\":{\"prompt_tokens\":" + std::to_string(prompt_tokens) + ",\"total_tokens\":" + std::to_string(prompt_tokens) +
+           ",\"completion_tokens\":0,\"prompt_tokens_details\":null}}";
+    w.begin(200, "application/json");
+    w.write(out);
+    return w.gone ? 499 : 200;
+  }
+}
+
 static std::string metrics_text(Server& sv) {
   std::string o;
   o += "# HELP kubeai_inference_requests_active The number of active requests by model\n# TYPE kubeai_inference_requests_active gauge\n";
@@ -993,15 +1217,21 @@ static int handle(Server& sv, const std::string& method, const std::string& full
   path = path.substr(7);  // http.StripPrefix("/openai", ...)
   if (path == "/v1/models" && method == "GET") {
     // openaiserver/models.go:13-77 (static: one model + adapters)
-    std::string o = "{\"object\":\"list\",\"data\":[{\"id\":" + json_str(sv.model) + ",\"object\":\"model\",\"created\":0,\"owned_by\":\"kubeai-b200\",\"features\":[\"TextGeneration\"]}";
+    const std::string feat = sv.pooling ? "TextEmbedding" : "TextGeneration";
+    std::string o = "{\"object\":\"list\",\"data\":[{\"id\":" + json_str(sv.model) + ",\"object\":\"model\",\"created\":0,\"owned_by\":\"kubeai-b200\",\"features\":[\"" + feat + "\"]}";
     for (auto& a : sv.adapters)
-      o += ",{\"id\":" + json_str(sv.model + "_" + a) + ",\"object\":\"model\",\"created\":0,\"owned_by\":\"kubeai-b200\",\"features\":[\"TextGeneration\"]}";
+      o += ",{\"id\":" + json_str(sv.model + "_" + a) + ",\"object\":\"model\",\"created\":0,\"owned_by\":\"kubeai-b200\",\"features\":[\"" + feat + "\"]}";
     o += "]}";
     w.begin(200, "application/json");
     w.write(o);
     return 200;
   }
   // "X-Proxy: lingo" (handler.go:60) is added by the HTTP layer below / by the Go shim
+  if (sv.pooling) {
+    if (path == "/v1/embeddings") return serve_embeddings(sv, path, ctype, body, len, w);
+    if (path == "/v1/chat/completions" || path == "/v1/completions" || path == "/v1/rerank" || path == "/v1/audio/transcriptions")
+      return send_error(w, 404, "model not found: this engine serves TextEmbedding only");
+  }
   if (path == "/v1/chat/completions" || path == "/v1/completions") return serve_inference(sv, path, ctype, body, len, w);
   if (path == "/v1/embeddings" || path == "/v1/rerank" || path == "/v1/audio/transcriptions")
     return send_error(w, 404, "model not found: this engine serves TextGeneration only");
@@ -1167,6 +1397,18 @@ int b200_server_create(const b200_server_config* cfg, b200_engine* const* replic
   sv.edits = cfg->enable_logits_processors != 0;
   sv.prompt_lp = cfg->enable_prompt_logprobs != 0;
   sv.max_n = cfg->max_n;
+  // the replicas share one runner: a server serves generation or embeddings, never both
+  for (int i = 0, seen = 0; i < n; ++i) {
+    if (!replicas[i]) continue;
+    const bool pool = engine_runner(replicas[i]) == B200_RUNNER_POOLING;
+    if (seen++ && pool != sv.pooling) {
+      delete s;
+      set_error("b200_server_create: the replicas mix the generate and pooling runners");
+      return B200_ERR_INVALID;
+    }
+    sv.pooling = pool;
+    sv.hidden = engine_hidden(replicas[i]);
+  }
   if (b200_router_create(sv.replication, &sv.router)) { delete s; return B200_ERR_INVALID; }
   std::vector<std::string> names;
   std::string ad = cfg->adapters ? cfg->adapters : "";

@@ -130,6 +130,42 @@ class Engine:
         check(self._l.b200_submit_n(self._h, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), C.byref(sp), n, rids))
         return list(rids[:n])
 
+    def submit_embed(self, prompt_ids, normalize: bool = True) -> int:
+        """One embedding request (pooling runner, b200_submit_embed): the last prompt position's final-normed hidden state,
+        L2-normalised in fp32 when normalize."""
+        ids = np.ascontiguousarray(prompt_ids, dtype=np.int32)
+        rid = C.c_uint64()
+        check(self._l.b200_submit_embed(self._h, ids.ctypes.data_as(_PI32), len(ids), 1 if normalize else 0, C.byref(rid)))
+        return rid.value
+
+    def poll_embedding(self, rid: int):
+        """(vector float32 [hidden] or None until finished, finish reason, usage) of an embedding request."""
+        out = np.zeros(self.cfg.hidden, dtype=np.float32)
+        fin, u = C.c_int32(), Usage()
+        check(self._l.b200_poll_embedding(self._h, rid, out.ctypes.data_as(C.c_void_p), self.cfg.hidden, C.byref(fin),
+                                          C.byref(u)))
+        return (out if fin.value == 1 else None), FINISH[fin.value], (u.prompt_tokens, u.cached_tokens, u.completion_tokens)
+
+    def embed(self, prompts, normalize: bool = True, max_steps: int = 100000):
+        """Manual-step helper: submit every prompt, step until all are finished, return float32 [len(prompts), hidden]."""
+        rids = [self.submit_embed(p, normalize) for p in prompts]
+        vecs = [None] * len(rids)
+        for _ in range(max_steps):
+            ran, _info = self.step()
+            for i, r in enumerate(rids):
+                if vecs[i] is None:
+                    v, fin, _u = self.poll_embedding(r)
+                    if fin is not None and v is None:
+                        raise RuntimeError(f"embedding request finished with {fin}")
+                    vecs[i] = v
+            if all(v is not None for v in vecs):
+                break
+            if not ran:
+                raise RuntimeError("engine idle with unfinished requests")
+        for r in rids:
+            self.release(r)
+        return np.stack(vecs)
+
     def wait_any(self, rids, timeout_s: float = -1.0) -> bool:
         """Block until any of rids (one submit_n group, or a single id) has undrained tokens or is finished."""
         arr = (C.c_uint64 * len(rids))(*rids)

@@ -81,6 +81,29 @@ func (e *Engine) Poll(id uint64, buf []int32) (n int, finished int, u C.b200_usa
 	return int(cn), int(fin), u, nil
 }
 
+// Embedding API (an engine created with runner = 1, pooling): one request per input; Embedding blocks at most 200 ms and
+// returns the vector (len = the model's hidden size) once finished is B200_FINISH_STOP.
+func (e *Engine) SubmitEmbed(ids []int32, normalize bool) (uint64, error) {
+	var id C.uint64_t
+	norm := C.int32_t(0)
+	if normalize {
+		norm = 1
+	}
+	if rc := C.b200_submit_embed(e.h, (*C.int32_t)(unsafe.Pointer(&ids[0])), C.int32_t(len(ids)), norm, &id); rc != 0 {
+		return 0, errors.New(C.GoString(C.b200_last_error()))
+	}
+	return uint64(id), nil
+}
+
+func (e *Engine) Embedding(id uint64, vec []float32) (finished int, u C.b200_usage, err error) {
+	var fin C.int32_t
+	C.b200_wait(e.h, C.uint64_t(id), 200000)
+	if rc := C.b200_poll_embedding(e.h, C.uint64_t(id), (*C.float)(unsafe.Pointer(&vec[0])), C.int32_t(len(vec)), &fin, &u); rc != 0 {
+		return 0, u, errors.New(C.GoString(C.b200_last_error()))
+	}
+	return int(fin), u, nil
+}
+
 // SubmitN starts n parallel samples of one prompt (vLLM's n): one prefill, n request ids for Poll / Abort.
 func (e *Engine) SubmitN(prompt []int32, sp *C.b200_sampling, n int) ([]uint64, error) {
 	ids := make([]C.uint64_t, n)
