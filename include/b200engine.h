@@ -567,15 +567,14 @@ typedef struct {
 } b200_penalty_row;
 int b200_op_penalize(void* logits, int32_t ld, int32_t S, int32_t V, const b200_penalty_row* rows, void* edited, void* stream);
 /* work: int32[num_work][4] = {q_tok0, q_count, q_pos0, seq}; kv_layer: [block][2][kv_heads][16][128]; kv_heads divides
- * q_heads and G = q_heads / kv_heads is 1..16.  decode = 1: every item has 1 <= q_count <= 16 / G consecutive query
+ * q_heads and G = q_heads / kv_heads is 1..16.  Decode attention: every item has 1 <= q_count <= 16 / G consecutive query
  * positions (a speculative verify), position j masked causally at q_pos0 + j, and the item's K/V read once for all of
- * them; decode = 0: q_count <= 16 and G = 4 only (B200_ERR_INVALID otherwise). */
+ * them.  decode = 0 returns B200_ERR_INVALID: chunked prefill is b200_op_paged_attn_prefill_tc[_hd]. */
 int b200_op_paged_attn(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                        const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
                        int32_t q_heads, int32_t kv_heads, float scale, int32_t decode, void* stream);
 /* The attention entry points at head size head_dim = 64 or 128: q / out rows of head_dim per head, kv_layer
- * [block][2][kv_heads][16][head_dim].  Each function without _hd is its _hd sibling at 128.  The prefill form of
- * b200_op_paged_attn_hd (decode = 0) serves head_dim 128 only. */
+ * [block][2][kv_heads][16][head_dim].  Each function without _hd is its _hd sibling at 128. */
 int b200_op_paged_attn_hd(const void* q, int32_t ldq, void* out, int32_t ldo, const void* kv_layer,
                           const int32_t* block_tables, int32_t max_blocks, const int32_t* work, int32_t num_work,
                           int32_t q_heads, int32_t kv_heads, float scale, int32_t decode, int32_t head_dim, void* stream);

@@ -248,7 +248,7 @@ int b200_op_rope_kvwrite_hd(void* qkv, const int32_t* positions, const int32_t* 
     return B200_ERR_INVALID;
   }
   int rc = rope_kv_write(qkv, positions, slots, cos_sin, kv_layer, T, q_heads, kv_heads, max_pos,
-                         static_cast<cudaStream_t>(stream), no_partials(), head_dim);
+                         static_cast<cudaStream_t>(stream), head_dim);
   return rc ? cuda_fail("rope_kv_write", rc) : 0;
 }
 
@@ -375,13 +375,12 @@ int b200_op_paged_attn_hd(const void* q, int32_t ldq, void* out, int32_t ldo, co
                           int32_t q_heads, int32_t kv_heads, float scale, int32_t decode, int32_t head_dim, void* stream) {
   if (int rc = require_device()) return rc;
   static_assert(sizeof(AttnWork) == 16, "AttnWork is int32[4] on the wire");
-  if (!attn_head_dim_ok(head_dim)) {
-    set_error("b200_op_paged_attn: head_dim=%d; 64 and 128 are served", head_dim);
+  if (!decode) {
+    set_error("b200_op_paged_attn: decode = 0 is not served; chunked prefill is b200_op_paged_attn_prefill_tc[_hd]");
     return B200_ERR_INVALID;
   }
-  if (!decode && head_dim != 128) {
-    set_error("b200_op_paged_attn: the prefill form (decode = 0) serves head_dim 128 only, got %d; "
-              "chunked prefill of any head size is b200_op_paged_attn_prefill_tc_hd", head_dim);
+  if (!attn_head_dim_ok(head_dim)) {
+    set_error("b200_op_paged_attn: head_dim=%d; 64 and 128 are served", head_dim);
     return B200_ERR_INVALID;
   }
   if (!attn_group_ok(q_heads, kv_heads)) {
@@ -389,13 +388,8 @@ int b200_op_paged_attn_hd(const void* q, int32_t ldq, void* out, int32_t ldo, co
               q_heads, kv_heads);
     return B200_ERR_INVALID;
   }
-  if (!decode && q_heads != 4 * kv_heads) {
-    set_error("b200_op_paged_attn: the prefill form (decode = 0) serves 4 query heads per KV head only, got %d:%d; "
-              "chunked prefill of any group size is b200_op_paged_attn_prefill_tc", q_heads, kv_heads);
-    return B200_ERR_INVALID;
-  }
   int rc = paged_attention(q, ldq, out, ldo, kv_layer, block_tables, max_blocks,
-                           reinterpret_cast<const AttnWork*>(work), num_work, q_heads, kv_heads, scale, decode,
+                           reinterpret_cast<const AttnWork*>(work), num_work, q_heads, kv_heads, scale,
                            static_cast<cudaStream_t>(stream), nullptr, 1, head_dim);
   return rc ? cuda_fail("paged_attention", rc) : 0;
 }
@@ -430,7 +424,7 @@ int b200_op_paged_attn_decode_split_hd(const void* q, int32_t ldq, void* out, in
     ws_bytes = need;
   }
   int rc = paged_attention(q, ldq, out, ldo, kv_layer, block_tables, max_blocks, reinterpret_cast<const AttnWork*>(work), num_work,
-                           q_heads, kv_heads, scale, 1, static_cast<cudaStream_t>(stream), ws, split, head_dim);
+                           q_heads, kv_heads, scale, static_cast<cudaStream_t>(stream), ws, split, head_dim);
   return rc ? cuda_fail("paged_attention(split)", rc) : 0;
 }
 

@@ -1,4 +1,4 @@
-// Paged causal attention for the per-step hot path (SURVEY.md §8a K6 decode, K7 chunked prefill).
+// Paged causal decode attention for the per-step hot path (SURVEY.md §8a K6; chunked prefill is attention_wgmma.cu).
 // Computes softmax(q . K^T / sqrt(D)) . V over the tokens reachable through a sequence's block
 // table, with head size D = 64 or 128 and G = Hq / Hkv query heads per KV head — the operation the reference backend
 // delegates to FlashInfer/FlashAttention
@@ -21,8 +21,6 @@
 //     head kvh * G + h at position j; rows past G * q_count stay zero, and the K/V of the group is still
 //     read once.  The decode kernel is compiled twice: for G = 4 (the row map folds to shifts and masks)
 //     and for a group size read at run time.
-//   * prefill (op-level only, G = 4): a CTA owns 16 query tokens x 4 heads, one head per warp, and
-//     walks the causal prefix.
 // Rows of a page that lie beyond the sequence's last token are loaded as they are in HBM and masked; the pool is
 // zero-initialised and only ever holds finite K/V values, so a masked probability of 0 never meets a NaN.
 #include <cuda.h>
@@ -30,7 +28,6 @@
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
-#include <stdlib.h>
 
 #include <functional>
 #include <mutex>
@@ -54,23 +51,26 @@ __host__ __device__ constexpr int tile_bytes() { return (D / 64) * kHalfBytes; }
 template <int D>
 __host__ __device__ constexpr int stage_bytes() { return 2 * tile_bytes<D>(); }  // K + V
 
-template <int S, int D>
+// Tiles in flight per CTA.  A 64-token tile is 32 KiB of K + V at D = 128 and 16 KiB at D = 64, so D = 64 keeps twice the
+// tiles in flight: the bytes in flight per CTA are the same at both head sizes.
+template <int D>
+__host__ __device__ constexpr int stages() { return 2 * 128 / D; }
+template <int D>
 constexpr int attn_smem_bytes() {
-  return S * stage_bytes<D>() + 64 + 1024;  // stages + mbarriers + slack for the 1 KiB alignment the swizzle needs
+  return stages<D>() * stage_bytes<D>() + 64 + 1024;  // stages + mbarriers + slack for the 1 KiB alignment the swizzle needs
 }
 
-// S = tiles in flight per CTA; GC = the group size G when it is known at compile time (4), 0 = read G from group;
-// D = head size (64 or 128)
-template <bool DECODE, int S, int GC, int D>
+// GC = the group size G when it is known at compile time (4), 0 = read G from group; D = head size (64 or 128)
+template <int GC, int D>
 __global__ void __launch_bounds__(128)
 paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16* __restrict__ q, int ldq,
                   __nv_bfloat16* __restrict__ out, int ldo, const int* __restrict__ block_tables, int max_blocks,
                   const AttnWork* __restrict__ work, int Hkv, int group, float scale_log2, float* __restrict__ split_ws) {
-  static_assert(DECODE || (GC == 4 && D == 128), "the prefill form is specialised for G = 4 and D = 128");
   static_assert(D == 64 || D == 128, "head size 64 or 128");
+  constexpr int S = stages<D>();
   constexpr int kTileBytes = tile_bytes<D>(), kStageBytes = stage_bytes<D>();
   constexpr int KS = D / 16;  // k-steps of Q K^T, and n16 column pairs of P V
-  constexpr int WT = DECODE ? 16 : 64;  // tokens of each tile handled by one warp
+  constexpr int WT = 16;      // tokens of each tile handled by one warp
   constexpr int NT = WT / 8;
   const int G = GC ? GC : group;
   extern __shared__ uint8_t smem_raw[];
@@ -88,10 +88,10 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
   const int kv_end = wk.q_pos0 + wk.q_count;  // tokens [0, kv_end) are visible to the last query
   const int ntiles = (kv_end + kTile - 1) / kTile;
   const int last_page = (kv_end - 1) >> 4;
-  // split-KV (decode with few sequences: gridDim.z parts per work item so that the context streams on all SMs): this CTA
-  // owns tiles [t_begin, t_end) and leaves an unnormalised (max, sum, acc) per head for attn_merge_kernel
-  const int parts = DECODE ? static_cast<int>(gridDim.z) : 1;
-  const int part = DECODE ? static_cast<int>(blockIdx.z) : 0;
+  // split-KV (few sequences: gridDim.z parts per work item so that the context streams on all SMs): this CTA owns tiles
+  // [t_begin, t_end) and leaves an unnormalised (max, sum, acc) per head for attn_merge_kernel
+  const int parts = static_cast<int>(gridDim.z);
+  const int part = static_cast<int>(blockIdx.z);
   const int tpp = (ntiles + parts - 1) / parts;
   const int t_begin = part * tpp;
   const int t_end = min(ntiles, t_begin + tpp);
@@ -106,7 +106,6 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
   __syncthreads();
 
   // thread 0: gather tile `tile` into stage `stage` (pages past the sequence's last one repeat it; they are masked)
-  const uint64_t hint = DECODE ? kEvictFirst : kEvictNormal;
   auto issue_tile = [&](int tile, int stage) {
     const uint32_t dst = sbase + stage * kStageBytes;
     mbar_arrive_expect_tx(full_bar(stage), kStageBytes);
@@ -119,17 +118,16 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
       const int row_v = row_k + Hkv * 16;
 #pragma unroll
       for (int half = 0; half < D / 64; ++half) {
-        tma_load_2d(dst + half * kHalfBytes + pg * 2048, &tm_kv, full_bar(stage), half * 64, row_k, hint);
-        tma_load_2d(dst + kTileBytes + half * kHalfBytes + pg * 2048, &tm_kv, full_bar(stage), half * 64, row_v, hint);
+        tma_load_2d(dst + half * kHalfBytes + pg * 2048, &tm_kv, full_bar(stage), half * 64, row_k, kEvictFirst);
+        tma_load_2d(dst + kTileBytes + half * kHalfBytes + pg * 2048, &tm_kv, full_bar(stage), half * 64, row_v, kEvictFirst);
       }
     }
   };
 
-  // All S stages are put in flight as early as the data allows.  Decode: every cached token except the newest was
-  // written by an earlier step, so tiles that end before the newest token are gathered BEFORE the dependency wait
-  // (ptx.cuh griddep_enter) and overlap the RoPE/KV-write kernel upstream.  Prefill tiles may hold rows written by
-  // this step: wait first.
-  const int safe_tiles = DECODE ? wk.q_pos0 / kTile : 0;
+  // All S stages are put in flight as early as the data allows.  Every cached token except the newest was written by an
+  // earlier step, so tiles that end before the newest token are gathered BEFORE the dependency wait (ptx.cuh
+  // griddep_enter) and overlap the RoPE/KV-write kernel upstream.
+  const int safe_tiles = wk.q_pos0 / kTile;
   bool waited = false;
 #pragma unroll
   for (int i = 0; i < S; ++i) {
@@ -142,22 +140,16 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
   if (!waited) griddep_enter();
 
   // ---- Q fragments (A operand, 16 rows x D dims as D / 16 k-steps)
-  // decode: fragment rows g and g + 8 are tile rows r = G * j + h, i.e. (j, h) = divmod(r, G); prefill: query tokens
-  const int j0 = DECODE ? g / G : g, j1 = DECODE ? (g + 8) / G : g + 8;
+  // fragment rows g and g + 8 are tile rows r = G * j + h, i.e. (j, h) = divmod(r, G)
+  const int j0 = g / G, j1 = (g + 8) / G;
   uint32_t qf[KS][4];
   {
     const __nv_bfloat16* r0p = nullptr;
     const __nv_bfloat16* r1p = nullptr;
-    if (DECODE) {
-      // rows past the live ones (G * q_count) stay zero: they never touch the rows of the positions that exist
-      const int nrows = G * wk.q_count;
-      if (g < nrows) r0p = q + static_cast<size_t>(wk.q_tok0 + j0) * ldq + (kvh * G + g - j0 * G) * D;
-      if (g + 8 < nrows) r1p = q + static_cast<size_t>(wk.q_tok0 + j1) * ldq + (kvh * G + g + 8 - j1 * G) * D;
-    } else {
-      const int head = kvh * 4 + warp;
-      if (g < wk.q_count) r0p = q + static_cast<size_t>(wk.q_tok0 + g) * ldq + head * D;
-      if (g + 8 < wk.q_count) r1p = q + static_cast<size_t>(wk.q_tok0 + g + 8) * ldq + head * D;
-    }
+    // rows past the live ones (G * q_count) stay zero: they never touch the rows of the positions that exist
+    const int nrows = G * wk.q_count;
+    if (g < nrows) r0p = q + static_cast<size_t>(wk.q_tok0 + j0) * ldq + (kvh * G + g - j0 * G) * D;
+    if (g + 8 < nrows) r1p = q + static_cast<size_t>(wk.q_tok0 + j1) * ldq + (kvh * G + g + 8 - j1 * G) * D;
 #pragma unroll
     for (int ks = 0; ks < KS; ++ks) {
       const int d = ks * 16 + tq * 2;
@@ -172,7 +164,7 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
 #pragma unroll
   for (int i = 0; i < 2 * KS; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
   float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
-  const int wo = DECODE ? warp * 16 : 0;  // this warp's token offset inside a tile
+  const int wo = warp * 16;  // this warp's token offset inside a tile
 
   for (int t = t_begin; t < t_end; ++t) {
     const int stage = (t - t_begin) % S;
@@ -204,8 +196,8 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
         }
       }
       // ---- causal mask, online softmax (fp32, base-2)
-      const int qp0 = DECODE ? wk.q_pos0 + j0 : wk.q_pos0 + g;
-      const int qp1 = DECODE ? wk.q_pos0 + j1 : wk.q_pos0 + g + 8;
+      const int qp0 = wk.q_pos0 + j0;
+      const int qp1 = wk.q_pos0 + j1;
       float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
       for (int nt = 0; nt < NT; ++nt) {
@@ -273,80 +265,63 @@ paged_attn_kernel(const __grid_constant__ CUtensorMap tm_kv, const __nv_bfloat16
   l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
   l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
 
-  if (!DECODE) {
-    const int head = kvh * 4 + warp;
-    const float i0 = l0 > 0.f ? 1.f / l0 : 0.f, i1 = l1 > 0.f ? 1.f / l1 : 0.f;
-    if (g < wk.q_count) {
-      __nv_bfloat16* dst = out + static_cast<size_t>(wk.q_tok0 + g) * ldo + head * D + tq * 2;
+  // merge the 4 warps' partial softmax states: row r = G * j + h of each warp tile is head kvh * G + h at query position
+  // j.  The stages are free here (the loop's last barrier followed the last tile, and no gather is in flight).
+  float* so = reinterpret_cast<float*>(smem);            // [4 warps][16 rows][D]
+  float* sm = so + 4 * 16 * D;                           // [4][16]
+  float* sl = sm + 4 * 16;                               // [4][16]
+  const int nrows = G * wk.q_count;
+  if (g < nrows) {
 #pragma unroll
-      for (int dn = 0; dn < 2 * KS; ++dn)
-        *reinterpret_cast<uint32_t*>(dst + dn * 8) = pack_bf16x2(o[dn][0] * i0, o[dn][1] * i0);
+    for (int dn = 0; dn < 2 * KS; ++dn) {
+      float2 v = make_float2(o[dn][0], o[dn][1]);
+      *reinterpret_cast<float2*>(so + (warp * 16 + g) * D + dn * 8 + tq * 2) = v;
     }
-    if (g + 8 < wk.q_count) {
-      __nv_bfloat16* dst = out + static_cast<size_t>(wk.q_tok0 + g + 8) * ldo + head * D + tq * 2;
-#pragma unroll
-      for (int dn = 0; dn < 2 * KS; ++dn)
-        *reinterpret_cast<uint32_t*>(dst + dn * 8) = pack_bf16x2(o[dn][2] * i1, o[dn][3] * i1);
+    if (tq == 0) {
+      sm[warp * 16 + g] = m0;
+      sl[warp * 16 + g] = l0;
     }
-  } else {
-    // merge the 4 warps' partial softmax states: row r = G * j + h of each warp tile is head kvh * G + h at query position
-    // j.  The stages are free here (the loop's last barrier followed the last tile, and no gather is in flight).
-    float* so = reinterpret_cast<float*>(smem);            // [4 warps][16 rows][D]
-    float* sm = so + 4 * 16 * D;                           // [4][16]
-    float* sl = sm + 4 * 16;                               // [4][16]
-    const int nrows = G * wk.q_count;
-    if (g < nrows) {
+  }
+  if (g + 8 < nrows) {
 #pragma unroll
-      for (int dn = 0; dn < 2 * KS; ++dn) {
-        float2 v = make_float2(o[dn][0], o[dn][1]);
-        *reinterpret_cast<float2*>(so + (warp * 16 + g) * D + dn * 8 + tq * 2) = v;
-      }
-      if (tq == 0) {
-        sm[warp * 16 + g] = m0;
-        sl[warp * 16 + g] = l0;
-      }
+    for (int dn = 0; dn < 2 * KS; ++dn) {
+      float2 v = make_float2(o[dn][2], o[dn][3]);
+      *reinterpret_cast<float2*>(so + (warp * 16 + g + 8) * D + dn * 8 + tq * 2) = v;
     }
-    if (g + 8 < nrows) {
-#pragma unroll
-      for (int dn = 0; dn < 2 * KS; ++dn) {
-        float2 v = make_float2(o[dn][2], o[dn][3]);
-        *reinterpret_cast<float2*>(so + (warp * 16 + g + 8) * D + dn * 8 + tq * 2) = v;
-      }
-      if (tq == 0) {
-        sm[warp * 16 + g + 8] = m1;
-        sl[warp * 16 + g + 8] = l1;
-      }
+    if (tq == 0) {
+      sm[warp * 16 + g + 8] = m1;
+      sl[warp * 16 + g + 8] = l1;
     }
-    __syncthreads();
-    // 128 / D rows at a time: thread tid owns dim tid % D of rows tid / D, tid / D + 128 / D, ... (at D = 128 the block's
-    // 128 threads make tid / D zero; it is spelled out so that the D = 128 code is the single-row loop)
-    const int d = D == 128 ? tid : tid % D;
-    for (int r = D == 128 ? 0 : tid / D; r < nrows; r += 128 / D) {
-      const int j = r / G, h = r - j * G;
-      float mm = -INFINITY;
+  }
+  __syncthreads();
+  // 128 / D rows at a time: thread tid owns dim tid % D of rows tid / D, tid / D + 128 / D, ... (at D = 128 the block's
+  // 128 threads make tid / D zero; it is spelled out so that the D = 128 code is the single-row loop)
+  const int d = D == 128 ? tid : tid % D;
+  for (int r = D == 128 ? 0 : tid / D; r < nrows; r += 128 / D) {
+    const int j = r / G, h = r - j * G;
+    float mm = -INFINITY;
 #pragma unroll
-      for (int w = 0; w < 4; ++w) mm = fmaxf(mm, sm[w * 16 + r]);
-      float num = 0.f, den = 0.f;
+    for (int w = 0; w < 4; ++w) mm = fmaxf(mm, sm[w * 16 + r]);
+    float num = 0.f, den = 0.f;
 #pragma unroll
-      for (int w = 0; w < 4; ++w) {
-        const float mw = sm[w * 16 + r];
-        const float wgt = (mw == -INFINITY) ? 0.f : exp2f(mw - mm);
-        num += so[(w * 16 + r) * D + d] * wgt;
-        den += sl[w * 16 + r] * wgt;
-      }
-      if (parts == 1) {
-        out[static_cast<size_t>(wk.q_tok0 + j) * ldo + (kvh * G + h) * D + d] = __float2bfloat16_rn(den > 0.f ? num / den : 0.f);
-      } else {
-        // position j's slab of [position][work][kv head][part][G heads][D acc | max | sum]: a launch whose items all
-        // have q_count == 1 uses slab 0 only
-        const size_t slab = static_cast<size_t>(gridDim.y) * Hkv * parts * (G * (D + 2));
-        float* dst = split_ws + j * slab + ((static_cast<size_t>(blockIdx.y) * Hkv + kvh) * parts + part) * (G * (D + 2)) +
-                     h * (D + 2);
-        dst[d] = num;
-        if (d == 0) {
-          dst[D] = mm;
-          dst[D + 1] = den;
-        }
+    for (int w = 0; w < 4; ++w) {
+      const float mw = sm[w * 16 + r];
+      const float wgt = (mw == -INFINITY) ? 0.f : exp2f(mw - mm);
+      num += so[(w * 16 + r) * D + d] * wgt;
+      den += sl[w * 16 + r] * wgt;
+    }
+    if (parts == 1) {
+      out[static_cast<size_t>(wk.q_tok0 + j) * ldo + (kvh * G + h) * D + d] = __float2bfloat16_rn(den > 0.f ? num / den : 0.f);
+    } else {
+      // position j's slab of [position][work][kv head][part][G heads][D acc | max | sum]: a launch whose items all
+      // have q_count == 1 uses slab 0 only
+      const size_t slab = static_cast<size_t>(gridDim.y) * Hkv * parts * (G * (D + 2));
+      float* dst = split_ws + j * slab + ((static_cast<size_t>(blockIdx.y) * Hkv + kvh) * parts + part) * (G * (D + 2)) +
+                   h * (D + 2);
+      dst[d] = num;
+      if (d == 0) {
+        dst[D] = mm;
+        dst[D + 1] = den;
       }
     }
   }
@@ -378,17 +353,6 @@ attn_merge_kernel(const float* __restrict__ split_ws, __nv_bfloat16* __restrict_
   }
 }
 
-constexpr int kPrefillStages = 2;
-
-int decode_stages() {  // B200_ATTN_STAGES=2|3|4 (tiles in flight per decode CTA)
-  static const int v = [] {
-    const char* e = getenv("B200_ATTN_STAGES");
-    const int n = e ? atoi(e) : 2;
-    return n == 3 || n == 4 ? n : 2;
-  }();
-  return v;
-}
-
 // One tensor map per (KV-layer base pointer, head size D): the layer is viewed as [rows][D] bf16 with 2 * D-byte rows,
 // gathered in boxes of 16 rows x 64 columns (one page-head half at D = 128, one page-head at D = 64).  The row count is an
 // upper bound, not the allocation size: the kernel only ever addresses pages named by the block table.  The key holds D
@@ -416,35 +380,21 @@ int kv_map_for(const void* kv_layer, CUtensorMap* out, int head_dim) {
 
 namespace {
 
-template <bool DECODE, int S, int GC, int D = 128>
-int launch_attn(const CUtensorMap& tm, dim3 grid, cudaStream_t st, const __nv_bfloat16* q, int ldq, __nv_bfloat16* out,
-                int ldo, const int* block_tables, int max_blocks, const AttnWork* work, int Hkv, int G, float scale_log2,
-                float* split_ws = nullptr) {
+template <int GC, int D>
+int launch_decode(const CUtensorMap& tm, dim3 grid, cudaStream_t st, const __nv_bfloat16* q, int ldq, __nv_bfloat16* out,
+                  int ldo, const int* block_tables, int max_blocks, const AttnWork* work, int Hkv, int G, float scale_log2,
+                  float* split_ws) {
   static std::atomic<unsigned long long> attr_done{0};
-  if (!ensure_dynamic_smem(paged_attn_kernel<DECODE, S, GC, D>, attn_smem_bytes<S, D>(), &attr_done)) return -3;
-  launch_pdl(paged_attn_kernel<DECODE, S, GC, D>, grid, dim3(128), attn_smem_bytes<S, D>(), st, tm, q, ldq, out, ldo, block_tables,
+  if (!ensure_dynamic_smem(paged_attn_kernel<GC, D>, attn_smem_bytes<D>(), &attr_done)) return -3;
+  launch_pdl(paged_attn_kernel<GC, D>, grid, dim3(128), attn_smem_bytes<D>(), st, tm, q, ldq, out, ldo, block_tables,
              max_blocks, work, Hkv, G, scale_log2, split_ws);
   if (cudaGetLastError() != cudaSuccess) return -2;
-  if (DECODE && grid.z > 1) {
+  if (grid.z > 1) {
     launch_pdl(attn_merge_kernel<D>, dim3(grid.x, grid.y), dim3(128), 0, st, static_cast<const float*>(split_ws), out, ldo, work, Hkv,
                G, static_cast<int>(grid.z));
     if (cudaGetLastError() != cudaSuccess) return -2;
   }
   return 0;
-}
-
-// A 64-token tile is 32 KiB of K + V at D = 128 and 16 KiB at D = 64, so D = 64 keeps twice the tiles in flight: the bytes
-// in flight per CTA are the same at both head sizes for every B200_ATTN_STAGES setting.
-template <int GC, int D>
-int launch_decode(const CUtensorMap& tm, dim3 grid, cudaStream_t st, const __nv_bfloat16* q, int ldq, __nv_bfloat16* out,
-                  int ldo, const int* block_tables, int max_blocks, const AttnWork* work, int Hkv, int G, float scale_log2,
-                  float* split_ws) {
-  constexpr int M = 128 / D;
-  switch (decode_stages()) {
-    case 3: return launch_attn<true, 3 * M, GC, D>(tm, grid, st, q, ldq, out, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
-    case 4: return launch_attn<true, 4 * M, GC, D>(tm, grid, st, q, ldq, out, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
-    default: return launch_attn<true, 2 * M, GC, D>(tm, grid, st, q, ldq, out, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
-  }
 }
 
 }  // namespace
@@ -466,10 +416,10 @@ int attn_decode_split(int num_work, int Hkv, int max_ctx, int sms) {
 
 int paged_attention(const void* q, int ldq, void* out, int ldo, const void* kv_layer, const int* block_tables,
                     int max_blocks, const AttnWork* work, int num_work, int Hq, int Hkv, float scale,
-                    int decode, cudaStream_t st, float* split_ws, int split, int head_dim) {
+                    cudaStream_t st, float* split_ws, int split, int head_dim) {
   if (num_work <= 0) return 0;
-  if (!attn_group_ok(Hq, Hkv) || !attn_head_dim_ok(head_dim) || (!decode && (Hq != 4 * Hkv || head_dim != 128))) return -1;
-  if (split > 1 && (!decode || !split_ws)) return -1;
+  if (!attn_group_ok(Hq, Hkv) || !attn_head_dim_ok(head_dim)) return -1;
+  if (split > 1 && !split_ws) return -1;
   const int G = Hq / Hkv;
   CUtensorMap tm;
   if (int rc = kv_map_for(kv_layer, &tm, head_dim)) return rc;
@@ -477,8 +427,6 @@ int paged_attention(const void* q, int ldq, void* out, int ldo, const void* kv_l
   dim3 grid(Hkv, num_work, split > 1 ? split : 1);
   const __nv_bfloat16* qq = static_cast<const __nv_bfloat16*>(q);
   __nv_bfloat16* oo = static_cast<__nv_bfloat16*>(out);
-  if (!decode)
-    return launch_attn<false, kPrefillStages, 4>(tm, grid, st, qq, ldq, oo, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2);
   if (head_dim == 64) {
     if (G == 4) return launch_decode<4, 64>(tm, grid, st, qq, ldq, oo, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);
     return launch_decode<0, 64>(tm, grid, st, qq, ldq, oo, ldo, block_tables, max_blocks, work, Hkv, G, scale_log2, split_ws);

@@ -11,7 +11,6 @@
 
 #include "kernels.h"
 #include "launch.h"
-#include "partials.cuh"
 #include "ptx.cuh"
 
 namespace b200 {
@@ -23,6 +22,16 @@ union Vec8 {
   __nv_bfloat16 h[8];
 };
 
+__device__ __forceinline__ void unpack8_bf16(const uint4& u, float (&o)[8]) {
+  const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float2 f = __bfloat1622float2(h[j]);
+    o[2 * j] = f.x;
+    o[2 * j + 1] = f.y;
+  }
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -30,38 +39,15 @@ __device__ __forceinline__ float warp_sum(float v) {
 }
 
 // ------------------------------------------------------------------ embedding gather
-// ssq (optional): [T, ssq_slabs] per-slab sums of squares of the row, the form the fused GEMM's RMSNorm prologue reads
-// (gemm_wgmma.cu PRO_NORM); the whole row's sum goes to slab 0, the other slabs are zeroed.
 __global__ void embed_kernel(const __nv_bfloat16* __restrict__ table, const int* __restrict__ ids,
-                             __nv_bfloat16* __restrict__ out, int H, int vocab, float* __restrict__ ssq, int ssq_slabs) {
+                             __nv_bfloat16* __restrict__ out, int H, int vocab) {
   griddep_enter();
   const int t = blockIdx.x;
   int id = ids[t];
   if (id < 0 || id >= vocab) id = 0;
   const uint4* src = reinterpret_cast<const uint4*>(table + static_cast<size_t>(id) * H);
   uint4* dst = reinterpret_cast<uint4*>(out + static_cast<size_t>(t) * H);
-  float ss = 0.f;
-  for (int i = threadIdx.x; i < H / 8; i += blockDim.x) {
-    Vec8 v;
-    v.u = __ldg(src + i);
-    dst[i] = v.u;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float f = __bfloat162float(v.h[j]);
-      ss += f * f;
-    }
-  }
-  if (!ssq) return;
-  __shared__ float red[32];
-  ss = warp_sum(ss);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = ss;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    float v = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
-    v = warp_sum(v);
-    if (threadIdx.x == 0) ssq[static_cast<size_t>(t) * ssq_slabs] = v;
-  }
-  for (int i = 1 + threadIdx.x; i < ssq_slabs; i += blockDim.x) ssq[static_cast<size_t>(t) * ssq_slabs + i] = 0.f;
+  for (int i = threadIdx.x; i < H / 8; i += blockDim.x) dst[i] = __ldg(src + i);
 }
 
 // ------------------------------------------------------------------ (fused add) RMSNorm
@@ -70,10 +56,9 @@ __global__ void embed_kernel(const __nv_bfloat16* __restrict__ table, const int*
 template <int VPT>  // uint4 vectors per thread (H = VPT * 8 * blockDim)
 __global__ void rmsnorm_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ residual,
                                const __nv_bfloat16* __restrict__ w, __nv_bfloat16* __restrict__ out,
-                               const int* __restrict__ row_index, int H, float eps, PartialView pv) {
+                               const int* __restrict__ row_index, int H, float eps) {
   // ---- before the dependency wait (ptx.cuh griddep_enter): everything that does not come from the producer GEMM —
-  // the row index (step input), the residual (written four or more launches upstream), the norm weight and the
-  // partial-segment table entries (static)
+  // the row index (step input), the residual (written four or more launches upstream) and the norm weight
   const int s = blockIdx.x;
   const int r = row_index ? row_index[s] : s;
   const uint4* xin = reinterpret_cast<const uint4*>(x + static_cast<size_t>(r) * H);
@@ -81,27 +66,19 @@ __global__ void rmsnorm_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat1
   float v[VPT][8];
   float ss = 0.f;
   Vec8 rb[VPT], ww[VPT];
-  int n0[VPT];
-  int2 ent[VPT];
 #pragma unroll
   for (int i = 0; i < VPT; ++i) {
     const int idx = threadIdx.x + i * blockDim.x;
-    n0[i] = idx * 8;
     ww[i].u = __ldg(reinterpret_cast<const uint4*>(w) + idx);
     if (res) rb[i].u = res[idx];
   }
-  if (pv.ws) partial_entries<VPT>(pv, r, n0, ent);
   griddep_enter();
   float xa[VPT][8];
-  if (pv.ws) {
-    load8xM_entries<VPT>(pv, ent, r, n0, xa);  // x = bf16(sum of the GEMM's stream-K segments)
-  } else {
-    uint4 raw[VPT];
+  uint4 raw[VPT];
 #pragma unroll
-    for (int i = 0; i < VPT; ++i) raw[i] = xin[threadIdx.x + i * blockDim.x];
+  for (int i = 0; i < VPT; ++i) raw[i] = xin[threadIdx.x + i * blockDim.x];
 #pragma unroll
-    for (int i = 0; i < VPT; ++i) unpack8_bf16(raw[i], xa[i]);
-  }
+  for (int i = 0; i < VPT; ++i) unpack8_bf16(raw[i], xa[i]);
 #pragma unroll
   for (int i = 0; i < VPT; ++i) {
     const int idx = threadIdx.x + i * blockDim.x;
@@ -154,12 +131,12 @@ __global__ void rmsnorm_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat1
 template <int D>
 __global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ qkv, const int* __restrict__ positions,
                                const int* __restrict__ slots, const __nv_bfloat16* __restrict__ cos_sin,
-                               __nv_bfloat16* __restrict__ kv, int Hq, int Hkv, int max_pos, PartialView pv) {
+                               __nv_bfloat16* __restrict__ kv, int Hq, int Hkv, int max_pos) {
   constexpr int HALF = D / 2, RT = HALF / 8, VT = D / 8;  // rotation / V-copy tasks per head
   constexpr int RTL = D == 128 ? 3 : 2, VTL = RTL + 1;     // their log2
   const int t = blockIdx.x;
-  // ---- before the dependency wait: step inputs (positions, slots), cos/sin rows and table entries (static).  The
-  // first task of every thread is prepared here; later tasks (only when blockDim < tasks) look theirs up afterwards.
+  // ---- before the dependency wait: step inputs (positions, slots) and cos/sin rows.  The first task of every thread is
+  // prepared here; later tasks (only when blockDim < tasks) load theirs afterwards.
   int pos = positions[t];
   pos = pos < 0 ? 0 : (pos >= max_pos ? max_pos - 1 : pos);
   const int slot = slots[t];
@@ -174,15 +151,10 @@ __global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ qkv, const int* __res
   const int rot_tasks = (Hq + Hkv) * RT;  // 8 elements of x1 (and the matching 8 of x2) per task
   const int v_tasks = Hkv * VT;
   Vec8 co0, si0;
-  int2 ent0[2] = {make_int2(0, 1), make_int2(0, 1)};
   if (static_cast<int>(threadIdx.x) < rot_tasks) {
-    const int head = threadIdx.x >> RTL, c = threadIdx.x & (RT - 1);
+    const int c = threadIdx.x & (RT - 1);
     co0.u = __ldg(reinterpret_cast<const uint4*>(cs + c * 8));
     si0.u = __ldg(reinterpret_cast<const uint4*>(cs + HALF + c * 8));
-    if (pv.ws) {
-      const int n0[2] = {head * D + c * 8, head * D + HALF + c * 8};
-      partial_entries<2>(pv, t, n0, ent0);
-    }
   }
   griddep_enter();
   // rotation tasks and V-copy tasks share one index space so that a 512-thread CTA gives every thread one task
@@ -190,34 +162,9 @@ __global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ qkv, const int* __res
     const int head = task >> RTL, c = task & (RT - 1);
     const bool first = task == static_cast<int>(threadIdx.x);
     __nv_bfloat16* hp = row + head * D;
-    Vec8 co, si, o1, o2;
-    float xa[8], xb[8];
-    if (pv.ws) {
-      const int n0[2] = {head * D + c * 8, head * D + HALF + c * 8};
-      int2 ent[2];
-      if (first) {
-        ent[0] = ent0[0];
-        ent[1] = ent0[1];
-      } else {
-        partial_entries<2>(pv, t, n0, ent);
-      }
-      float xx[2][8];
-      load8xM_entries<2>(pv, ent, t, n0, xx);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        xa[j] = xx[0][j];
-        xb[j] = xx[1][j];
-      }
-    } else {
-      Vec8 x1, x2;
-      x1.u = *reinterpret_cast<const uint4*>(hp + c * 8);
-      x2.u = *reinterpret_cast<const uint4*>(hp + HALF + c * 8);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        xa[j] = __bfloat162float(x1.h[j]);
-        xb[j] = __bfloat162float(x2.h[j]);
-      }
-    }
+    Vec8 x1, x2, co, si, o1, o2;
+    x1.u = *reinterpret_cast<const uint4*>(hp + c * 8);
+    x2.u = *reinterpret_cast<const uint4*>(hp + HALF + c * 8);
     if (first) {
       co = co0;
       si = si0;
@@ -227,7 +174,7 @@ __global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ qkv, const int* __res
     }
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      const float a = xa[j], b = xb[j];
+      const float a = __bfloat162float(x1.h[j]), b = __bfloat162float(x2.h[j]);
       const float cc = __bfloat162float(co.h[j]), sn = __bfloat162float(si.h[j]);
       // every bf16 op rounds, exactly like the reference kernel's scalar_t arithmetic
       // (x * cos - y * sin with c10::BFloat16 operators == rotary_embedding/common.py:173-174)
@@ -252,18 +199,8 @@ __global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ qkv, const int* __res
     for (int task = static_cast<int>((threadIdx.x + blockDim.x - rot_tasks % blockDim.x) % blockDim.x); task < v_tasks;
          task += blockDim.x) {
       const int head = task >> VTL, c = task & (VT - 1);
-      uint4 val;
-      if (pv.ws) {
-        float f[8];
-        load8_partials(pv, t, (Hq + Hkv + head) * D + c * 8, f);
-        val.x = pack_bf16x2(f[0], f[1]);
-        val.y = pack_bf16x2(f[2], f[3]);
-        val.z = pack_bf16x2(f[4], f[5]);
-        val.w = pack_bf16x2(f[6], f[7]);
-      } else {
-        val = *reinterpret_cast<const uint4*>(vrow + head * D + c * 8);
-      }
-      *reinterpret_cast<uint4*>(vbase + (static_cast<size_t>(head) * 16 + off) * D + c * 8) = val;
+      *reinterpret_cast<uint4*>(vbase + (static_cast<size_t>(head) * 16 + off) * D + c * 8) =
+          *reinterpret_cast<const uint4*>(vrow + head * D + c * 8);
     }
   }
 }
@@ -273,7 +210,7 @@ template <int VPT>  // uint4 output vectors per thread
 // interleaved != 0: gate and up columns alternate in 64-column blocks (the engine's gate_up weight rows are laid out
 // that way so that the decode GEMM's epilogue finds a gate row and its up row in one 128-row slab)
 __global__ void silu_mul_kernel(const __nv_bfloat16* __restrict__ gu, __nv_bfloat16* __restrict__ out, int I,
-                                int ldi, PartialView pv, int interleaved) {
+                                int ldi, int interleaved) {
   const int t = blockIdx.y;
   const uint4* g = reinterpret_cast<const uint4*>(gu + static_cast<size_t>(t) * ldi);
   uint4* o = reinterpret_cast<uint4*>(out + static_cast<size_t>(t) * I);
@@ -281,7 +218,6 @@ __global__ void silu_mul_kernel(const __nv_bfloat16* __restrict__ gu, __nv_bfloa
   const int i0 = blockIdx.x * blockDim.x * VPT + threadIdx.x;
   float x[2 * VPT][8];  // gate vectors, then up vectors
   int n0[2 * VPT];
-  int2 ent[2 * VPT];
 #pragma unroll
   for (int k = 0; k < VPT; ++k) {
     const int i = min(i0 + k * static_cast<int>(blockDim.x), nvec - 1);
@@ -289,20 +225,15 @@ __global__ void silu_mul_kernel(const __nv_bfloat16* __restrict__ gu, __nv_bfloa
     n0[k] = interleaved ? ((c >> 6) << 7) + (c & 63) : c;
     n0[VPT + k] = interleaved ? n0[k] + 64 : I + c;
   }
-  if (pv.ws) partial_entries<2 * VPT>(pv, t, n0, ent);  // static table: looked up before the dependency wait
   griddep_enter();
-  if (pv.ws) {
-    load8xM_entries<2 * VPT>(pv, ent, t, n0, x);
-  } else {
-    uint4 raw[2 * VPT];
+  uint4 raw[2 * VPT];
 #pragma unroll
-    for (int k = 0; k < VPT; ++k) {
-      raw[k] = g[n0[k] >> 3];
-      raw[VPT + k] = g[n0[VPT + k] >> 3];
-    }
-#pragma unroll
-    for (int k = 0; k < 2 * VPT; ++k) unpack8_bf16(raw[k], x[k]);
+  for (int k = 0; k < VPT; ++k) {
+    raw[k] = g[n0[k] >> 3];
+    raw[VPT + k] = g[n0[VPT + k] >> 3];
   }
+#pragma unroll
+  for (int k = 0; k < 2 * VPT; ++k) unpack8_bf16(raw[k], x[k]);
 #pragma unroll
   for (int k = 0; k < VPT; ++k) {
     const int i = i0 + k * blockDim.x;
@@ -319,8 +250,7 @@ __global__ void silu_mul_kernel(const __nv_bfloat16* __restrict__ gu, __nv_bfloa
 }
 
 // ------------------------------------------------------------------ greedy argmax over bf16 logits
-__global__ void argmax_kernel(const __nv_bfloat16* __restrict__ logits, int* __restrict__ out, int V, int ld,
-                              PartialView pv) {
+__global__ void argmax_kernel(const __nv_bfloat16* __restrict__ logits, int* __restrict__ out, int V, int ld) {
   griddep_enter();
   const int s = blockIdx.x;
   const __nv_bfloat16* row = logits + static_cast<size_t>(s) * ld;
@@ -329,18 +259,11 @@ __global__ void argmax_kernel(const __nv_bfloat16* __restrict__ logits, int* __r
   const int nvec = V / 8;
   const uint4* r4 = reinterpret_cast<const uint4*>(row);
   for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
-    float fa[8];
-    if (pv.ws) {
-      load8_partials(pv, s, i * 8, fa);
-    } else {
-      Vec8 a;
-      a.u = r4[i];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) fa[j] = __bfloat162float(a.h[j]);
-    }
+    Vec8 a;
+    a.u = r4[i];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      const float f = fa[j];
+      const float f = __bfloat162float(a.h[j]);
       const int idx = i * 8 + j;
       if (f > best || (f == best && idx < bi)) {
         best = f;
@@ -348,7 +271,7 @@ __global__ void argmax_kernel(const __nv_bfloat16* __restrict__ logits, int* __r
       }
     }
   }
-  for (int idx = nvec * 8 + threadIdx.x; idx < V && !pv.ws; idx += blockDim.x) {
+  for (int idx = nvec * 8 + threadIdx.x; idx < V; idx += blockDim.x) {
     const float f = __bfloat162float(row[idx]);
     if (f > best || (f == best && idx < bi)) {
       best = f;
@@ -424,17 +347,16 @@ __global__ void init_uniform_kernel(__nv_bfloat16* __restrict__ p, size_t n, uin
 
 }  // namespace
 
-int embed_gather(const void* table, const int* ids, void* out, int T, int H, int vocab, cudaStream_t st, float* ssq,
-                 int ssq_slabs) {
+int embed_gather(const void* table, const int* ids, void* out, int T, int H, int vocab, cudaStream_t st) {
   if (T <= 0) return 0;
   if (H % 8) return -1;
   launch_pdl(embed_kernel, dim3(T), dim3(256), 0, st, static_cast<const __nv_bfloat16*>(table), ids,
-             static_cast<__nv_bfloat16*>(out), H, vocab, ssq, ssq_slabs);
+             static_cast<__nv_bfloat16*>(out), H, vocab);
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 
 int rmsnorm(const void* x, void* residual, const void* w, void* out, const int* row_index, int rows, int H,
-            float eps, cudaStream_t st, PartialView pv) {
+            float eps, cudaStream_t st) {
   if (rows <= 0) return 0;
   const __nv_bfloat16* xx = static_cast<const __nv_bfloat16*>(x);
   __nv_bfloat16* rr = static_cast<__nv_bfloat16*>(residual);
@@ -442,18 +364,16 @@ int rmsnorm(const void* x, void* residual, const void* w, void* out, const int* 
   __nv_bfloat16* oo = static_cast<__nv_bfloat16*>(out);
   if (H % 8) return -1;
   const int vecs = H / 8;
-  // one 8-element vector per thread when the row fits a CTA (most loads in flight per row: the partial
-  // reads are L2 round trips), otherwise 256 threads with up to 4 vectors each
   // few rows (decode): one vector per thread so each row has the most loads in flight; many rows (prefill bursts):
   // 256-thread CTAs with 2-4 vectors each (measured: 24 us vs 29 us per call at T=2048, H=4096)
   if (vecs % 32 == 0 && vecs <= 1024 && (rows < 512 || vecs % 256 != 0 || vecs / 256 > 4)) {
-    launch_pdl(rmsnorm_kernel<1>, dim3(rows), dim3(vecs), 0, st, xx, rr, ww, oo, row_index, H, eps, pv);
+    launch_pdl(rmsnorm_kernel<1>, dim3(rows), dim3(vecs), 0, st, xx, rr, ww, oo, row_index, H, eps);
   } else if (vecs % 256 == 0 && vecs / 256 <= 4) {
     switch (vecs / 256) {
-      case 1: launch_pdl(rmsnorm_kernel<1>, dim3(rows), dim3(256), 0, st, xx, rr, ww, oo, row_index, H, eps, pv); break;
-      case 2: launch_pdl(rmsnorm_kernel<2>, dim3(rows), dim3(256), 0, st, xx, rr, ww, oo, row_index, H, eps, pv); break;
-      case 3: launch_pdl(rmsnorm_kernel<3>, dim3(rows), dim3(256), 0, st, xx, rr, ww, oo, row_index, H, eps, pv); break;
-      default: launch_pdl(rmsnorm_kernel<4>, dim3(rows), dim3(256), 0, st, xx, rr, ww, oo, row_index, H, eps, pv); break;
+      case 1: launch_pdl(rmsnorm_kernel<1>, dim3(rows), dim3(256), 0, st, xx, rr, ww, oo, row_index, H, eps); break;
+      case 2: launch_pdl(rmsnorm_kernel<2>, dim3(rows), dim3(256), 0, st, xx, rr, ww, oo, row_index, H, eps); break;
+      case 3: launch_pdl(rmsnorm_kernel<3>, dim3(rows), dim3(256), 0, st, xx, rr, ww, oo, row_index, H, eps); break;
+      default: launch_pdl(rmsnorm_kernel<4>, dim3(rows), dim3(256), 0, st, xx, rr, ww, oo, row_index, H, eps); break;
     }
   } else {
     return -1;
@@ -462,7 +382,7 @@ int rmsnorm(const void* x, void* residual, const void* w, void* out, const int* 
 }
 
 int rope_kv_write(void* qkv, const int* positions, const int* slots, const void* cos_sin, void* kv_layer,
-                  int T, int Hq, int Hkv, int max_pos, cudaStream_t st, PartialView pv, int head_dim) {
+                  int T, int Hq, int Hkv, int max_pos, cudaStream_t st, int head_dim) {
   if (T <= 0) return 0;
   if (head_dim != 64 && head_dim != 128) return -1;
   const int tasks = ((Hq + Hkv) * 8 + Hkv * 16) * head_dim / 128;
@@ -470,27 +390,27 @@ int rope_kv_write(void* qkv, const int* positions, const int* slots, const void*
   const int threads = T >= 512 ? 128 : tasks >= 512 ? 512 : tasks >= 256 ? 256 : 128;
   launch_pdl(head_dim == 64 ? rope_kv_kernel<64> : rope_kv_kernel<128>, dim3(T), dim3(threads), 0, st,
              static_cast<__nv_bfloat16*>(qkv), positions, slots, static_cast<const __nv_bfloat16*>(cos_sin),
-             static_cast<__nv_bfloat16*>(kv_layer), Hq, Hkv, max_pos, pv);
+             static_cast<__nv_bfloat16*>(kv_layer), Hq, Hkv, max_pos);
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 
-int silu_mul(const void* gate_up, void* out, int T, int I, cudaStream_t st, PartialView pv, int interleaved) {
+int silu_mul(const void* gate_up, void* out, int T, int I, cudaStream_t st, int interleaved) {
   if (T <= 0) return 0;
   if (I % 8) return -1;
   const __nv_bfloat16* gu = static_cast<const __nv_bfloat16*>(gate_up);
   __nv_bfloat16* o = static_cast<__nv_bfloat16*>(out);
   // decode: one output vector per thread (2 loads in flight); prefill bursts: two (4 batched loads in flight)
   if (T >= 512)
-    launch_pdl(silu_mul_kernel<2>, dim3((I / 8 + 511) / 512, T), dim3(256), 0, st, gu, o, I, 2 * I, pv, interleaved);
+    launch_pdl(silu_mul_kernel<2>, dim3((I / 8 + 511) / 512, T), dim3(256), 0, st, gu, o, I, 2 * I, interleaved);
   else
-    launch_pdl(silu_mul_kernel<1>, dim3((I / 8 + 255) / 256, T), dim3(256), 0, st, gu, o, I, 2 * I, pv, interleaved);
+    launch_pdl(silu_mul_kernel<1>, dim3((I / 8 + 255) / 256, T), dim3(256), 0, st, gu, o, I, 2 * I, interleaved);
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 
-int argmax_rows(const void* logits, int* out, int S, int V, int ld, cudaStream_t st, PartialView pv) {
+int argmax_rows(const void* logits, int* out, int S, int V, int ld, cudaStream_t st) {
   if (S <= 0) return 0;
-  if (ld % 8 || (pv.ws && V % 8)) return -1;
-  launch_pdl(argmax_kernel, dim3(S), dim3(1024), 0, st, static_cast<const __nv_bfloat16*>(logits), out, V, ld, pv);
+  if (ld % 8) return -1;
+  launch_pdl(argmax_kernel, dim3(S), dim3(1024), 0, st, static_cast<const __nv_bfloat16*>(logits), out, V, ld);
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 

@@ -529,7 +529,7 @@ struct Engine {
     int split = 1;
     if (m.nd <= kSplitMaxWork) split = std::min(attn_split_force > 0 ? attn_split_force : attn_decode_split(m.nd, Hkv, m.dmax_ctx, sms), kSplitMaxParts);
     if (split > 1) ++stats.kernel_launches;   // the merge kernel
-    return paged_attention(qkv, QKV, attn, Hq * Dh, kv_l, btab, max_blocks_per_seq, dwork, m.nd, Hq, Hkv, scale, 1, stream, attn_ws, split, Dh);
+    return paged_attention(qkv, QKV, attn, Hq * Dh, kv_l, btab, max_blocks_per_seq, dwork, m.nd, Hq, Hkv, scale, stream, attn_ws, split, Dh);
   }
   int prefill_attention(bf16* kv_l, const int* btab, const AttnWork* pwork, int np, float scale) {
     return paged_attention_prefill_tc(qkv, Tcap, QKV, attn, Hq * Dh, kv_l, btab, max_blocks_per_seq, pwork, np, Hq, Hkv, scale, stream, Dh);
@@ -986,7 +986,7 @@ int Engine::forward(const StepMeta& m, int32_t* dbuf, bool all_logits, bf16* log
       rc |= launch_proj(p, xm_normed, T);
     }
     Q();
-    if (!fused) { P(B200_K_ROPE); if (on(B200_K_ROPE)) rc |= rope_kv_write(qkv, pos, slots, cos_sin, kv_l, T, Hq, Hkv, cfg.max_model_len, stream, no_partials(), Dh); Q(); launched(1); }
+    if (!fused) { P(B200_K_ROPE); if (on(B200_K_ROPE)) rc |= rope_kv_write(qkv, pos, slots, cos_sin, kv_l, T, Hq, Hkv, cfg.max_model_len, stream, Dh); Q(); launched(1); }
     if (m.nd) { P(B200_K_ATTN_DECODE); if (on(B200_K_ATTN_DECODE)) rc |= decode_attention(m, kv_l, btab, dwork, scale); Q(); launched(1); }
     if (m.np) { P(B200_K_ATTN_PREFILL); if (on(B200_K_ATTN_PREFILL)) rc |= prefill_attention(kv_l, btab, pwork, m.np, scale); Q(); launched(1); }
     P(B200_K_GEMM_O); if (on(B200_K_GEMM_O)) resadd_proj(ly.p_o, xm_attn); Q();
@@ -998,7 +998,7 @@ int Engine::forward(const StepMeta& m, int32_t* dbuf, bool all_logits, bf16* log
       rc |= launch_proj(p, xm_normed, T);
     }
     Q();
-    if (!fused) { P(B200_K_SILU); if (on(B200_K_SILU)) rc |= silu_mul(gu, act, T, I, stream, no_partials(), 1); Q(); launched(1); }
+    if (!fused) { P(B200_K_SILU); if (on(B200_K_SILU)) rc |= silu_mul(gu, act, T, I, stream, 1); Q(); launched(1); }
     P(B200_K_GEMM_DOWN); if (on(B200_K_GEMM_DOWN)) resadd_proj(ly.p_down, xm_act); Q();
   }
   if (rc) return cuda_fail("forward", -2);

@@ -7,19 +7,13 @@
 
 #include <vector>
 
-#include "partials.cuh"
-
 namespace b200 {
 
-// ssq (optional): [T, ssq_slabs] fp32, the row's sum of squares in slab 0 and zeros elsewhere (RMSNorm prologue of the fused GEMM)
-int embed_gather(const void* table, const int* ids, void* out, int T, int H, int vocab, cudaStream_t st, float* ssq = nullptr,
-                 int ssq_slabs = 0);
+int embed_gather(const void* table, const int* ids, void* out, int T, int H, int vocab, cudaStream_t st);
 // out[s] = rmsnorm(x[r] (+ residual[r])) * w,  r = row_index ? row_index[s] : s.
 // residual (optional) is updated in place with bf16(x + residual) unless row_index is given.
-// Every consumer of a GEMM output takes an optional PartialView: when pv.ws != nullptr the input is the fp32
-// stream-K partials of the preceding deferred GEMM (summed + rounded to bf16 on load) instead of the bf16 tensor.
 int rmsnorm(const void* x, void* residual, const void* w, void* out, const int* row_index, int rows, int H,
-            float eps, cudaStream_t st, PartialView pv = no_partials());
+            float eps, cudaStream_t st);
 // Last-token pooling (pooling.cu): out[s] (fp32 [rows, H]) = the final RMSNorm of row row_index[s] of x (+ residual, as
 // rmsnorm with a row_index), bit-identical in bf16 to rmsnorm over the same rows, then L2-normalised in fp32 when
 // flags[s] != 0.  H % 256 == 0 and H <= 8192; row_index and flags are device int arrays [rows].
@@ -27,12 +21,12 @@ int pool_rows(const void* x, const void* residual, const void* w, const int* row
               float eps, float* out, cudaStream_t st);
 // head_dim D = 64 or 128: qkv rows [(Hq + 2 Hkv) * D], cos_sin rows [D], kv_layer [block][2][Hkv][16][D]
 int rope_kv_write(void* qkv, const int* positions, const int* slots, const void* cos_sin, void* kv_layer,
-                  int T, int Hq, int Hkv, int max_pos, cudaStream_t st, PartialView pv = no_partials(), int head_dim = 128);
+                  int T, int Hq, int Hkv, int max_pos, cudaStream_t st, int head_dim = 128);
 // interleaved: gate/up columns alternate in 64-column blocks (engine layout) instead of [gate | up]
-int silu_mul(const void* gate_up, void* out, int T, int I, cudaStream_t st, PartialView pv = no_partials(), int interleaved = 0);
+int silu_mul(const void* gate_up, void* out, int T, int I, cudaStream_t st, int interleaved = 0);
 // gate_up weight rows: logical [gate | up] <-> physical (64 gate rows, their 64 up rows, ...); dst != src
 int permute_gate_up(void* dst, const void* src, int I, int H, int to_physical, cudaStream_t st);
-int argmax_rows(const void* logits, int* out, int S, int V, int ld, cudaStream_t st, PartialView pv = no_partials());
+int argmax_rows(const void* logits, int* out, int S, int V, int ld, cudaStream_t st);
 int init_uniform(void* p, size_t n, uint32_t seed, float scale, float offset, cudaStream_t st);
 // Parallel sampling's fork (kv_fork.cu): for every pair i and every layer l, copy the block_bytes of page src[i] to page
 // dst[i] at kv + l * layer_stride_bytes (src / dst device int arrays; sizes and kv 16-byte aligned).  Bit-exact; nothing
@@ -99,7 +93,7 @@ int logprobs_rows(const void* logits, int ld, int V, const int* rows, const int*
 // step's token batch; the first of them sits at absolute position q_pos0 in the sequence.
 struct AttnWork {
   int q_tok0;
-  int q_count;  // decode: 1, or up to kDecodeRows / G consecutive positions (a speculative verify); <= 16 for a prefill tile
+  int q_count;  // decode: 1, or up to kDecodeRows / G consecutive positions (a speculative verify); prefill: <= kPrefillQueryBlock
   int q_pos0;
   int seq;      // row of block_tables
 };
@@ -117,11 +111,11 @@ inline bool attn_head_dim_ok(int D) { return D == 64 || D == 128; }
 // Paged causal attention, head_dim D (attn_head_dim_ok), G = Hq / Hkv query heads per KV head (attn_group_ok), page = 16 tokens.
 //   q: rows of the fused qkv buffer (leading dim ldq), out: [T, Hq*D] (leading dim ldo)
 //   kv_layer: [block][2][Hkv][16][D];  block_tables: [num_seqs, max_blocks] int32
-//   decode != 0: every work item has 1 <= q_count and G * q_count <= kDecodeRows (position j causally masked at q_pos0 + j)
-//   and the CTA's 4 warps split the KV range.  decode == 0 (the op-level prefill form) needs G == 4 and D == 128.
+//   every work item has 1 <= q_count and G * q_count <= kDecodeRows (position j causally masked at q_pos0 + j); the CTA's
+//   4 warps split the KV range.  Chunked prefill is paged_attention_prefill_tc.
 int paged_attention(const void* q, int ldq, void* out, int ldo, const void* kv_layer, const int* block_tables,
                     int max_blocks, const AttnWork* work, int num_work, int Hq, int Hkv, float scale,
-                    int decode, cudaStream_t st, float* split_ws = nullptr, int split = 1, int head_dim = 128);
+                    cudaStream_t st, float* split_ws = nullptr, int split = 1, int head_dim = 128);
 // split-KV decode (few sequences): `split` CTAs per (work item, KV head) each stream a slice of the context and leave an
 // unnormalised partial per query head in split_ws (attn_split_ws_bytes, max_q = the largest q_count of the launch), merged
 // by a second tiny kernel.  attn_decode_split picks `split`.

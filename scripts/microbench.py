@@ -98,7 +98,7 @@ def large_bench():
 def attn_prefill_bench():
     """chunked-prefill attention (tensor-core kernel, 64-query work items) vs FlashInfer's paged prefill on burst-like shapes:
     (requests, cached prefix, new tokens)"""
-    print("== paged prefill attention, Hq=32/Hkv=8: (requests x [cached + new]) mine (wgmma) / mine (mma.sync) / FlashInfer")
+    print("== paged prefill attention, Hq=32/Hkv=8: (requests x [cached + new]) mine (wgmma) / FlashInfer")
     Hq, Hkv, D = 32, 8, 128
     for nreq, cached, new in ((10, 320, 130), (4, 0, 384), (1, 0, 1536), (3, 1500, 500), (24, 400, 64)):
         ctx = cached + new
@@ -108,19 +108,11 @@ def attn_prefill_bench():
         perm = torch.randperm(nblk, device="cuda").to(torch.int32).reshape(nreq, -1).contiguous()
         T = nreq * new
         qkv = torch.randn(T, (Hq + 2 * Hkv) * D, device="cuda").bfloat16()
-        res = {}
-        for name, qb, fn in (("tc", 64, ops.paged_attn_prefill_tc), ("mma", 16, None)):
-            work = []
-            for r in range(nreq):
-                for j in range(0, new, qb):
-                    work.append([r * new + j, min(qb, new - j), cached + j, r])
-            wt = torch.tensor(work, dtype=torch.int32, device="cuda")
-            out = torch.zeros(T, Hq * D, dtype=torch.bfloat16, device="cuda")
-            if fn is not None:
-                res[name] = (timeit(lambda: fn(qkv, kv, perm, wt, Hq, Hkv, out=out)), out)
-            else:
-                res[name] = (timeit(lambda: ops.paged_attn(qkv, kv, perm, wt, Hq, Hkv, False, out=out)), out)
-        line = f"{nreq:3d} x [{cached:4d} + {new:4d}]  wgmma {res['tc'][0]:7.1f} us   mma.sync {res['mma'][0]:7.1f} us"
+        work = [[r * new + j, min(64, new - j), cached + j, r] for r in range(nreq) for j in range(0, new, 64)]
+        wt = torch.tensor(work, dtype=torch.int32, device="cuda")
+        out = torch.zeros(T, Hq * D, dtype=torch.bfloat16, device="cuda")
+        t_tc = timeit(lambda: ops.paged_attn_prefill_tc(qkv, kv, perm, wt, Hq, Hkv, out=out))
+        line = f"{nreq:3d} x [{cached:4d} + {new:4d}]  wgmma {t_tc:7.1f} us"
         try:
             import flashinfer
             ws = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
@@ -132,7 +124,7 @@ def attn_prefill_bench():
             q = qkv[:, :Hq * D].reshape(T, Hq, D).contiguous()
             tf = timeit(lambda: wr.run(q, kv))
             o2 = wr.run(q, kv).reshape(T, Hq * D)
-            line += f"   flashinfer {tf:7.1f} us   ratio {tf / res['tc'][0]:4.2f}x   max |mine - flashinfer| {float((res['tc'][1].float() - o2.float()).abs().max()):.4f}"
+            line += f"   flashinfer {tf:7.1f} us   ratio {tf / t_tc:4.2f}x   max |mine - flashinfer| {float((out.float() - o2.float()).abs().max()):.4f}"
         except Exception as e:  # noqa: BLE001
             line += "   flashinfer unavailable: " + repr(e)[:160]
         print(line, flush=True)

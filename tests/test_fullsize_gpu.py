@@ -255,11 +255,11 @@ def test_split_kv_decode_attention_matches_oracle_and_the_unsplit_kernel(split):
     assert torch.equal(ops.paged_attn(q, kv, btab, work, Hq, Hkv, decode=True, split=1).float(), base)
 
 
-@pytest.mark.parametrize("kernel", ["tensor_core", "mma_sync"])
+@pytest.mark.parametrize("kernel", ["tensor_core"])
 def test_chunked_prefill_attention_at_production_shape_with_cached_prefix(kernel):
     from kubeai_b200 import ops
     Hq, Hkv = 32, 8
-    qb = 64 if kernel == "tensor_core" else 16
+    qb = 64
     case = [(2048, 512), (1023, 1023), (16, 16), (1500, 37), (2047, 1), (777, 300), (64, 64), (1025, 1000)]   # (context, new tokens)
     lens = [c[0] for c in case]
     kv, btab, ks, vs = _pool(lens, Hkv, seed=22)
@@ -273,8 +273,7 @@ def test_chunked_prefill_attention_at_production_shape_with_cached_prefix(kernel
         spans.append(tok)
         tok += n
     wt = torch.tensor(work, dtype=torch.int32).cuda()
-    got = (ops.paged_attn_prefill_tc(q, kv, btab, wt, Hq, Hkv) if kernel == "tensor_core"
-           else ops.paged_attn(q, kv, btab, wt, Hq, Hkv, decode=False)).float()
+    got = ops.paged_attn_prefill_tc(q, kv, btab, wt, Hq, Hkv).float()
     torch.cuda.synchronize()
     for i, (L, n) in enumerate(case):
         t0 = spans[i]
@@ -283,7 +282,7 @@ def test_chunked_prefill_attention_at_production_shape_with_cached_prefix(kernel
         _attn_close(got[t0:t0 + n], want, f"prefill seq {i} ctx {L} new {n}")
 
 
-@pytest.mark.parametrize("kernel", ["decode", "decode_split_7", "tensor_core", "mma_sync"])
+@pytest.mark.parametrize("kernel", ["decode", "decode_split_7", "tensor_core"])
 def test_peaky_attention_at_production_shape(kernel):
     """Random data with queries x 4: a few tokens carry most of each softmax, so P's bf16 rounding lands on large weights."""
     from kubeai_b200 import ops
@@ -291,7 +290,7 @@ def test_peaky_attention_at_production_shape(kernel):
     case = [(2048, 1 if kernel.startswith("decode") else 200), (1023, 1 if kernel.startswith("decode") else 64), (65, 1), (4097, 1)]
     lens = [c[0] for c in case]
     kv, btab, ks, vs = _pool(lens, Hkv, seed=24)
-    qb = 64 if kernel == "tensor_core" else 16
+    qb = 64
     T = sum(n for _, n in case)
     q = 4 * torch.randn(T, Hq * 128, generator=torch.Generator(device="cuda").manual_seed(6), device="cuda").bfloat16()
     work, spans, tok = [], [], 0
@@ -305,10 +304,8 @@ def test_peaky_attention_at_production_shape(kernel):
         got = ops.paged_attn(q, kv, btab, wt, Hq, Hkv, decode=True)
     elif kernel == "decode_split_7":
         got = ops.paged_attn(q, kv, btab, wt, Hq, Hkv, decode=True, split=7)
-    elif kernel == "tensor_core":
-        got = ops.paged_attn_prefill_tc(q, kv, btab, wt, Hq, Hkv)
     else:
-        got = ops.paged_attn(q, kv, btab, wt, Hq, Hkv, decode=False)
+        got = ops.paged_attn_prefill_tc(q, kv, btab, wt, Hq, Hkv)
     got = got.float()
     torch.cuda.synchronize()
     for i, (L, n) in enumerate(case):

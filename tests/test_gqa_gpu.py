@@ -148,10 +148,11 @@ def test_chunked_prefill_attention_matches_oracle(G):
 
 
 @pytest.mark.parametrize("hq, hkv", [(2, 2), (6, 2), (8, 1), (16, 1)])
-def test_op_level_prefill_form_refuses_group_sizes_other_than_4(hq, hkv):
+def test_op_level_paged_attn_refuses_decode_0_and_uneven_groups(hq, hkv):
     q, kv, btab, work, _ = make_case([(0, 16)], hkv, hq // hkv, seed=1)
-    with pytest.raises(B200Error, match=r"prefill form \(decode = 0\) serves 4 query heads per KV head only"):
-        ops.paged_attn(q, kv, btab, work, hq, hkv, decode=False)
+    for head_dim in (None, 64, 128):
+        with pytest.raises(B200Error, match=r"decode = 0 is not served; chunked prefill is b200_op_paged_attn_prefill_tc"):
+            ops.paged_attn(q, kv, btab, work, hq, hkv, decode=False, head_dim=head_dim)
     with pytest.raises(B200Error, match="kv_heads must divide q_heads"):
         ops.paged_attn(q, kv, btab, work, 2 * hkv + 1 if hkv > 1 else 17, hkv, decode=True)
 

@@ -162,18 +162,10 @@ def test_hd_entry_points_at_128_give_the_bits_of_the_old_ones():
     b = ops.paged_attn_prefill_tc(q, kv, btab, work, G * Hkv, Hkv, head_dim=128)
     torch.cuda.synchronize()
     assert torch.equal(a.view(torch.int16), b.view(torch.int16))
-    # the op-level mma.sync prefill form (decode = 0)
-    q, kv, btab, work, _ = make_case([(0, 16), (40, 16)], Hkv, 4, seed=79, d=128)
-    a = ops.paged_attn(q, kv, btab, work, 8, Hkv, decode=False)
-    b = ops.paged_attn(q, kv, btab, work, 8, Hkv, decode=False, head_dim=128)
-    torch.cuda.synchronize()
-    assert torch.equal(a.view(torch.int16), b.view(torch.int16))
 
 
-def test_op_level_prefill_form_refuses_head_dim_64():
+def test_op_level_paged_attn_refuses_head_dim_96():
     q, kv, btab, work, _ = make_case([(0, 16)], 2, 4, seed=1)
-    with pytest.raises(B200Error, match=r"prefill form \(decode = 0\) serves head_dim 128 only"):
-        ops.paged_attn(q, kv, btab, work, 8, 2, decode=False, head_dim=64)
     with pytest.raises(B200Error, match="head_dim=96; 64 and 128 are served"):
         ops.paged_attn(q, kv, btab, work, 8, 2, decode=True, head_dim=96)
 
