@@ -6,7 +6,8 @@
 //
 //   b200serve --gpus 8 --model llama-3-8b [--model-dir /models/llama-3-8b] [--strategy PrefixHash] [--port 8000]
 //             [--speculative-config '{"method": "ngram", "num_speculative_tokens": 3, "prompt_lookup_max": 4}']
-//             [--runner generate|pooling]   (default: pooling for a LlamaModel / MistralModel directory, else generate)
+//             [--runner generate|pooling]   (default: pooling for a LlamaModel / MistralModel directory and for a
+//                                            *ForSequenceClassification one, which serves /v1/rerank; else generate)
 #include <signal.h>
 #include <stdio.h>
 #include <stdlib.h>

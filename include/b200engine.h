@@ -85,9 +85,22 @@ typedef struct {
   /* sliding-window attention span of the checkpoint (Mistral's sliding_window), 0 = none.  The kernels attend to the whole
    * context, which inside the window is the same attention: b200_engine_create refuses max_model_len > sliding_window. */
   int32_t sliding_window;
+  /* score head (vLLM's pooling runner on a *ForSequenceClassification checkpoint): 0 = none, the pooling runner serves
+   * embeddings; 1..B200_MAX_SCORE_LABELS = a score weight [num_labels, hidden] ("score") applied to the final-normed last
+   * position in fp32, requests submitted with b200_submit_score.  Needs runner = pooling; no lm_head is allocated. */
+  int32_t num_labels;
+  /* the activation a score request gets when it asks for one (vLLM's PoolerClassify / get_act_fn): 0 = by label count
+   * (sigmoid at 1 label, softmax over the labels above), 1 = sigmoid, 2 = softmax, 3 = none (regression) */
+  int32_t score_activation;
+  /* how the serving shell tokenizes a (query, document) pair for a score head: 0 = the tokenizer's pair template (vLLM's
+   * use_sep_token = true, its default), 1 = its single template over the text query + document (use_sep_token = false).
+   * b200_config_from_hf sets it from config.json; the engine itself does not read it. */
+  int32_t score_join_pair;
 } b200_config;
 
 enum { B200_RUNNER_GENERATE = 0, B200_RUNNER_POOLING = 1 };
+/* labels a score head may have: one warp applies the activation, lane l holding logit l */
+#define B200_MAX_SCORE_LABELS 32
 
 /* drafts per step at most: a verify item's G query heads times its 1 + m positions share decode attention's 16-row tile,
  * so 3 drafts fill it at G = 4 and fewer fit at larger G (k_max(G) above) */
@@ -191,6 +204,15 @@ int b200_submit_embed(b200_engine* e, const int32_t* ids, int32_t n, int32_t nor
  * out[0..dim) gets the vector (dim must be the model's hidden size, else B200_ERR_INVALID).  usage: prompt and cached
  * tokens, completion_tokens 0. */
 int b200_poll_embedding(b200_engine* e, uint64_t req_id, float* out, int32_t dim, int32_t* finished, b200_usage* usage);
+/* Score head only (num_labels > 0; such an engine refuses b200_submit_embed, and an embedding or generate engine refuses
+ * this call, with B200_ERR_INVALID): one score request of 1..max_model_len prompt ids (a cross-encoder's tokenized pair).
+ * It is scheduled, chunked and prefix-cached like an embedding request and finishes (B200_FINISH_STOP) at the step that
+ * computes its last position.  use_activation != 0: the logits get the engine's score_activation, else they are the raw
+ * fp32 logits. */
+int b200_submit_score(b200_engine* e, const int32_t* ids, int32_t n, int32_t use_activation, uint64_t* req_id);
+/* The scores of a b200_submit_score request: *finished gets a B200_FINISH_* code or 0, and once it is B200_FINISH_STOP
+ * out[0..num_labels) gets them (num_labels must be the engine's, else B200_ERR_INVALID).  usage as b200_poll_embedding. */
+int b200_poll_score(b200_engine* e, uint64_t req_id, float* out, int32_t num_labels, int32_t* finished, b200_usage* usage);
 /* Drain newly generated token ids (at most cap).  *finished gets a B200_FINISH_* code or 0. */
 int b200_poll(b200_engine* e, uint64_t req_id, int32_t* out_ids, int32_t cap, int32_t* n_out, int32_t* finished,
               b200_usage* usage);
@@ -255,7 +277,7 @@ int b200_engine_profile_range(b200_engine* e, int32_t n, int32_t min_tokens, int
 /* Drop every cached prefix block (after a replay, which clobbers KV contents). */
 int b200_engine_reset_prefix_cache(b200_engine* e);
 
-/* Weights / buffers by name ("embed", "lm_head", "final_norm", "layers.<i>.{wqkv,wo,wgu,wdown,norm1,norm2}",
+/* Weights / buffers by name ("embed", "lm_head", "final_norm", "score", "layers.<i>.{wqkv,wo,wgu,wdown,norm1,norm2}",
  * "cos_sin").  Tests copy weights out for the CPU oracle or write their own in. */
 int b200_engine_tensor_info(b200_engine* e, const char* name, uint64_t* num_bytes, void** device_ptr);
 int b200_engine_tensor_read(b200_engine* e, const char* name, void* host_dst, uint64_t cap);
@@ -441,6 +463,13 @@ int32_t b200_tokenizer_token_id(const b200_tokenizer* t, const char* content);  
  * allow_special: added / special tokens spelled in the text become their ids (as HF `encode` does). */
 int64_t b200_tokenizer_encode(const b200_tokenizer* t, const char* text, size_t len, int32_t allow_special, int32_t* ids, size_t cap);
 int64_t b200_tokenizer_decode(const b200_tokenizer* t, const int32_t* ids, size_t n, int32_t skip_special, char* buf, size_t cap);
+/* A score pair's ids, as vLLM tokenizes (query a, document b) for a cross-encoder: join 0 = HF tokenizer(text=a,
+ * text_pair=b), the tokenizer.json's TemplateProcessing "pair" template (b200_config.score_join_pair 0, vLLM's
+ * use_sep_token = true); join 1 = tokenizer(text=a + b), its "single" template (use_sep_token = false).  Without a template
+ * in the file, or with add_special_tokens 0, the encodings are concatenated without special tokens.  Returns the full
+ * count (may exceed cap), -1 on bad arguments. */
+int64_t b200_tokenizer_encode_pair(const b200_tokenizer* t, const char* a, size_t alen, const char* b, size_t blen,
+                                   int32_t join, int32_t add_special_tokens, int32_t* ids, size_t cap);
 /* Incremental detokenisation of a generated stream: a token may end inside a UTF-8 sequence, so push returns only complete text
  * (id < 0 flushes what is held).  The pushes concatenated equal b200_tokenizer_decode of all ids. */
 typedef struct b200_detok_stream b200_detok_stream;
@@ -514,6 +543,15 @@ int b200_op_rmsnorm(const void* x, void* residual, const void* w, void* out, con
  * H <= 8192; row_index and flags are device int32 [rows]. */
 int b200_op_pool_rows(const void* hidden, const void* w, const int32_t* row_index, const int32_t* flags, int32_t rows,
                       int32_t H, float eps, float* out, void* stream);
+/* A score head's tail, as a score-head engine runs it on its pooled rows: out[s, 0..num_labels) (fp32 [rows, num_labels],
+ * device) = the logits score_w [num_labels, H] . y, y the final RMSNorm (weight norm_w, eps) of bf16 row row_index[s] of
+ * hidden, bit-identical in bf16 to b200_op_rmsnorm over the same rows; fp32 sums in a fixed order (per label each thread's
+ * FMAs in visit order, then the warp sums in warp order).  flags[s] != 0 then applies `activation` (b200_config's
+ * score_activation: 0 by label count, 1 sigmoid, 2 softmax, 3 none).  H % 256 == 0 and H <= 8192, 1 <= num_labels <=
+ * B200_MAX_SCORE_LABELS; row_index and flags are device int32 [rows]. */
+int b200_op_score_rows(const void* hidden, const void* norm_w, const void* score_w, const int32_t* row_index,
+                       const int32_t* flags, int32_t rows, int32_t H, int32_t num_labels, int32_t activation, float eps,
+                       float* out, void* stream);
 int b200_op_rope_kvwrite(void* qkv, const int32_t* positions, const int32_t* slots, const void* cos_sin,
                          void* kv_layer, int32_t T, int32_t q_heads, int32_t kv_heads, int32_t max_pos, void* stream);
 /* b200_op_rope_kvwrite at head size head_dim = 64 or 128: qkv rows of (q_heads + 2 * kv_heads) * head_dim, cos_sin rows of

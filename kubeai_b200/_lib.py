@@ -31,6 +31,7 @@ class Config(C.Structure):
         ("rope_high_freq_factor", C.c_float), ("rope_original_max_pos", C.c_int32),
         ("num_speculative_tokens", C.c_int32), ("prompt_lookup_min", C.c_int32), ("prompt_lookup_max", C.c_int32),
         ("head_dim", C.c_int32), ("runner", C.c_int32), ("sliding_window", C.c_int32),
+        ("num_labels", C.c_int32), ("score_activation", C.c_int32), ("score_join_pair", C.c_int32),
     ]
 
 
@@ -145,6 +146,8 @@ SYMBOLS = {
     "b200_poll_prompt_logprobs": (C.c_int, [_vp, _u64, _vp, _pi32, _pi32, _vp, _i32, _pi32]),
     "b200_submit_embed": (C.c_int, [_vp, _pi32, _i32, _i32, C.POINTER(_u64)]),
     "b200_poll_embedding": (C.c_int, [_vp, _u64, _vp, _i32, _pi32, C.POINTER(Usage)]),
+    "b200_submit_score": (C.c_int, [_vp, _pi32, _i32, _i32, C.POINTER(_u64)]),
+    "b200_poll_score": (C.c_int, [_vp, _u64, _vp, _i32, _pi32, C.POINTER(Usage)]),
     "b200_submit_n": (C.c_int, [_vp, _pi32, _i32, C.POINTER(Sampling), _i32, C.POINTER(_u64)]),
     "b200_wait": (C.c_int, [_vp, _u64, _i64]),
     "b200_wait_any": (C.c_int, [_vp, C.POINTER(_u64), _i32, _i64]),
@@ -209,6 +212,7 @@ SYMBOLS = {
     "b200_op_embed": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "b200_op_rmsnorm": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _f, _vp]),
     "b200_op_pool_rows": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _f, _vp, _vp]),
+    "b200_op_score_rows": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f, _vp, _vp]),
     "b200_op_rope_kvwrite": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
     "b200_op_rope_kvwrite_hd": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
     "b200_op_silu_mul": (C.c_int, [_vp, _vp, _i32, _i32, _vp]),
@@ -227,6 +231,8 @@ SYMBOLS = {
     "b200_tokenizer_token_id": (C.c_int32, [C.c_void_p, C.c_char_p]),
     "b200_tokenizer_encode": (C.c_int64, [C.c_void_p, C.c_char_p, C.c_size_t, _i32, _vp, C.c_size_t]),
     "b200_tokenizer_decode": (C.c_int64, [C.c_void_p, _vp, C.c_size_t, _i32, C.c_char_p, C.c_size_t]),
+    "b200_tokenizer_encode_pair": (C.c_int64, [C.c_void_p, C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t, _i32, _i32, _vp,
+                                               C.c_size_t]),
     "b200_tokenizer_stream_new": (C.c_void_p, [C.c_void_p, _i32]),
     "b200_tokenizer_stream_free": (None, [C.c_void_p]),
     "b200_tokenizer_stream_push": (C.c_int64, [C.c_void_p, _i32, C.c_char_p, C.c_size_t]),

@@ -233,6 +233,22 @@ int b200_op_pool_rows(const void* hidden, const void* w, const int32_t* row_inde
   return rc ? cuda_fail("pool_rows", rc) : 0;
 }
 
+int b200_op_score_rows(const void* hidden, const void* norm_w, const void* score_w, const int32_t* row_index,
+                       const int32_t* flags, int32_t rows, int32_t H, int32_t num_labels, int32_t activation, float eps,
+                       float* out, void* stream) {
+  if (int rc = require_device()) return rc;
+  if (rows < 0 || H % 256 || H <= 0 || H > 8192 || num_labels < 1 || num_labels > kMaxScoreLabels || activation < 0 ||
+      activation > kScoreNone || (rows > 0 && (!hidden || !norm_w || !score_w || !row_index || !flags || !out))) {
+    set_error("b200_op_score_rows: bad arguments (rows %d, H %d, num_labels %d, activation %d: H %% 256 == 0 and <= 8192, "
+              "1 <= num_labels <= %d, activation 0..3)", rows, H, num_labels, activation, kMaxScoreLabels);
+    return B200_ERR_INVALID;
+  }
+  const int act = activation ? activation : (num_labels == 1 ? kScoreSigmoid : kScoreSoftmax);
+  int rc = score_rows(hidden, nullptr, norm_w, score_w, row_index, flags, rows, H, num_labels, act, eps, out,
+                      static_cast<cudaStream_t>(stream));
+  return rc ? cuda_fail("score_rows", rc) : 0;
+}
+
 int b200_op_rope_kvwrite(void* qkv, const int32_t* positions, const int32_t* slots, const void* cos_sin,
                          void* kv_layer, int32_t T, int32_t q_heads, int32_t kv_heads, int32_t max_pos,
                          void* stream) {

@@ -222,7 +222,8 @@ struct Seq {
   std::shared_ptr<WaitGroup> group;
   // speculative decoding (engine thread): the drafts proposed for the step being launched (Sched::n_draft of them)
   std::vector<int32_t> draft;
-  // pooling runner (b200_submit_embed): the request's last position is pooled, L2-normalised when `normalize`; its vector
+  // pooling runner (b200_submit_embed, or b200_submit_score on a score head): the request's last position is pooled,
+  // L2-normalised (or, on a score head, its logits activated) when `normalize`; its vector (the logits on a score head)
   // is written by the engine thread before the finish code is published, and read by API threads once finished
   bool embed = false;
   bool normalize = true;
@@ -397,6 +398,9 @@ struct Engine {
   int L, H, Hq, Hkv, I, V, QKV;
   int Dh = 128;   // head size: 64 or 128 (b200_config.head_dim)
   bool pooling = false;   // b200_config.runner == B200_RUNNER_POOLING: no lm_head, pooled rows instead of sampled ones
+  // score head (pooling runner, b200_config.num_labels > 0): labels L and the activation resolved from score_activation
+  int num_labels = 0, score_act = 0;
+  int pooled_width() const { return num_labels > 0 ? num_labels : H; }   // floats per pooled row: the vector or the logits
   // n-gram speculative decoding: drafts per decoding sequence (0 = off) and the lookup n-gram lengths
   int spec_k = 0, spec_min = 0, spec_max = 0;
   int Tcap, Scap, max_blocks_per_seq;
@@ -411,6 +415,7 @@ struct Engine {
   };
   std::vector<Layer> layers;
   bf16 *embed = nullptr, *lm_head = nullptr, *final_norm = nullptr, *cos_sin = nullptr;
+  bf16* score = nullptr;   // score head [num_labels, H] (num_labels > 0)
   GemmPlan p_lm;
   bf16* weights_blob = nullptr;
   size_t weights_bytes = 0;
@@ -428,7 +433,7 @@ struct Engine {
   int *lp_ids_dev = nullptr, *plp_ids_dev = nullptr, *plp_rank_dev = nullptr;
   int32_t *sampled_host = nullptr, *lp_ids_host = nullptr, *plp_ids_host = nullptr, *plp_rank_host = nullptr;
   float *lp_host = nullptr, *plp_f_host = nullptr;
-  float *pooled = nullptr, *pooled_host = nullptr;   // per pooled row its fp32 vector [H] (pooling runner)
+  float *pooled = nullptr, *pooled_host = nullptr;   // per pooled row its fp32 vector [H] or logits [L] (pooling runner)
   template <class F>
   void for_each_readback(size_t S, size_t n_lp, size_t n_plp, size_t E, F fn) {
     const size_t rec = (1 + kMaxLogprobs) * sizeof(float), ids = kMaxLogprobs * sizeof(int32_t);
@@ -438,7 +443,7 @@ struct Engine {
     fn(plp_f_dev, plp_f_host, n_plp * rec);
     fn(plp_ids_dev, plp_ids_host, n_plp * ids);
     fn(plp_rank_dev, plp_rank_host, n_plp * sizeof(int32_t));
-    fn(pooled, pooled_host, E * H * sizeof(float));
+    fn(pooled, pooled_host, E * pooled_width() * sizeof(float));
   }
   int alloc_readbacks(int S, int n_lp, int n_plp, int E);
   // record i of the token (prompt = false) or prompt-logprob readbacks
@@ -684,6 +689,7 @@ int Engine::alloc_all() {
     items.push_back({p + "norm2", static_cast<size_t>(H), &layers[l].norm2, 0.1f, 1.0f});
   }
   items.push_back({"final_norm", static_cast<size_t>(H), &final_norm, 0.1f, 1.0f});
+  if (num_labels > 0) items.push_back({"score", static_cast<size_t>(num_labels) * H, &score, s_h, 0.f});
   if (!pooling)   // a pooling engine never runs the lm_head
     items.push_back({"lm_head", static_cast<size_t>(V) * H, &lm_head, s_h * (cfg.init_scale > 0 ? cfg.init_scale : 4.0f), 0.f});
   size_t total = 0;
@@ -883,6 +889,9 @@ int Engine::init(const b200_config& c) {
   L = c.num_layers; H = c.hidden; Hq = c.q_heads; Hkv = c.kv_heads; I = c.intermediate; V = c.vocab;
   if (int rc = head_dim_resolve(c, &Dh)) return rc;
   pooling = c.runner == B200_RUNNER_POOLING;
+  num_labels = c.num_labels;
+  // vLLM's PoolerClassify default: sigmoid for one label, softmax for more
+  score_act = c.score_activation ? c.score_activation : (num_labels == 1 ? kScoreSigmoid : kScoreSoftmax);
   QKV = (Hq + 2 * Hkv) * Dh;
   // the constraints of every kernel the forward launches, checked here so that a bad shape fails at create time with a
   // message instead of poisoning the replica at its first step: RMSNorm rows are 256-element multiples up to 8192,
@@ -1047,12 +1056,16 @@ int Engine::forward(const StepMeta& m, int32_t* dbuf, bool all_logits, bf16* log
       launched(1);
     }
   }
-  // pooled rows: the gathered final norm and the L2 normalisation in one launch, into the pooled readback.  Only scratch
-  // is written, so a replay changes nothing a later step reads.
+  // pooled rows: the gathered final norm and the L2 normalisation (on a score head: the score logits and their
+  // activation) in one launch, into the pooled readback.  Only scratch is written, so a replay changes nothing a later
+  // step reads.
   if (!all_logits && m.E > 0) {
     const int* prow = dbuf + m.off_pool;
+    const bf16* px = x_pending ? x : res;
+    bf16* pres = x_pending ? res : nullptr;
     P(B200_K_NORM);
-    if (!x_pending) rc |= pool_rows(res, nullptr, final_norm, prow, prow + m.E, m.E, H, cfg.rms_eps, pooled, stream);
+    if (num_labels > 0) rc |= score_rows(px, pres, final_norm, score, prow, prow + m.E, m.E, H, num_labels, score_act, cfg.rms_eps, pooled, stream);
+    else if (!x_pending) rc |= pool_rows(res, nullptr, final_norm, prow, prow + m.E, m.E, H, cfg.rms_eps, pooled, stream);
     else rc |= pool_rows(x, res, final_norm, prow, prow + m.E, m.E, H, cfg.rms_eps, pooled, stream);
     Q();
     launched(1);
@@ -1628,10 +1641,10 @@ int Engine::complete(InFlight& f, const StepMeta& m, b200_step_info* info) {
       continue;
     }
     if (s.embed) {   // pooled rows come back in step order; the request finishes with its vector
-      const float* v = pooled_host + static_cast<size_t>(ei++) * H;
+      const float* v = pooled_host + static_cast<size_t>(ei++) * pooled_width();
       {
         std::lock_guard<std::mutex> lk(s.m);
-        s.embedding.assign(v, v + H);
+        s.embedding.assign(v, v + pooled_width());
       }
       pending_pub.push_back({sp, 0, false, B200_FINISH_STOP});
       release_blocks(s);
@@ -1920,6 +1933,18 @@ int b200_engine_create(const b200_config* cfg, b200_engine** out) {
     set_error("runner must be 0 (generate) or 1 (pooling), got %d", cfg->runner);
     return B200_ERR_INVALID;
   }
+  if (cfg->num_labels < 0 || cfg->num_labels > kMaxScoreLabels) {
+    set_error("num_labels %d is not supported: a score head has 1 to %d labels (0 = none)", cfg->num_labels, kMaxScoreLabels);
+    return B200_ERR_INVALID;
+  }
+  if (cfg->num_labels > 0 && cfg->runner != B200_RUNNER_POOLING) {
+    set_error("a score head (num_labels = %d) needs the pooling runner", cfg->num_labels);
+    return B200_ERR_INVALID;
+  }
+  if (cfg->score_activation < 0 || cfg->score_activation > kScoreNone) {
+    set_error("score_activation must be 0 (default), 1 (sigmoid), 2 (softmax) or 3 (none), got %d", cfg->score_activation);
+    return B200_ERR_INVALID;
+  }
   if (cfg->runner == B200_RUNNER_POOLING && cfg->num_speculative_tokens > 0) {
     set_error("speculative decoding (num_speculative_tokens=%d) needs the generate runner", cfg->num_speculative_tokens);
     return B200_ERR_INVALID;
@@ -2034,10 +2059,15 @@ static int submit_impl(b200_engine* e, const int32_t* prompt_ids, int32_t n, con
   return 0;
 }
 
-int b200_submit_embed(b200_engine* e, const int32_t* ids, int32_t n, int32_t normalize, uint64_t* req_id) {
-  if (!e || !ids || n <= 0 || !req_id) { set_error("b200_submit_embed: bad arguments"); return B200_ERR_INVALID; }
+// b200_submit_embed and b200_submit_score: one prefill-only request whose last position is pooled
+static int submit_pooled(b200_engine* e, const int32_t* ids, int32_t n, int32_t flag, uint64_t* req_id, bool score) {
+  const char* fn = score ? "b200_submit_score" : "b200_submit_embed";
+  if (!e || !ids || n <= 0 || !req_id) { set_error("%s: bad arguments", fn); return B200_ERR_INVALID; }
   Engine& g = e->impl;
-  if (!g.pooling) { set_error("this engine runs the generate runner: embedding requests need an engine created with runner = pooling"); return B200_ERR_INVALID; }
+  if (!g.pooling && !score) { set_error("this engine runs the generate runner: embedding requests need an engine created with runner = pooling"); return B200_ERR_INVALID; }
+  if (!g.pooling) { set_error("this engine runs the generate runner: score requests need an engine created with runner = pooling and num_labels > 0"); return B200_ERR_INVALID; }
+  if (score && g.num_labels == 0) { set_error("this engine has no score head (num_labels = 0): it serves embeddings, submitted with b200_submit_embed"); return B200_ERR_INVALID; }
+  if (!score && g.num_labels > 0) { set_error("this engine has a score head (num_labels = %d): submit score requests with b200_submit_score", g.num_labels); return B200_ERR_INVALID; }
   if (n > g.cfg.max_model_len) { set_error("prompt (%d tokens) exceeds max_model_len %d", n, g.cfg.max_model_len); return B200_ERR_INVALID; }
   for (int i = 0; i < n; ++i)
     if (ids[i] < 0 || ids[i] >= g.V) { set_error("token id %d out of range [0, %d)", ids[i], g.V); return B200_ERR_INVALID; }
@@ -2047,7 +2077,7 @@ int b200_submit_embed(b200_engine* e, const int32_t* ids, int32_t n, int32_t nor
   s->arrival_key = xxh64(ids, static_cast<size_t>(n) * sizeof(int32_t), 0);
   s->max_tokens = 0;
   s->embed = true;
-  s->normalize = normalize != 0;
+  s->normalize = flag != 0;
   {
     std::lock_guard<std::mutex> lk(g.mu_);
     if (g.fatal) { set_error("engine is in a failed state"); return B200_ERR_CUDA; }
@@ -2060,8 +2090,19 @@ int b200_submit_embed(b200_engine* e, const int32_t* ids, int32_t n, int32_t nor
   return 0;
 }
 
-int b200_poll_embedding(b200_engine* e, uint64_t req_id, float* out, int32_t dim, int32_t* finished, b200_usage* usage) {
-  if (!e || !finished) { set_error("b200_poll_embedding: bad arguments"); return B200_ERR_INVALID; }
+int b200_submit_embed(b200_engine* e, const int32_t* ids, int32_t n, int32_t normalize, uint64_t* req_id) {
+  return submit_pooled(e, ids, n, normalize, req_id, false);
+}
+
+int b200_submit_score(b200_engine* e, const int32_t* ids, int32_t n, int32_t use_activation, uint64_t* req_id) {
+  return submit_pooled(e, ids, n, use_activation, req_id, true);
+}
+
+// b200_poll_embedding (dim = H) and b200_poll_score (dim = num_labels)
+static int poll_pooled(b200_engine* e, uint64_t req_id, float* out, int32_t dim, int32_t* finished, b200_usage* usage,
+                       bool score) {
+  const char* fn = score ? "b200_poll_score" : "b200_poll_embedding";
+  if (!e || !finished) { set_error("%s: bad arguments", fn); return B200_ERR_INVALID; }
   Engine& g = e->impl;
   std::shared_ptr<Seq> s;
   {
@@ -2070,11 +2111,17 @@ int b200_poll_embedding(b200_engine* e, uint64_t req_id, float* out, int32_t dim
     if (it != g.requests.end()) s = it->second;
   }
   if (!s) { set_error("unknown request %llu", static_cast<unsigned long long>(req_id)); return B200_ERR_NOT_FOUND; }
-  if (!s->embed) { set_error("request %llu is not an embedding request", static_cast<unsigned long long>(req_id)); return B200_ERR_INVALID; }
-  if (dim != g.H || !out) { set_error("b200_poll_embedding: dim %d != hidden size %d", dim, g.H); return B200_ERR_INVALID; }
+  if (!s->embed || score != (g.num_labels > 0)) {
+    set_error("request %llu is not %s request", static_cast<unsigned long long>(req_id), score ? "a score" : "an embedding");
+    return B200_ERR_INVALID;
+  }
+  if (dim != g.pooled_width() || !out) {
+    set_error("%s: dim %d != %s %d", fn, dim, score ? "num_labels" : "hidden size", g.pooled_width());
+    return B200_ERR_INVALID;
+  }
   std::lock_guard<std::mutex> lk(s->m);
   *finished = s->finished;
-  if (s->finished == B200_FINISH_STOP) memcpy(out, s->embedding.data(), static_cast<size_t>(g.H) * sizeof(float));
+  if (s->finished == B200_FINISH_STOP) memcpy(out, s->embedding.data(), static_cast<size_t>(dim) * sizeof(float));
   if (usage) {
     const int nc = s->n_cached.load();
     usage->prompt_tokens = s->n_prompt;
@@ -2082,6 +2129,14 @@ int b200_poll_embedding(b200_engine* e, uint64_t req_id, float* out, int32_t dim
     usage->completion_tokens = 0;
   }
   return 0;
+}
+
+int b200_poll_embedding(b200_engine* e, uint64_t req_id, float* out, int32_t dim, int32_t* finished, b200_usage* usage) {
+  return poll_pooled(e, req_id, out, dim, finished, usage, false);
+}
+
+int b200_poll_score(b200_engine* e, uint64_t req_id, float* out, int32_t num_labels, int32_t* finished, b200_usage* usage) {
+  return poll_pooled(e, req_id, out, num_labels, finished, usage, true);
 }
 
 int b200_submit(b200_engine* e, const int32_t* prompt_ids, int32_t n, const b200_sampling* sp, uint64_t* req_id) {
@@ -2461,6 +2516,8 @@ int b200_engine_read_logits(b200_engine* e, void* host_logits_bf16, int32_t rows
 }  // extern "C"
 
 int b200::engine_runner(const b200_engine* e) { return e->impl.pooling ? B200_RUNNER_POOLING : B200_RUNNER_GENERATE; }
+int b200::engine_num_labels(const b200_engine* e) { return e->impl.num_labels; }
+int b200::engine_score_join_pair(const b200_engine* e) { return e->impl.cfg.score_join_pair; }
 int b200::engine_hidden(const b200_engine* e) { return e->impl.H; }
 
 int b200::engine_relayout_gate_up(b200_engine* e, const char* name) {

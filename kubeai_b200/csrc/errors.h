@@ -14,4 +14,8 @@ int engine_relayout_gate_up(b200_engine* e, const char* name);
 // b200_config.runner and hidden size of an engine (the serving shell routes and sizes embeddings by them)
 int engine_runner(const b200_engine* e);
 int engine_hidden(const b200_engine* e);
+// b200_config.num_labels (0 = no score head) and score_join_pair of an engine (the serving shell routes /v1/rerank and
+// tokenizes its pairs by them)
+int engine_num_labels(const b200_engine* e);
+int engine_score_join_pair(const b200_engine* e);
 }

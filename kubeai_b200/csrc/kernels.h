@@ -19,6 +19,13 @@ int rmsnorm(const void* x, void* residual, const void* w, void* out, const int* 
 // flags[s] != 0.  H % 256 == 0 and H <= 8192; row_index and flags are device int arrays [rows].
 int pool_rows(const void* x, const void* residual, const void* w, const int* row_index, const int* flags, int rows, int H,
               float eps, float* out, cudaStream_t st);
+// A score head's tail (pooling.cu): out[s, 0..L) (fp32 [rows, L]) = the logits sw [L, H] . y of the same normed row y
+// as pool_rows, in fp32 in a fixed order, then, when flags[s] != 0, the activation act (kScore*: sigmoid, softmax over
+// the L logits, or none).  1 <= L <= kMaxScoreLabels: one warp applies the activation, lane l holding logit l.
+constexpr int kMaxScoreLabels = 32;
+enum { kScoreSigmoid = 1, kScoreSoftmax = 2, kScoreNone = 3 };
+int score_rows(const void* x, const void* residual, const void* w, const void* sw, const int* row_index, const int* flags,
+               int rows, int H, int L, int act, float eps, float* out, cudaStream_t st);
 // head_dim D = 64 or 128: qkv rows [(Hq + 2 Hkv) * D], cos_sin rows [D], kv_layer [block][2][Hkv][16][D]
 int rope_kv_write(void* qkv, const int* positions, const int* slots, const void* cos_sin, void* kv_layer,
                   int T, int Hq, int Hkv, int max_pos, cudaStream_t st, int head_dim = 128);

@@ -12,6 +12,7 @@
 #include <unistd.h>
 
 #include <math.h>
+#include <string.h>
 
 #include <map>
 #include <memory>
@@ -282,6 +283,51 @@ int b200_config_from_hf(const char* dir, b200_config* cfg) {
       return B200_ERR_INVALID;
     }
   }
+  // the runner (vLLM's --runner auto): a base model (LlamaModel, MistralModel) has no lm_head and serves embeddings; a
+  // *ForSequenceClassification model pools into its score head (vLLM's as_seq_cls_model).  Any other *For* head is refused
+  // by name rather than served as whatever the runner defaults to.
+  int runner = cfg->runner;
+  int num_labels = cfg->num_labels, score_activation = cfg->score_activation, score_join_pair = cfg->score_join_pair;
+  if (const JVal* ar = root.get("architectures"); ar && ar->type == JVal::Arr && !ar->arr.empty() && ar->arr[0].type == JVal::Str) {
+    const std::string& a = ar->arr[0].str;
+    auto ends_with = [&](const char* suf) { const size_t n = strlen(suf); return a.size() > n && a.compare(a.size() - n, n, suf) == 0; };
+    num_labels = 0;
+    score_activation = 0;
+    score_join_pair = 0;
+    if (a == "LlamaModel" || a == "MistralModel") {
+      runner = B200_RUNNER_POOLING;
+    } else if (ends_with("ForCausalLM")) {
+      runner = B200_RUNNER_GENERATE;
+    } else if (a == "LlamaForSequenceClassification" || a == "MistralForSequenceClassification") {
+      runner = B200_RUNNER_POOLING;
+      // HF PretrainedConfig: num_labels, else len(id2label), else 2
+      num_labels = 2;
+      if (const JVal* v = root.get("id2label"); v && v->type == JVal::Obj) num_labels = static_cast<int>(v->obj.size());
+      if (const JVal* v = root.get("num_labels"); v && v->type == JVal::Num) num_labels = static_cast<int>(v->num);
+      if (num_labels < 1 || num_labels > B200_MAX_SCORE_LABELS) {
+        set_error("%s with %d labels is not supported: a score head has 1 to %d labels (one warp applies the activation, "
+                  "lane l holding logit l)", a.c_str(), num_labels, B200_MAX_SCORE_LABELS);
+        return B200_ERR_INVALID;
+      }
+      // vLLM's get_act_fn / PoolerClassify: problem_type picks the activation, its absence the default by label count
+      if (const JVal* pt = root.get("problem_type"); pt && pt->type == JVal::Str) {
+        if (pt->str == "regression") score_activation = 3;
+        else if (pt->str == "single_label_classification") score_activation = num_labels == 1 ? 1 : 2;
+        else if (pt->str == "multi_label_classification") score_activation = 1;
+        else {
+          set_error("problem_type \"%s\" is not supported (regression, single_label_classification, "
+                    "multi_label_classification)", pt->str.c_str());
+          return B200_ERR_INVALID;
+        }
+      }
+      // vLLM's CrossEncoderIOProcessor: use_sep_token (default true) tokenizes (query, document) as a pair
+      if (const JVal* v = root.get("use_sep_token"); v && v->type == JVal::Bool) score_join_pair = v->b ? 0 : 1;
+    } else if (a.find("For") != std::string::npos) {
+      set_error("architecture %s is not supported (*ForCausalLM, LlamaModel, MistralModel, LlamaForSequenceClassification, "
+                "MistralForSequenceClassification)", a.c_str());
+      return B200_ERR_INVALID;
+    }
+  }
   // architecture switches the kernels do not implement are refused, not ignored.  Mistral is the Llama block with an
   // optional sliding window, which b200_engine_create bounds max_model_len by.
   if (const JVal* mt = root.get("model_type"); mt && mt->type == JVal::Str && mt->str != "llama" && mt->str != "mistral") {
@@ -295,13 +341,6 @@ int b200_config_from_hf(const char* dir, b200_config* cfg) {
       return B200_ERR_INVALID;
     }
     sliding_window = static_cast<int>(sw->num);
-  }
-  // the runner (vLLM's --runner auto): a base model (LlamaModel, MistralModel) has no lm_head and serves embeddings
-  int runner = cfg->runner;
-  if (const JVal* ar = root.get("architectures"); ar && ar->type == JVal::Arr && !ar->arr.empty() && ar->arr[0].type == JVal::Str) {
-    const std::string& a = ar->arr[0].str;
-    if (a == "LlamaModel" || a == "MistralModel") runner = B200_RUNNER_POOLING;
-    else if (a.size() > 11 && a.compare(a.size() - 11, 11, "ForCausalLM") == 0) runner = B200_RUNNER_GENERATE;
   }
   // the pooling type a sentence-transformers checkpoint declares (modules.json, then <Pooling module>/config.json, as
   // vLLM's get_pooling_config reads them), checked when the checkpoint pools: none declared = last token, the only mode
@@ -390,6 +429,9 @@ int b200_config_from_hf(const char* dir, b200_config* cfg) {
   cfg->head_dim = head_dim;
   cfg->runner = runner;
   cfg->sliding_window = sliding_window;
+  cfg->num_labels = num_labels;
+  cfg->score_activation = score_activation;
+  cfg->score_join_pair = score_join_pair;
   if (const JVal* e = root.get("eos_token_id"); e && e->type == JVal::Num) cfg->eos_token_id = static_cast<int>(e->num);
   return 0;
 }
@@ -415,6 +457,19 @@ int b200_engine_load_safetensors(b200_engine* e, const char* path) {
   LD(pre + "embed_tokens.weight", 0, V, H);
   if (dev("final_norm", &p, &nb)) return B200_ERR_NOT_FOUND;
   LD(pre + "norm.weight", 0, 1, H);
+  if (b200_engine_tensor_info(e, "score", &nb, &p) == 0) {   // a score head [num_labels, H], bf16 as loaded
+    const int64_t labels = static_cast<int64_t>(nb / 2) / H;
+    if (!ck.index.count("score.weight")) {
+      set_error("missing tensor score.weight: the engine has a score head of [%lld, %lld] (num_labels = %lld)",
+                static_cast<long long>(labels), static_cast<long long>(H), static_cast<long long>(labels));
+      return B200_ERR_NOT_FOUND;
+    }
+    LD("score.weight", 0, labels, H);
+  } else if (ck.index.count("score.weight") && !ck.index.count("lm_head.weight")) {
+    set_error("the checkpoint has a score head (score.weight) and no lm_head.weight: a sequence-classification model is "
+              "served by a pooling engine with num_labels > 0, not loaded as %s", b200_engine_tensor_info(e, "lm_head", &nb, &p) == 0 ? "a generator" : "an embedding model");
+    return B200_ERR_INVALID;
+  }
   if (b200_engine_tensor_info(e, "lm_head", &nb, &p) == 0) {   // a pooling engine has no lm_head
     // tie_word_embeddings: checkpoints without lm_head.weight reuse the embedding matrix
     const std::string head = ck.index.count("lm_head.weight") ? "lm_head.weight" : pre + "embed_tokens.weight";

@@ -55,6 +55,10 @@ struct Server {
   int max_n = 0;           // b200_server_config.max_n: >= 2 serves n up to it (else n > 1 is a 400)
   bool pooling = false;    // the replicas run the pooling runner: /v1/embeddings is served, the generation routes are not
   int hidden = 0;          // embedding size (pooling)
+  // the replicas' score head (b200_config.num_labels > 0): /v1/rerank is served, /v1/embeddings and generation are not;
+  // join_pair: b200_config.score_join_pair (pairs tokenized as query + document through the single template)
+  int num_labels = 0;
+  bool join_pair = false;
   // optional real tokenizer (b200_server_set_tokenizer): a checkpoint's tokenizer.json instead of the synthetic byte/word ids
   const b200_tokenizer* real_tok = nullptr;
 
@@ -159,6 +163,7 @@ int send_error(Writer& w, int status, const std::string& msg) {
 struct ParsedRequest {
   bool chat = true;
   bool embed = false;   // /v1/embeddings (the reference's EmbeddingRequest: no Prefix)
+  bool rerank = false;  // /v1/rerank on a score-head server (the reference's RerankRequest: no Prefix)
   std::string requested_model, model, adapter, prefix;
   std::vector<std::pair<std::string, std::string>> messages;
   std::vector<int32_t> prompt_ids;  // completions with token-id prompt
@@ -208,6 +213,7 @@ int parse_request(Server& sv, const std::string& path, const std::string& ctype,
   if (path == "/v1/chat/completions") pr->chat = true;
   else if (path == "/v1/completions") pr->chat = false;
   else if (path == "/v1/embeddings") pr->embed = true;
+  else if (path == "/v1/rerank" && sv.num_labels > 0) pr->rerank = true;
   else {
     *err = "bad request: reading model from body: unknown path: \"" + path + "\"";
     return 400;
@@ -217,6 +223,34 @@ int parse_request(Server& sv, const std::string& path, const std::string& ctype,
   if (!JParser(body, len).parse(&root, &jerr) || root.type != JVal::Obj) {
     *err = "bad request: reading model from body: decoding: " + (jerr.empty() ? std::string("expected JSON object") : jerr);
     return 400;
+  }
+  if (pr->rerank) {
+    // RerankRequest's typed fields, as Go decodes them (api/openai/v1/rerank.go): query a string, documents a list of
+    // strings, top_n an integer; null leaves a field at its zero value
+    auto type_name = [](const JVal& v) {
+      switch (v.type) {
+        case JVal::Bool: return "boolean";
+        case JVal::Num: return "number";
+        case JVal::Str: return "string";
+        case JVal::Arr: return "array";
+        case JVal::Obj: return "object";
+        default: return "null";
+      }
+    };
+    auto decoding = [&](const JVal& v, const char* go_type, const std::string& where) {
+      *err = std::string("bad request: reading model from body: decoding: json: cannot unmarshal JSON ") + type_name(v) +
+             " into Go " + go_type + " within \"" + where + "\"";
+      return 400;
+    };
+    if (const JVal* q = root.get("query"); q && q->type != JVal::Null && q->type != JVal::Str) return decoding(*q, "string", "/query");
+    if (const JVal* d = root.get("documents"); d && d->type != JVal::Null) {
+      if (d->type != JVal::Arr) return decoding(*d, "[]string", "/documents");
+      for (size_t i = 0; i < d->arr.size(); ++i)
+        if (d->arr[i].type != JVal::Str && d->arr[i].type != JVal::Null) return decoding(d->arr[i], "string", "/documents/" + std::to_string(i));
+    }
+    if (const JVal* t = root.get("top_n"); t && t->type != JVal::Null &&
+        (t->type != JVal::Num || t->num != std::floor(t->num) || std::fabs(t->num) > 9.2e18))
+      return decoding(*t, "int", "/top_n");
   }
   const JVal* m = root.get("model");
   if (!m || m->type != JVal::Str || m->str.empty()) {
@@ -233,7 +267,7 @@ int parse_request(Server& sv, const std::string& path, const std::string& ctype,
     *err = "model not found: \"" + pr->requested_model + "\"";
     return 404;
   }
-  if (pr->embed) return 0;   // its fields are read by serve_embeddings
+  if (pr->embed || pr->rerank) return 0;   // their fields are read by serve_embeddings / serve_rerank
   if (pr->chat) {
     const JVal* msgs = root.get("messages");
     if (msgs && msgs->type == JVal::Arr) {
@@ -1145,6 +1179,170 @@ static int serve_embeddings(Server& sv, const std::string& path, const std::stri
   }
 }
 
+// The pairs and options of a /v1/rerank body (vLLM 0.22's RerankRequest; its types were checked by parse_request).  Returns
+// 0 or 400 with *err set.  Every field the engine does not implement is refused, never dropped.
+struct RerankRequest {
+  std::vector<std::string> documents;
+  std::vector<std::vector<int32_t>> pairs;   // the tokenized (query, document i)
+  int top_n = 0;
+  bool use_activation = true;
+};
+static int parse_rerank_body(const Server& sv, const char* body, size_t len, RerankRequest* rr, std::string* err) {
+  JVal root;
+  std::string jerr;
+  if (!JParser(body, len).parse(&root, &jerr) || root.type != JVal::Obj) { *err = "bad request: expected a JSON object"; return 400; }
+  auto bad = [&](const std::string& m) { *err = "bad request: " + m; return 400; };
+  auto present = [&](const char* k) { const JVal* v = root.get(k); return v && v->type != JVal::Null; };
+  for (const char* k : {"max_tokens_per_query", "max_tokens_per_doc"})
+    if (const JVal* v = root.get(k); v && v->type != JVal::Null && !(v->type == JVal::Num && v->num == 0))
+      return bad(std::string(k) + " (per-document truncation) is not supported by this engine");
+  for (const char* k : {"truncate_prompt_tokens", "instruction", "chat_template_kwargs", "priority"})
+    if (present(k)) return bad(std::string(k) + " is not supported by this engine");
+  if (sv.num_labels != 1)   // vLLM's ScoringOutput.from_base: a rerank score is the one logit of its row
+    return bad("pooled_data should be a scalar score: /v1/rerank needs a score head of 1 label, this model has " +
+               std::to_string(sv.num_labels));
+  if (const JVal* v = root.get("use_activation"); v && v->type != JVal::Null) {
+    if (v->type != JVal::Bool) return bad("use_activation must be a boolean or null");
+    rr->use_activation = v->b;
+  }
+  bool special = true;
+  if (const JVal* v = root.get("add_special_tokens"); v && v->type != JVal::Null) {
+    if (v->type != JVal::Bool) return bad("add_special_tokens must be a boolean");
+    special = v->b;
+  }
+  if (const JVal* v = root.get("top_n"); v && v->type == JVal::Num)
+    rr->top_n = v->num > 2147483647.0 ? 2147483647 : v->num < -2147483648.0 ? -2147483647 - 1 : static_cast<int>(v->num);
+  std::string query;
+  if (const JVal* v = root.get("query"); v && v->type == JVal::Str) query = v->str;
+  if (const JVal* v = root.get("documents"); v && v->type == JVal::Arr)
+    for (auto& d : v->arr) rr->documents.push_back(d.type == JVal::Str ? d.str : "");
+  if (rr->documents.empty()) return bad("documents must not be empty");
+  for (auto& d : rr->documents) {
+    rr->pairs.emplace_back();
+    std::vector<int32_t>& ids = rr->pairs.back();
+    if (sv.real_tok) {
+      tokenizer_encode_pair(sv.real_tok, query, d, sv.join_pair, special, &ids);
+    } else {   // the synthetic tokenizer has no special tokens: the two encodings, concatenated
+      sv.tok.encode(sv.join_pair ? query + d : query, &ids);
+      if (!sv.join_pair) sv.tok.encode(d, &ids);
+    }
+    if (ids.empty()) return bad("the query and document must not both be empty");
+    // the embeddings route's message: vLLM 0.22 renderers/params.py _token_len_check with 0 output tokens
+    if (static_cast<int>(ids.size()) > sv.max_model_len) {
+      const std::string n = (static_cast<int>(ids.size()) == sv.max_model_len + 1 ? "at least " : "") + std::to_string(ids.size());
+      return bad("This model's maximum context length is " + std::to_string(sv.max_model_len) +
+                 " tokens. However, you requested 0 output tokens and your prompt contains " + n +
+                 " input tokens, for a total of " + n + " tokens. Please reduce the length of the input prompt or the number "
+                 "of requested output tokens.");
+    }
+  }
+  return 0;
+}
+
+// The shortest decimal that reads back as the same double (Python's float repr, which vLLM's JSON dump of a score
+// prints); the double holds the fp32 score exactly, so a client recovers the score to the bit.
+static std::string shortest_double(double v) {
+  char b[40];
+  for (int p = 1; p <= 17; ++p) {
+    snprintf(b, sizeof(b), "%.*g", p, v);
+    if (strtod(b, nullptr) == v) break;
+  }
+  return b;
+}
+
+// /v1/rerank on a score-head server: every (query, document) pair is one engine request, all submitted before any is
+// waited on; the response is vLLM's RerankResponse, results sorted by score (descending, stable: equal scores keep the
+// document order, as Python's sort(reverse=True) does) and cut to top_n when 0 < top_n < len(documents).  Retries and
+// the 499 of a client that went away follow serve_embeddings.
+static int serve_rerank(Server& sv, const std::string& path, const std::string& ctype, const char* body, size_t len,
+                        Writer& w) {
+  ParsedRequest pr;
+  std::string err;
+  if (int st = parse_request(sv, path, ctype, body, len, &pr, &err)) return send_error(w, st, err);
+  RerankRequest rr;
+  if (int st = parse_rerank_body(sv, body, len, &rr, &err)) return send_error(w, st, err);
+  {
+    std::lock_guard<std::mutex> lk(sv.mmu);
+    ++sv.active[pr.requested_model];
+  }
+  sv.requests_total.fetch_add(1);
+  struct Dec {
+    Server& s;
+    std::string m;
+    ~Dec() {
+      std::lock_guard<std::mutex> lk(s.mmu);
+      --s.active[m];
+    }
+  } dec{sv, pr.requested_model};
+  const size_t n_in = rr.pairs.size();
+  std::vector<uint64_t> tokens_held;
+  auto release_all = [&] {
+    for (auto t : tokens_held) b200_router_done(sv.router, t);
+    tokens_held.clear();
+  };
+  for (int attempt = 0;; ++attempt) {
+    char addr[64];
+    uint64_t ep_token = 0;
+    if (b200_router_pick(sv.router, sv.strategy, pr.adapter.c_str(), "", 0, sv.mean_load_pct, 30ll * 1000 * 1000, addr,
+                         sizeof(addr), &ep_token)) {
+      release_all();
+      sv.errors_total.fetch_add(1);
+      return send_error(w, 504, "request timeout while finding host");
+    }
+    tokens_held.push_back(ep_token);
+    const int replica = atoi(addr + 4);  // "gpu:<i>"
+    b200_engine* eng = sv.replicas[replica];
+    bool failed = false;
+    if (sv.faults[replica]->load() < 0) failed = true;
+    else if (sv.faults[replica]->load() > 0 && sv.faults[replica]->fetch_sub(1) > 0) failed = true;
+    std::vector<uint64_t> rids;
+    for (size_t i = 0; i < n_in && !failed; ++i) {
+      uint64_t rid = 0;
+      if (b200_submit_score(eng, rr.pairs[i].data(), static_cast<int>(rr.pairs[i].size()), rr.use_activation ? 1 : 0, &rid)) failed = true;
+      else rids.push_back(rid);
+    }
+    std::vector<float> scores(n_in);
+    std::vector<b200_usage> usage(n_in);
+    std::vector<int> fin(n_in, 0);
+    for (size_t i = 0; i < rids.size() && !failed;) {
+      if (fin[i]) { ++i; continue; }
+      b200_wait(eng, rids[i], 200000);
+      if (b200_poll_score(eng, rids[i], &scores[i], 1, &fin[i], &usage[i])) failed = true;
+      else if (fin[i] && fin[i] != B200_FINISH_STOP) failed = true;
+    }
+    for (auto r : rids) b200_release(eng, r);   // releasing an unfinished request (a failed attempt) aborts it
+    if (failed) {
+      if (b200_engine_is_failed(eng) || sv.faults[replica]->load() < 0) sv.drop_replica(replica);
+      if (attempt < sv.max_retries) {
+        sv.retries_total.fetch_add(1);
+        continue;
+      }
+      release_all();
+      sv.errors_total.fetch_add(1);
+      return send_error(w, 502, "proxy: exceeded retries");
+    }
+    release_all();
+    int prompt_tokens = 0;
+    for (auto& u : usage) prompt_tokens += u.prompt_tokens;
+    std::vector<size_t> order(n_in);
+    for (size_t i = 0; i < n_in; ++i) order[i] = i;
+    std::stable_sort(order.begin(), order.end(), [&](size_t a, size_t b) { return scores[a] > scores[b]; });
+    if (rr.top_n > 0 && static_cast<size_t>(rr.top_n) < n_in) order.resize(static_cast<size_t>(rr.top_n));
+    std::string out = "{\"id\":\"score-" + hex_id(32) + "\",\"model\":" + json_str(pr.requested_model) +
+                      ",\"usage\":{\"prompt_tokens\":" + std::to_string(prompt_tokens) + ",\"total_tokens\":" +
+                      std::to_string(prompt_tokens) + "},\"results\":[";
+    for (size_t k = 0; k < order.size(); ++k) {
+      const size_t i = order[k];
+      out += (k ? ",{\"index\":" : "{\"index\":") + std::to_string(i) + ",\"document\":{\"text\":" + json_str(rr.documents[i]) +
+             ",\"multi_modal\":null},\"relevance_score\":" + shortest_double(static_cast<double>(scores[i])) + "}";
+    }
+    out += "]}";
+    w.begin(200, "application/json");
+    w.write(out);
+    return w.gone ? 499 : 200;
+  }
+}
+
 static std::string metrics_text(Server& sv) {
   std::string o;
   o += "# HELP kubeai_inference_requests_active The number of active requests by model\n# TYPE kubeai_inference_requests_active gauge\n";
@@ -1217,7 +1415,7 @@ static int handle(Server& sv, const std::string& method, const std::string& full
   path = path.substr(7);  // http.StripPrefix("/openai", ...)
   if (path == "/v1/models" && method == "GET") {
     // openaiserver/models.go:13-77 (static: one model + adapters)
-    const std::string feat = sv.pooling ? "TextEmbedding" : "TextGeneration";
+    const std::string feat = sv.num_labels > 0 ? "Reranking" : sv.pooling ? "TextEmbedding" : "TextGeneration";
     std::string o = "{\"object\":\"list\",\"data\":[{\"id\":" + json_str(sv.model) + ",\"object\":\"model\",\"created\":0,\"owned_by\":\"kubeai-b200\",\"features\":[\"" + feat + "\"]}";
     for (auto& a : sv.adapters)
       o += ",{\"id\":" + json_str(sv.model + "_" + a) + ",\"object\":\"model\",\"created\":0,\"owned_by\":\"kubeai-b200\",\"features\":[\"" + feat + "\"]}";
@@ -1227,7 +1425,12 @@ static int handle(Server& sv, const std::string& method, const std::string& full
     return 200;
   }
   // "X-Proxy: lingo" (handler.go:60) is added by the HTTP layer below / by the Go shim
-  if (sv.pooling) {
+  if (sv.num_labels > 0) {
+    if (path == "/v1/rerank") return serve_rerank(sv, path, ctype, body, len, w);
+    if (path == "/v1/chat/completions" || path == "/v1/completions" || path == "/v1/embeddings" || path == "/v1/audio/transcriptions")
+      return send_error(w, 404, "model not found: this engine serves Reranking only");
+  }
+  if (sv.pooling && sv.num_labels == 0) {
     if (path == "/v1/embeddings") return serve_embeddings(sv, path, ctype, body, len, w);
     if (path == "/v1/chat/completions" || path == "/v1/completions" || path == "/v1/rerank" || path == "/v1/audio/transcriptions")
       return send_error(w, 404, "model not found: this engine serves TextEmbedding only");
@@ -1401,13 +1604,22 @@ int b200_server_create(const b200_server_config* cfg, b200_engine* const* replic
   for (int i = 0, seen = 0; i < n; ++i) {
     if (!replicas[i]) continue;
     const bool pool = engine_runner(replicas[i]) == B200_RUNNER_POOLING;
-    if (seen++ && pool != sv.pooling) {
+    if (seen && pool != sv.pooling) {
       delete s;
       set_error("b200_server_create: the replicas mix the generate and pooling runners");
       return B200_ERR_INVALID;
     }
+    // a server serves embeddings or one score head, never both
+    if (seen && (engine_num_labels(replicas[i]) != sv.num_labels || (engine_score_join_pair(replicas[i]) != 0) != sv.join_pair)) {
+      set_error("b200_server_create: the replicas mix heads (num_labels %d and %d)", sv.num_labels, engine_num_labels(replicas[i]));
+      delete s;
+      return B200_ERR_INVALID;
+    }
+    ++seen;
     sv.pooling = pool;
     sv.hidden = engine_hidden(replicas[i]);
+    sv.num_labels = engine_num_labels(replicas[i]);
+    sv.join_pair = engine_score_join_pair(replicas[i]) != 0;
   }
   if (b200_router_create(sv.replication, &sv.router)) { delete s; return B200_ERR_INVALID; }
   std::vector<std::string> names;

@@ -157,6 +157,15 @@ struct b200_tokenizer {
   std::unordered_map<uint32_t, uint8_t> cp_to_byte;
   int byte_symbol[256];                                          // id of the one-byte symbol
   int bos = -1, start_header = -1, end_header = -1, eot = -1;
+  // the TemplateProcessing post-processor (HF tokenizers processors/template.rs): per template, its pieces in order, each
+  // sequence A (0), sequence B (1) or a special token's ids (-1).  has_template false: none, so encodings are concatenated
+  // without special tokens.
+  struct TplPiece {
+    int seq;
+    std::vector<int32_t> ids;
+  };
+  bool has_template = false;
+  std::vector<TplPiece> tpl_single, tpl_pair;
 
   void bpe(const char* s, size_t n, std::vector<int32_t>* out) const;
   void encode_plain(const char* s, size_t n, std::vector<int32_t>* out) const;
@@ -271,6 +280,29 @@ void tokenizer_token_bytes(const b200_tokenizer* t, int32_t id, bool skip_specia
   }
 }
 int32_t tokenizer_bos(const b200_tokenizer* t) { return t ? t->bos : -1; }
+
+void tokenizer_encode_pair(const b200_tokenizer* t, const std::string& a, const std::string& b, bool join, bool special,
+                           std::vector<int32_t>* out) {
+  // HF tokenizer(text, text_pair) encodes each text on its own (added tokens in the text become their ids), then applies
+  // the post-processor; tokenizer(text) the same with the single template
+  std::vector<int32_t> enc[2];
+  if (join) {
+    const std::string ab = a + b;
+    t->encode(ab.data(), ab.size(), true, &enc[0]);
+  } else {
+    t->encode(a.data(), a.size(), true, &enc[0]);
+    t->encode(b.data(), b.size(), true, &enc[1]);
+  }
+  const auto& tpl = join ? t->tpl_single : t->tpl_pair;
+  if (!special || !t->has_template) {
+    for (auto& e : enc) out->insert(out->end(), e.begin(), e.end());
+    return;
+  }
+  for (const auto& p : tpl) {
+    const std::vector<int32_t>& src = p.seq < 0 ? p.ids : enc[p.seq];
+    out->insert(out->end(), src.begin(), src.end());
+  }
+}
 int32_t tokenizer_eot(const b200_tokenizer* t) { return t ? t->eot : -1; }
 
 namespace {
@@ -483,6 +515,47 @@ int b200_tokenizer_load(const char* path, b200_tokenizer** out) {
       if (a.first == s) return a.second;
     return -1;
   };
+  // post_processor: a TemplateProcessing, alone or inside a Sequence (Llama-3: Sequence[ByteLevel, TemplateProcessing]);
+  // any other processor adds no token ids to a byte-level BPE encoding and is ignored, as is the absence of one
+  {
+    const JVal* pp = root.get("post_processor");
+    const JVal* tp = nullptr;
+    if (pp && pp->type == JVal::Obj && pp->get("type") && pp->get("type")->str == "TemplateProcessing") tp = pp;
+    else if (pp && pp->type == JVal::Obj && pp->get("type") && pp->get("type")->str == "Sequence" && pp->get("processors") &&
+             pp->get("processors")->type == JVal::Arr)
+      for (const auto& q : pp->get("processors")->arr)
+        if (q.type == JVal::Obj && q.get("type") && q.get("type")->str == "TemplateProcessing") tp = &q;
+    if (tp) {
+      const JVal* specials = tp->get("special_tokens");
+      auto parse = [&](const char* key, std::vector<b200_tokenizer::TplPiece>* out) {
+        const JVal* arr = tp->get(key);
+        if (!arr || arr->type != JVal::Arr) return false;
+        for (const auto& piece : arr->arr) {
+          if (const JVal* sq = piece.get("Sequence")) {
+            const JVal* id = sq->get("id");
+            if (!id || id->type != JVal::Str || (id->str != "A" && id->str != "B")) return false;
+            out->push_back({id->str == "A" ? 0 : 1, {}});
+          } else if (const JVal* sp = piece.get("SpecialToken")) {
+            const JVal* id = sp->get("id");
+            const JVal* st = id && id->type == JVal::Str && specials ? specials->get(id->str.c_str()) : nullptr;
+            const JVal* ids = st ? st->get("ids") : nullptr;
+            if (!ids || ids->type != JVal::Arr) return false;
+            b200_tokenizer::TplPiece p{-1, {}};
+            for (const auto& v : ids->arr) {
+              if (v.type != JVal::Num || v.num < 0 || v.num >= static_cast<double>(t->id_to_token.size())) return false;
+              p.ids.push_back(static_cast<int32_t>(v.num));
+            }
+            out->push_back(std::move(p));
+          } else {
+            return false;
+          }
+        }
+        return true;
+      };
+      if (!parse("single", &t->tpl_single) || !parse("pair", &t->tpl_pair)) { delete t; return refuse("post_processor TemplateProcessing"); }
+      t->has_template = true;
+    }
+  }
   t->bos = find_added("<|begin_of_text|>");
   t->start_header = find_added("<|start_header_id|>");
   t->end_header = find_added("<|end_header_id|>");
@@ -507,6 +580,16 @@ int64_t b200_tokenizer_encode(const b200_tokenizer* t, const char* text, size_t 
   if (!t || (!text && len)) return -1;
   std::vector<int32_t> out;
   t->encode(text, len, allow_special != 0, &out);
+  for (size_t i = 0; i < out.size() && i < cap; ++i) ids[i] = out[i];
+  return static_cast<int64_t>(out.size());
+}
+
+int64_t b200_tokenizer_encode_pair(const b200_tokenizer* t, const char* a, size_t alen, const char* b, size_t blen,
+                                   int32_t join, int32_t add_special_tokens, int32_t* ids, size_t cap) {
+  if (!t || (!a && alen) || (!b && blen)) return -1;
+  std::vector<int32_t> out;
+  b200::tokenizer_encode_pair(t, std::string(a ? a : "", alen), std::string(b ? b : "", blen), join != 0,
+                              add_special_tokens != 0, &out);
   for (size_t i = 0; i < out.size() && i < cap; ++i) ids[i] = out[i];
   return static_cast<int64_t>(out.size());
 }

@@ -3,6 +3,7 @@
 #include <stdint.h>
 
 #include <string>
+#include <vector>
 
 struct b200_tokenizer;
 
@@ -14,6 +15,12 @@ void tokenizer_token_bytes(const b200_tokenizer* t, int32_t id, bool skip_specia
 // ids of the Llama-3 control tokens (-1 if the vocabulary lacks one)
 int32_t tokenizer_bos(const b200_tokenizer* t);
 int32_t tokenizer_eot(const b200_tokenizer* t);
+// a cross-encoder's (query a, document b) ids, as vLLM tokenizes a score pair: join false = HF tokenizer(text=a,
+// text_pair=b) through the tokenizer.json's pair template (use_sep_token = true), join true = tokenizer(text=a + b)
+// through its single template (use_sep_token = false).  special false (add_special_tokens = false), or a tokenizer.json
+// without a TemplateProcessing post-processor: the encodings are concatenated without special tokens.
+void tokenizer_encode_pair(const b200_tokenizer* t, const std::string& a, const std::string& b, bool join, bool special,
+                           std::vector<int32_t>* out);
 // one id decoded on its own, special tokens kept, invalid UTF-8 replaced by U+FFFD (HF tokenizer.decode([id]))
 std::string tokenizer_token_text(const b200_tokenizer* t, int32_t id);
 

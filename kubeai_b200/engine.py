@@ -146,17 +146,41 @@ class Engine:
                                           C.byref(u)))
         return (out if fin.value == 1 else None), FINISH[fin.value], (u.prompt_tokens, u.cached_tokens, u.completion_tokens)
 
+    def submit_score(self, prompt_ids, use_activation: bool = True) -> int:
+        """One score request (score head, b200_submit_score): the score logits of the last prompt position, with the
+        engine's activation when use_activation."""
+        ids = np.ascontiguousarray(prompt_ids, dtype=np.int32)
+        rid = C.c_uint64()
+        check(self._l.b200_submit_score(self._h, ids.ctypes.data_as(_PI32), len(ids), 1 if use_activation else 0,
+                                        C.byref(rid)))
+        return rid.value
+
+    def poll_score(self, rid: int):
+        """(scores float32 [num_labels] or None until finished, finish reason, usage) of a score request."""
+        out = np.zeros(max(self.cfg.num_labels, 1), dtype=np.float32)
+        fin, u = C.c_int32(), Usage()
+        check(self._l.b200_poll_score(self._h, rid, out.ctypes.data_as(C.c_void_p), self.cfg.num_labels, C.byref(fin),
+                                      C.byref(u)))
+        return (out if fin.value == 1 else None), FINISH[fin.value], (u.prompt_tokens, u.cached_tokens, u.completion_tokens)
+
+    def score(self, prompts, use_activation: bool = True, max_steps: int = 100000):
+        """Manual-step helper: submit every prompt as a score request, step until all are finished, return float32
+        [len(prompts), num_labels]."""
+        return self._run_pooled([self.submit_score(p, use_activation) for p in prompts], self.poll_score, max_steps)
+
     def embed(self, prompts, normalize: bool = True, max_steps: int = 100000):
         """Manual-step helper: submit every prompt, step until all are finished, return float32 [len(prompts), hidden]."""
-        rids = [self.submit_embed(p, normalize) for p in prompts]
+        return self._run_pooled([self.submit_embed(p, normalize) for p in prompts], self.poll_embedding, max_steps)
+
+    def _run_pooled(self, rids, poll, max_steps):
         vecs = [None] * len(rids)
         for _ in range(max_steps):
             ran, _info = self.step()
             for i, r in enumerate(rids):
                 if vecs[i] is None:
-                    v, fin, _u = self.poll_embedding(r)
+                    v, fin, _u = poll(r)
                     if fin is not None and v is None:
-                        raise RuntimeError(f"embedding request finished with {fin}")
+                        raise RuntimeError(f"pooled request finished with {fin}")
                     vecs[i] = v
             if all(v is not None for v in vecs):
                 break

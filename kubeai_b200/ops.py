@@ -107,6 +107,17 @@ def rmsnorm(x, w, eps, residual=None, row_index=None):
     return out
 
 
+def score_rows(hidden, norm_w, score_w, row_index, flags, activation=0, eps=1e-5):
+    """A score head's tail (b200_op_score_rows): fp32 [rows, L] logits score_w [L, H] . rmsnorm(hidden[row_index[s]]),
+    with the activation (0 by label count, 1 sigmoid, 2 softmax, 3 none) on the rows whose flag is set."""
+    _chk(hidden), _chk(norm_w), _chk(score_w), _chk(row_index, torch.int32), _chk(flags, torch.int32)
+    rows, (L, H) = row_index.numel(), score_w.shape
+    out = torch.empty(rows, L, dtype=torch.float32, device=hidden.device)
+    check(lib().b200_op_score_rows(_p(hidden), _p(norm_w), _p(score_w), _p(row_index), _p(flags), rows, H, L, activation, eps,
+                                   _p(out), _stream()))
+    return out
+
+
 def rope_kvwrite(qkv, positions, slots, cos_sin, kv_layer, q_heads, kv_heads, head_dim=None):
     """head_dim None: b200_op_rope_kvwrite (D = 128); 64 or 128: b200_op_rope_kvwrite_hd."""
     _chk(qkv), _chk(positions, torch.int32), _chk(slots, torch.int32), _chk(cos_sin), _chk(kv_layer)

@@ -38,6 +38,16 @@ class Tokenizer:
         self._l.b200_tokenizer_encode(self._h, b, len(b), 1 if allow_special else 0, buf, n)
         return list(buf[:n])
 
+    def encode_pair(self, query: str, document: str, join: bool = False, add_special_tokens: bool = True) -> list:
+        """A score pair's ids (b200_tokenizer_encode_pair): join False = HF tokenizer(text=query, text_pair=document),
+        True = tokenizer(text=query + document)."""
+        a, b = query.encode("utf-8"), document.encode("utf-8")
+        args = (self._h, a, len(a), b, len(b), 1 if join else 0, 1 if add_special_tokens else 0)
+        n = self._l.b200_tokenizer_encode_pair(*args, None, 0)
+        buf = (C.c_int32 * max(n, 1))()
+        self._l.b200_tokenizer_encode_pair(*args, buf, n)
+        return list(buf[:n])
+
     def decode(self, ids, skip_special: bool = False) -> str:
         arr = (C.c_int32 * max(len(ids), 1))(*ids)
         n = self._l.b200_tokenizer_decode(self._h, arr, len(ids), 1 if skip_special else 0, None, 0)

@@ -104,6 +104,29 @@ func (e *Engine) Embedding(id uint64, vec []float32) (finished int, u C.b200_usa
 	return int(fin), u, nil
 }
 
+// Score API (a pooling engine with num_labels > 0, a cross-encoder): one request per tokenized (query, document) pair;
+// Score blocks at most 200 ms and returns the scores (len = num_labels) once finished is B200_FINISH_STOP.
+func (e *Engine) SubmitScore(ids []int32, useActivation bool) (uint64, error) {
+	var id C.uint64_t
+	act := C.int32_t(0)
+	if useActivation {
+		act = 1
+	}
+	if rc := C.b200_submit_score(e.h, (*C.int32_t)(unsafe.Pointer(&ids[0])), C.int32_t(len(ids)), act, &id); rc != 0 {
+		return 0, errors.New(C.GoString(C.b200_last_error()))
+	}
+	return uint64(id), nil
+}
+
+func (e *Engine) Score(id uint64, scores []float32) (finished int, u C.b200_usage, err error) {
+	var fin C.int32_t
+	C.b200_wait(e.h, C.uint64_t(id), 200000)
+	if rc := C.b200_poll_score(e.h, C.uint64_t(id), (*C.float)(unsafe.Pointer(&scores[0])), C.int32_t(len(scores)), &fin, &u); rc != 0 {
+		return 0, u, errors.New(C.GoString(C.b200_last_error()))
+	}
+	return int(fin), u, nil
+}
+
 // SubmitN starts n parallel samples of one prompt (vLLM's n): one prefill, n request ids for Poll / Abort.
 func (e *Engine) SubmitN(prompt []int32, sp *C.b200_sampling, n int) ([]uint64, error) {
 	ids := make([]C.uint64_t, n)
