@@ -560,6 +560,10 @@ int b200_op_rope_kvwrite_hd(void* qkv, const int32_t* positions, const int32_t* 
                             void* kv_layer, int32_t T, int32_t q_heads, int32_t kv_heads, int32_t max_pos, int32_t head_dim,
                             void* stream);
 int b200_op_silu_mul(const void* gate_up, void* out, int32_t T, int32_t I, void* stream);
+/* out [T, I] = bf16(bf16(silu(gate)) * up) of gate_up [T, 2 I].  interleaved 0: each row is [gate | up]; 1: the engine's
+ * layout, 64 gate columns, their 64 up columns, the next 64 gate columns, ... (I % 64 == 0).  b200_op_silu_mul is this
+ * at 0. */
+int b200_op_silu_mul_il(const void* gate_up, void* out, int32_t T, int32_t I, int32_t interleaved, void* stream);
 int b200_op_argmax(const void* logits, int32_t* out, int32_t S, int32_t V, int32_t ld, void* stream);
 /* One sampled row's parameters, as the engine packs them into a step: temperature < 1e-5 = greedy; top_k <= 0 or >= V and
  * top_p <= 0 or >= 1 = off; the noise is Philox4x32-10 with key (seed_lo, seed_hi) and counter (v / 4, n, 0, 0), n = the

@@ -216,6 +216,7 @@ SYMBOLS = {
     "b200_op_rope_kvwrite": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
     "b200_op_rope_kvwrite_hd": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
     "b200_op_silu_mul": (C.c_int, [_vp, _vp, _i32, _i32, _vp]),
+    "b200_op_silu_mul_il": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _vp]),
     "b200_op_argmax": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _vp]),
     "b200_op_sample": (C.c_int, [_vp, _i32, _vp, _i32, _i32, _vp, _vp]),
     "b200_op_penalize": (C.c_int, [_vp, _i32, _i32, _i32, C.POINTER(PenaltyRow), _vp, _vp]),

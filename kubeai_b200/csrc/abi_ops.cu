@@ -269,8 +269,16 @@ int b200_op_rope_kvwrite_hd(void* qkv, const int32_t* positions, const int32_t* 
 }
 
 int b200_op_silu_mul(const void* gate_up, void* out, int32_t T, int32_t I, void* stream) {
+  return b200_op_silu_mul_il(gate_up, out, T, I, 0, stream);
+}
+
+int b200_op_silu_mul_il(const void* gate_up, void* out, int32_t T, int32_t I, int32_t interleaved, void* stream) {
   if (int rc = require_device()) return rc;
-  int rc = silu_mul(gate_up, out, T, I, static_cast<cudaStream_t>(stream));
+  if (interleaved && I % 64) {
+    set_error("b200_op_silu_mul_il: the interleaved layout needs I %% 64 == 0 (I = %d)", I);
+    return B200_ERR_INVALID;
+  }
+  int rc = silu_mul(gate_up, out, T, I, static_cast<cudaStream_t>(stream), interleaved);
   return rc ? cuda_fail("silu_mul", rc) : 0;
 }
 

@@ -209,13 +209,14 @@ __global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ qkv, const int* __res
 template <int VPT>  // uint4 output vectors per thread
 // interleaved != 0: gate and up columns alternate in 64-column blocks (the engine's gate_up weight rows are laid out
 // that way so that the decode GEMM's epilogue finds a gate row and its up row in one 128-row slab)
+// Tokens are on gridDim.x (up to 2^31 - 1): gridDim.y stops at 65535, fewer than a large prefill step can hold.
 __global__ void silu_mul_kernel(const __nv_bfloat16* __restrict__ gu, __nv_bfloat16* __restrict__ out, int I,
                                 int ldi, int interleaved) {
-  const int t = blockIdx.y;
+  const int t = blockIdx.x;
   const uint4* g = reinterpret_cast<const uint4*>(gu + static_cast<size_t>(t) * ldi);
   uint4* o = reinterpret_cast<uint4*>(out + static_cast<size_t>(t) * I);
   const int nvec = I / 8;
-  const int i0 = blockIdx.x * blockDim.x * VPT + threadIdx.x;
+  const int i0 = blockIdx.y * blockDim.x * VPT + threadIdx.x;
   float x[2 * VPT][8];  // gate vectors, then up vectors
   int n0[2 * VPT];
 #pragma unroll
@@ -401,9 +402,9 @@ int silu_mul(const void* gate_up, void* out, int T, int I, cudaStream_t st, int 
   __nv_bfloat16* o = static_cast<__nv_bfloat16*>(out);
   // decode: one output vector per thread (2 loads in flight); prefill bursts: two (4 batched loads in flight)
   if (T >= 512)
-    launch_pdl(silu_mul_kernel<2>, dim3((I / 8 + 511) / 512, T), dim3(256), 0, st, gu, o, I, 2 * I, interleaved);
+    launch_pdl(silu_mul_kernel<2>, dim3(T, (I / 8 + 511) / 512), dim3(256), 0, st, gu, o, I, 2 * I, interleaved);
   else
-    launch_pdl(silu_mul_kernel<1>, dim3((I / 8 + 255) / 256, T), dim3(256), 0, st, gu, o, I, 2 * I, interleaved);
+    launch_pdl(silu_mul_kernel<1>, dim3(T, (I / 8 + 255) / 256), dim3(256), 0, st, gu, o, I, 2 * I, interleaved);
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 

@@ -128,11 +128,13 @@ def rope_kvwrite(qkv, positions, slots, cos_sin, kv_layer, q_heads, kv_heads, he
         check(lib().b200_op_rope_kvwrite_hd(*args, head_dim, _stream()))
 
 
-def silu_mul(gu):
+def silu_mul(gu, interleaved=False):
+    """gu: [T, 2 I] as [gate | up], or with interleaved=True gate and up columns alternating in 64-column blocks (the
+    engine's layout)."""
     _chk(gu)
     T, I2 = gu.shape
     out = torch.empty(T, I2 // 2, dtype=torch.bfloat16, device=gu.device)
-    check(lib().b200_op_silu_mul(_p(gu), _p(out), T, I2 // 2, _stream()))
+    check(lib().b200_op_silu_mul_il(_p(gu), _p(out), T, I2 // 2, int(interleaved), _stream()))
     return out
 
 

@@ -10,6 +10,7 @@ import pytest
 import torch
 
 from embeddings_common import hidden_rows, pool, write_base_checkpoint, write_word_tokenizer
+from kernel_numerics import norm_launch, warp_sum
 from kubeai_b200 import B200Error, lib
 from kubeai_b200.engine import Engine, config_from_hf, mini_config
 from kubeai_b200._lib import BEGIN_FN, WRITE_FN, ResponseWriter
@@ -30,29 +31,20 @@ def _ulp(x):
     return np.spacing(np.abs(x).astype(np.float32)).astype(np.float64)
 
 
-def _warp_sum(v):
-    """__shfl_xor_sync butterfly over 32 fp32 lanes (offsets 16..1); every lane ends with the same value."""
-    v = v.astype(np.float32)
-    for o in (16, 8, 4, 2, 1):
-        v = (v + v[np.arange(32) ^ o]).astype(np.float32)
-    return v[0]
-
-
 def _kernel_normalize(y, rows):
     """pool_rows_kernel's normalisation of one bf16 row y (fp32 values) in its fixed order: the block size and vectors per
     thread that rmsnorm() picks for `rows` rows, each thread's squares summed in visit order (a bf16 square is exact in
     fp32, so the kernel's FMA is one rounded add), the warp butterflies, then the warp sums in warp order; IEEE sqrt and
     division."""
     H = y.size
-    vecs = H // 8
-    threads, vpt = (vecs, 1) if (rows < 512 or vecs % 256) else (256, vecs // 256)
+    threads, vpt = norm_launch(rows, H)
     acc = np.zeros(threads, np.float32)
     for i in range(vpt):
         for j in range(8):
             idx = (np.arange(threads) + i * threads) * 8 + j
             acc = (acc + (y[idx] * y[idx]).astype(np.float32)).astype(np.float32)
-    warps = np.array([_warp_sum(acc[k * 32:(k + 1) * 32]) for k in range(threads // 32)], np.float32)
-    ss = _warp_sum(np.concatenate([warps, np.zeros(32 - warps.size, np.float32)]))
+    warps = np.array([warp_sum(acc[k * 32:(k + 1) * 32]) for k in range(threads // 32)], np.float32)
+    ss = warp_sum(np.concatenate([warps, np.zeros(32 - warps.size, np.float32)]))
     return (y / np.maximum(np.sqrt(np.float32(ss)), np.float32(1e-12))).astype(np.float32)
 
 
@@ -88,7 +80,7 @@ def test_pool_rows_matches_rmsnorm_and_float64_normalize(H, n):
         # root halves that, and sqrt and the division add half an ulp each
         yd = y.astype(np.float64)
         want = yd / np.maximum(np.linalg.norm(yd, axis=1, keepdims=True), 1e-12)
-        vpt = 1 if (n < 512 or (H // 8) % 256) else H // 2048
+        vpt = norm_launch(n, H)[1]
         u = _ulp(want.astype(np.float32))
         bound = 0.5 * (8 * vpt + 10) * 2.0 ** -24 * np.abs(want) + u
         assert (np.abs(o - want) <= bound).all()

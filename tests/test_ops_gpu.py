@@ -100,25 +100,6 @@ def test_gemm_deferred_rejects_unaligned_output_rows():
         ops.gemm_deferred(dev(rnd(50, 256, seed=1)), dev(rnd(1004, 256, seed=2)))
 
 
-@pytest.mark.parametrize("rows,H", [(7, 512), (128, 4096), (3, 1024)])
-def test_rmsnorm(rows, H):
-    from kubeai_b200 import ops
-    x, w = rnd(rows, H, seed=5), rnd(H, scale=0.1, seed=6) + 1.0
-    w = O.r(w)
-    close(ops.rmsnorm(dev(x), dev(w), 1e-5), O.rms_norm(x, w, 1e-5), what="rmsnorm")
-    res = rnd(rows, H, seed=7)
-    dres = dev(res)
-    got = ops.rmsnorm(dev(x), dev(w), 1e-5, residual=dres)
-    want, want_res = O.fused_add_rms_norm(x, res, w, 1e-5)
-    close(got, want, what="fused add rmsnorm")
-    assert torch.equal(dres.float().cpu(), want_res), "residual must be bit-exact (one fp32 add, one rounding)"
-    idx = torch.tensor([rows - 1, 0], dtype=torch.int32).cuda()
-    dres2 = dev(res)
-    got = ops.rmsnorm(dev(x), dev(w), 1e-5, residual=dres2, row_index=idx)
-    close(got, want[[rows - 1, 0]], what="gathered rmsnorm")
-    assert torch.equal(dres2.float().cpu(), res), "row_index variant must not write the residual"
-
-
 def test_embed_silu_argmax():
     from kubeai_b200 import ops
     table = rnd(300, 512, seed=8)
@@ -141,32 +122,6 @@ def test_init_uniform_matches_numpy_replica():
         got = ops.init_uniform(n, seed, scale, off).float().cpu().numpy()
         want = bf16_bits_to_f32(np_init_uniform(n, seed, scale, off))
         assert np.array_equal(got, want), (n, seed)
-
-
-def test_rope_bit_exact():
-    """Same rounding sequence as the reference kernel (every bf16 op rounds): bit-exact."""
-    from kubeai_b200 import ops
-    from oracle.weights import ModelCfg, cos_sin_cache
-    g = torch.Generator().manual_seed(21)
-    Hq, Hkv, D, L = 8, 2, 128, 200
-    cs = O.r(torch.from_numpy(cos_sin_cache(ModelCfg(max_model_len=L))))
-    qkv = O.r(torch.randn(L, (Hq + 2 * Hkv) * D, generator=g))
-    pos = torch.randperm(L, generator=g).to(torch.int32)
-    slots = torch.full((L,), -1, dtype=torch.int32)
-    kv = torch.zeros(4, 2, Hkv, 16, D, dtype=torch.bfloat16).cuda()
-    dq = dev(qkv)
-    ops.rope_kvwrite(dq, pos.cuda(), slots.cuda(), dev(cs), kv, Hq, Hkv)
-    got = dq.float().cpu()
-    want = torch.cat([
-        O.rope_neox(qkv[:, :(Hq + Hkv) * D].reshape(L, Hq + Hkv, D), pos.long(), cs).reshape(L, -1),
-        qkv[:, (Hq + Hkv) * D:]], dim=1)
-    bad = (got != want)
-    if bad.any():
-        idx = bad.nonzero()[:8]
-        detail = [(int(i), int(j), float(got[i, j]), float(want[i, j]), float(qkv[i, j]), int(pos[i])) for i, j in idx]
-        raise AssertionError(f"{int(bad.sum())}/{bad.numel()} differ; max abs {(got - want).abs().max():.4g}; "
-                             f"(row, col, got, want, x, pos): {detail}")
-    assert not kv.any(), "slot -1 must not write the cache"
 
 
 def _paged_setup(seq_lens, q_lens, Hq=4, Hkv=1, seed=0, nblocks=64, want_raw=False):
@@ -196,7 +151,7 @@ def _paged_setup(seq_lens, q_lens, Hq=4, Hkv=1, seed=0, nblocks=64, want_raw=Fal
         k = O.rope_neox(qkv[:, Hq * D:(Hq + Hkv) * D].reshape(L, Hkv, D), pos.long(), cs)
         v = qkv[:, (Hq + Hkv) * D:].reshape(L, Hkv, D)
         # the oracle's attention inputs are the kernel's own rotated q/k (RoPE itself is checked
-        # bit-exactly in test_rope_bit_exact), so attention parity is not coupled to RoPE rounding
+        # bit-exactly in test_elementwise_exact_gpu.py), so attention parity is not coupled to RoPE rounding
         q_dev = dq[:, :Hq * D].float().cpu().reshape(L, Hq, D)
         k_dev = dq[:, Hq * D:(Hq + Hkv) * D].float().cpu().reshape(L, Hkv, D)
         close(q_dev, q, what="rope(q)")

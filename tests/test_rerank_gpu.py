@@ -11,6 +11,7 @@ import pytest
 import torch
 
 from embeddings_common import hidden_rows
+from kernel_numerics import norm_launch, warp_sum
 from kubeai_b200 import B200Error, lib, ops
 from kubeai_b200.engine import Engine, config_from_hf, mini_config
 from kubeai_b200._lib import BEGIN_FN, WRITE_FN, ResponseWriter
@@ -22,21 +23,12 @@ from rerank_common import (activate, edit_config, llama3_tokenizer, logit_bound,
 pytestmark = pytest.mark.gpu
 
 
-def _warp_sum(v):
-    """__shfl_xor_sync butterfly over 32 fp32 lanes (offsets 16..1); every lane ends with the same value."""
-    v = v.astype(np.float32)
-    for o in (16, 8, 4, 2, 1):
-        v = (v + v[np.arange(32) ^ o]).astype(np.float32)
-    return v[0]
-
-
 def _kernel_logits(y, sw, rows):
     """score_rows_kernel's logits of one bf16 normed row y (fp32 values) in its fixed order: the block size and vectors per
     thread that rmsnorm() picks for `rows` rows; per label each thread's FMAs over its vectors i and elements j in visit
     order, the warp butterfly, then the warp sums added one after another in warp order."""
     H = y.size
-    vecs = H // 8
-    threads, vpt = (vecs, 1) if (rows < 512 or vecs % 256) else (256, vecs // 256)
+    threads, vpt = norm_launch(rows, H)
     out = np.zeros(sw.shape[0], np.float32)
     for l in range(sw.shape[0]):
         acc = np.zeros(threads, np.float32)
@@ -45,7 +37,7 @@ def _kernel_logits(y, sw, rows):
                 idx = (np.arange(threads) + i * threads) * 8 + j
                 # fmaf: the product of two bf16 values is exact in fp64, so one rounding of the fp64 sum is the FMA
                 acc = (acc.astype(np.float64) + y[idx].astype(np.float64) * sw[l, idx].astype(np.float64)).astype(np.float32)
-        warps = [_warp_sum(acc[k * 32:(k + 1) * 32]) for k in range(threads // 32)]
+        warps = [warp_sum(acc[k * 32:(k + 1) * 32]) for k in range(threads // 32)]
         t = np.float32(warps[0])
         for w in warps[1:]:
             t = np.float32(t + np.float32(w))
@@ -76,7 +68,7 @@ def test_score_rows_matches_rmsnorm_order_emulation_and_float64(H, n):
         # fp32 bound from float64: H / (8 * vectors per thread) products per thread reduced through 8 * vpt + 5 + warps
         # roundings; each rounding is at most 2^-24 relative of a partial sum bounded by sum |y w|
         want = y.astype(np.float64) @ swn.astype(np.float64).T
-        vpt = 1 if (n < 512 or (H // 8) % 256) else H // 2048
+        vpt = norm_launch(n, H)[1]
         warps = (H // 8 // vpt) // 32
         depth = 8 * vpt + 5 + warps
         bound = depth * 2.0 ** -24 * (np.abs(y).astype(np.float64) @ np.abs(swn).astype(np.float64).T) + 1e-30
