@@ -1,6 +1,6 @@
 // Host interface of the projection GEMM (gemm_wgmma.cu): out[t, n] = sum_k X[t, k] * W[n, k], one 128-row weight slab x
-// block_n-token tile per CTA, optional split-K reduced in-kernel in a fixed order, prologue/epilogue modes that absorb the
-// elementwise kernels around the projections.
+// block_n-token tile per CTA, optional split-K over thread-block clusters reduced in-kernel in a fixed order,
+// prologue/epilogue modes that absorb the elementwise kernels around the projections.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -43,8 +43,9 @@ struct Gemm3Params {
   // ARGMAX: per (token, 128-row slab) {best logit, index as int bits}; columns >= n_valid are ignored
   float2* cand;
   int n_valid;
-  // split-K partials [tile][split][block_n tokens][128 rows] fp32, and one arrival counter per tile plus one per token tile
-  // (zero-initialised, reset by the kernel that uses them)
+  // split-K partials [tile][split][block_n tokens][128 rows] fp32, written only when a tile's S pieces span several
+  // clusters (gemm_wgmma.cu); arrival counters: one per token tile (RESADD with normed_out), then one per tile and
+  // cluster rank (zero-initialised, reset by the kernel that uses them)
   float* ws;
   size_t ws_bytes;
   int* counters;
@@ -59,7 +60,7 @@ struct Gemm3Schedule {
   int grid;     // CTAs
 };
 
-// force (T <= 128): 0 automatic; 1..8 that many K-splits; -1 splits sized to the device; -n (n >= 2) n K-splits.
+// force (T <= 128): 0 automatic; 1..16 that many K-splits; -1 splits sized to the device; -n (n >= 2) n K-splits.
 // force (T > 128): 0 automatic; >= 64 the requested token-tile size: the kernel uses the largest of 64 / 128 / 256 that
 // does not exceed it (wgmma N is at most 256).  <0: shape or force not served.
 int gemm3_schedule(int N, int K, int T, int force, Gemm3Schedule* out);

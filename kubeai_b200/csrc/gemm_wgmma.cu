@@ -10,9 +10,13 @@
 //     memory stages guarded by full / empty mbarriers; the consumers run wgmma.mma_async on the stages directly.  The
 //     weight loads of the first ring fill go out before the PDL dependency wait (weights are static).
 //   * split-K: with fewer tiles than SMs (o_proj / down_proj / qkv of a decode step) each tile's K range is cut into S
-//     pieces on S CTAs.  Every piece leaves its fp32 partial in an L2-resident workspace; the last CTA to arrive sums the S
-//     partials in split order (a fixed order: the result does not depend on timing) and runs the epilogue.  It loads 16
-//     float4 of a piece per thread before it adds any, so the reduction of a decode-step tile costs about S L2 round trips.
+//     pieces on S CTAs, launched as thread-block clusters of c consecutive pieces: c = S when S-CTA clusters of the
+//     whole grid are resident at once, else the largest divisor of S that is (1 at worst).  Each CTA of a cluster
+//     finishes a 1/c share of the tile's tokens: it sums them over the S pieces in split order (a fixed order: the
+//     result does not depend on timing) and runs the epilogue on them.  With c = S the pieces are read from the peers'
+//     shared memory (DSMEM); with c < S every piece goes to an L2 workspace and, per share, the last cluster to arrive
+//     sums it.  A thread loads up to 16 float4 of a piece before it adds any, so a decode-step share costs about S
+//     round trips.
 //   * epilogues: the fp32 tile is staged in shared memory (reusing the ring) and rounded to bf16 once, the rounding point
 //     of a bf16 GEMM output; the elementwise op that follows a projection (residual add, SiLU * up, RoPE + paged KV write,
 //     per-slab argmax) is applied to that rounded value with the same arithmetic as the standalone kernels (elementwise.cu).
@@ -137,6 +141,11 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_wgmma_kernel(const __grid_co
         }
       }
     }
+    if (S > 1 && cluster_nctas() > 1) {   // the producer warpgroup takes part in the consumers' cluster barrier phases
+      cluster_arrive();
+      cluster_wait();
+      if (cluster_nctas() == S) cluster_arrive();
+    }
     return;
   }
 
@@ -217,70 +226,108 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_wgmma_kernel(const __grid_co
     }
   }
   consumer_sync();
-  const int tile = tt * tiles_n + slab;
+  const int t_end = min(BN, P.T - t0);
+  // With S > 1 the S pieces of a tile are S / c clusters of c (launch()): cluster rank == split % c.  Rank r finishes
+  // the share [ta, tb) of the tile's tokens, cut like the K range; with no split one CTA finishes them all.
+  const int csize = S > 1 ? cluster_nctas() : 1, rank = split % csize;
+  const int ta = rank * t_end / csize, tb = (rank + 1) * t_end / csize;
   if (S > 1) {
-    float* my = P.ws + (static_cast<size_t>(tile) * S + split) * (BN * kSlab);
-    for (int i = ctid; i < BN * kSlab / 4; i += kConsumers) {
-      const int t = (i * 4) / kSlab, r = (i * 4) % kSlab;
-      __stcg(reinterpret_cast<float4*>(my) + i, *reinterpret_cast<const float4*>(stg + t * kPitch + r));
+    // c == S: the peers' staged tiles are read through distributed shared memory once every piece is staged.  c < S:
+    // every piece goes to an L2 workspace; once a cluster's pieces are all out, its rank-r CTA counts one arrival for
+    // share r, and the CTA that brings the count to S / c sums that share.  Either way the sum runs in split order
+    // (p0 + p1 + ..), so the result does not depend on timing, and lands in the summing CTA's own staging tile.
+    const int tile = tt * tiles_n + slab;
+    const float* ws = P.ws + static_cast<size_t>(tile) * S * (BN * kSlab);
+    const bool dsm = csize == S;
+    if (!dsm) {
+      float* my = P.ws + (static_cast<size_t>(tile) * S + split) * (BN * kSlab);
+      for (int i = ctid; i < BN * kSlab / 4; i += kConsumers) {
+        const int t = (i * 4) / kSlab, r = (i * 4) % kSlab;
+        __stcg(reinterpret_cast<float4*>(my) + i, *reinterpret_cast<const float4*>(stg + t * kPitch + r));
+      }
+      __threadfence();
     }
-    __threadfence();
-    consumer_sync();
-    if (ctid == 0) {
-      const int prev = atomicAdd(P.counters + tile, 1);
-      const int last = prev == S - 1;
-      if (last) P.counters[tile] = 0;   // every piece has arrived: reset for the next launch
-      *flag_s = last;
+    if (csize > 1) {
+      cluster_arrive();
+      cluster_wait();
+    } else {
+      consumer_sync();
     }
-    consumer_sync();
-    if (!*flag_s) return;
-    __threadfence();
-    const float4* base = reinterpret_cast<const float4*>(P.ws + static_cast<size_t>(tile) * S * (BN * kSlab));
-    // U float4 of the tile per thread at a time, all S partials of them loaded one piece after the other: U loads in
-    // flight per thread instead of one, so the sum costs S L2 round trips per U float4 rather than one per float4
-    constexpr int kPer = BN * kSlab / 4 / kConsumers, U = kPer < 16 ? kPer : 16;
-    for (int c = 0; c < kPer; c += U) {
-      float4 v[U];
+    if (!dsm) {
+      if (ctid == 0) {
+        int* cnt = P.counters + ntt + tile * csize + rank;   // after the per-token-tile counters of normed_out
+        const int prev = atomicAdd(cnt, 1);
+        const int last = prev == S / csize - 1;
+        if (last) *cnt = 0;   // every cluster has arrived: reset for the next launch
+        *flag_s = last;
+      }
+      consumer_sync();
+      if (!*flag_s) return;
+      __threadfence();
+    }
+    // U float4 of the share per thread at a time, all S pieces of them loaded one piece after the other: U loads in
+    // flight per thread, so the sum costs S round trips per U float4.  U is the whole tile's float4 per thread in the 64-
+    // and 128-token instances (8 / 16): a share is one batch, as the whole tile is when one CTA sums it.  The 256-token
+    // instance (32 per thread) takes 8 at a time: at its 168-register cap 16 would spill.  Float4 c + 256 u of the share
+    // is row 8 u below float4 c.
+    constexpr int kRow4 = kSlab / 4, kPer = BN * kRow4 / kConsumers, U = kPer <= 16 ? kPer : 8;
+    constexpr int kRowsPerPass = kConsumers / kRow4;
+    const int n4 = (tb - ta) * kRow4;
+    auto sum_share = [&](auto load) {   // load(c, u, s): float4 c + 256 u of the share in piece s
+      for (int c = ctid; c < n4; c += U * kConsumers) {
+        float4 v[U], w[U];
 #pragma unroll
-      for (int u = 0; u < U; ++u) v[u] = __ldcg(base + ctid + (c + u) * kConsumers);
-      for (int s = 1; s < S; ++s) {   // split order: independent of which piece finished last
-        float4 w[U];
+        for (int u = 0; u < U; ++u)
+          if (c + u * kConsumers < n4) v[u] = load(c, u, 0);
+        for (int s = 1; s < S; ++s) {   // split order: p0 + p1 + .., whichever piece finished last
 #pragma unroll
-        for (int u = 0; u < U; ++u) w[u] = __ldcg(base + static_cast<size_t>(s) * (BN * kSlab / 4) + ctid + (c + u) * kConsumers);
+          for (int u = 0; u < U; ++u)
+            if (c + u * kConsumers < n4) w[u] = load(c, u, s);
 #pragma unroll
-        for (int u = 0; u < U; ++u) {
-          v[u].x += w[u].x; v[u].y += w[u].y; v[u].z += w[u].z; v[u].w += w[u].w;
+          for (int u = 0; u < U; ++u) {
+            v[u].x += w[u].x; v[u].y += w[u].y; v[u].z += w[u].z; v[u].w += w[u].w;
+          }
         }
-      }
+        float* dst = stg + (ta + c / kRow4) * kPitch + (c % kRow4) * 4;
 #pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const int i = ctid + (c + u) * kConsumers, t = (i * 4) / kSlab, r = (i * 4) % kSlab;
-        *reinterpret_cast<float4*>(stg + t * kPitch + r) = v[u];
+        for (int u = 0; u < U; ++u)
+          if (c + u * kConsumers < n4) *reinterpret_cast<float4*>(dst + u * kRowsPerPass * kPitch) = v[u];
       }
+    };
+    if (dsm) {
+      sum_share([&](int c, int u, int s) {
+        const uint32_t a = smem_u32(stg + (ta + c / kRow4) * kPitch + (c % kRow4) * 4);
+        return dsmem_ld_f4(dsmem_map(a, s) + u * kRowsPerPass * kPitch * 4);   // a peer's shared memory is contiguous
+      });
+    } else {
+      sum_share([&](int c, int u, int s) {
+        const float* p = ws + static_cast<size_t>(s) * (BN * kSlab) + (ta + c / kRow4) * kSlab + (c % kRow4) * 4;
+        return __ldcg(reinterpret_cast<const float4*>(p + u * kRowsPerPass * kSlab));
+      });
     }
+    if (dsm) cluster_arrive();   // done reading the peers' tiles; the matching wait comes before this CTA exits
     consumer_sync();
   }
 
   // ---------------- epilogue: one warp per token, each lane 4 consecutive rows of the slab
   constexpr int kWarps = kConsumers / 32;
   const int slabs = tiles_n;
-  const int t_end = min(BN, P.T - t0);
   if (P.epi == GEMM3_EPI_RESADD) {
     // the residual of 4 of the warp's tokens is read before any of them is written back: 4 round trips in flight per
     // lane instead of one
-    for (int tl0 = warp; tl0 < t_end; tl0 += 4 * kWarps) {
+    for (int tl0 = ta + warp; tl0 < tb; tl0 += 4 * kWarps) {
       float res[4][4];
 #pragma unroll
       for (int j = 0; j < 4; ++j)
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           const int tl = tl0 + j * kWarps, r = lane * 4 + e;
-          res[j][e] = tl < t_end && n0 + r < P.N ? ldbf(P.out + static_cast<size_t>(t0 + tl) * P.ldo + n0 + r) : 0.f;
+          res[j][e] = tl < tb && n0 + r < P.N ? ldbf(P.out + static_cast<size_t>(t0 + tl) * P.ldo + n0 + r) : 0.f;
         }
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const int tl = tl0 + j * kWarps, t = t0 + tl;
-        if (tl >= t_end) break;
+        if (tl >= tb) break;
         const float* row = stg + tl * kPitch;
         float ss = 0.f;
 #pragma unroll
@@ -299,7 +346,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_wgmma_kernel(const __grid_co
       }
     }
   }
-  for (int tl = warp; tl < t_end && P.epi != GEMM3_EPI_RESADD; tl += kWarps) {
+  for (int tl = ta + warp; tl < tb && P.epi != GEMM3_EPI_RESADD; tl += kWarps) {
     const int t = t0 + tl;
     const float* row = stg + tl * kPitch;
     if (P.epi == GEMM3_EPI_PLAIN) {
@@ -422,15 +469,17 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_wgmma_kernel(const __grid_co
     }
   }
 
+  if (S > 1 && csize == S) cluster_wait();   // no peer still reads this CTA's staging tile
+
   if (P.epi == GEMM3_EPI_RESADD && P.normed_out) {
-    // RMSNorm of the new residual for the next projection: needs the sums of every slab of these tokens, so the last CTA
-    // of the token tile to finish its slab does it (counters after the per-tile split-K counters)
+    // RMSNorm of the new residual for the next projection: needs the sums of every slab of these tokens, so the last of
+    // the token tile's slabs x c CTAs to finish its share does it
     __threadfence();
     consumer_sync();
     if (ctid == 0) {
-      int* c = P.counters + tiles_n * ntt + tt;
+      int* c = P.counters + tt;
       const int prev = atomicAdd(c, 1);
-      const int last = prev == tiles_n - 1;
+      const int last = prev == tiles_n * csize - 1;
       if (last) *c = 0;
       *flag_s = last;
     }
@@ -518,11 +567,46 @@ EncodeTiledFn get_encode_fn() {
 template <int BN, int HD>
 int launch(const Gemm3Params& p, const Gemm3Schedule& sch, cudaStream_t st) {
   using C = Cfg<BN>;
-  static std::atomic<unsigned long long> attr_done{0};
+  static std::atomic<unsigned long long> attr_done{0}, cluster_done{0};
   if (!ensure_dynamic_smem(gemm_wgmma_kernel<BN, HD>, C::kSmem, &attr_done)) return -3;
+  // clusters of up to kMaxSplits (16) CTAs: above 8 the cluster size is not portable
+  if (!ensure_func_attribute(gemm_wgmma_kernel<BN, HD>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1, &cluster_done))
+    return -3;
   const int slabs = (p.N + kSlab - 1) / kSlab, ntt = (p.T + BN - 1) / BN;
   const dim3 grid = ntt > 1 ? dim3(ntt, slabs, sch.S) : dim3(slabs, 1, sch.S);   // see the kernel's CTA order
-  cudaError_t e = launch_pdl(gemm_wgmma_kernel<BN, HD>, grid, dim3(kThreads), C::kSmem, st, p, sch.S);
+  // Clusters of c consecutive pieces of a tile: the largest c dividing S whose clusters are all resident at once.  A GPC
+  // holds a whole number of clusters, so on a 132-SM H100 only 30 clusters of 4 fit where 32 would be needed for
+  // Llama-3-8B's o_proj and down_proj; those run as 64 pairs.  The count is queried once per device and cluster size; a
+  // size the query refuses counts as not fitting, down to c = 1 (no cluster).
+  static std::atomic<int> max_clusters[64][kMaxSplits + 1];   // [device][c]: 1 + resident clusters, 0 until queried
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return -3;
+  std::atomic<int>* fit = max_clusters[dev & 63];
+  int c = sch.S;
+  for (; c > 1; --c) {
+    if (sch.S % c) continue;
+    if (fit[c].load(std::memory_order_relaxed) == 0) {
+      cudaLaunchConfig_t cfg = {};
+      cfg.gridDim = grid;
+      cfg.blockDim = dim3(kThreads);
+      cfg.dynamicSmemBytes = C::kSmem;
+      cudaLaunchAttribute a[1];
+      a[0].id = cudaLaunchAttributeClusterDimension;
+      a[0].val.clusterDim.x = 1;
+      a[0].val.clusterDim.y = 1;
+      a[0].val.clusterDim.z = c;
+      cfg.attrs = a;
+      cfg.numAttrs = 1;
+      int n = 0;
+      if (cudaOccupancyMaxActiveClusters(&n, gemm_wgmma_kernel<BN, HD>, &cfg) != cudaSuccess) {
+        cudaGetLastError();   // not an error of the launch: this size just does not fit
+        n = 0;
+      }
+      fit[c].store(n + 1, std::memory_order_relaxed);
+    }
+    if (static_cast<long long>(grid.x) * grid.y * (sch.S / c) <= fit[c].load(std::memory_order_relaxed) - 1) break;
+  }
+  cudaError_t e = launch_pdl_cluster(gemm_wgmma_kernel<BN, HD>, grid, dim3(1, 1, c), dim3(kThreads), C::kSmem, st, p, sch.S);
   return e == cudaSuccess ? 0 : -4;
 }
 
@@ -627,7 +711,7 @@ size_t gemm3_ws_bytes(int N, const Gemm3Schedule& sch, int T) {
 
 int gemm3_counters_needed(int N, const Gemm3Schedule& sch, int T) {
   const int ntt = (T + sch.block_n - 1) / sch.block_n;
-  return ((N + kSlab - 1) / kSlab) * ntt + ntt;
+  return ntt + ((N + kSlab - 1) / kSlab) * ntt * sch.S;
 }
 
 int gemm3_launch(const Gemm3Params& p, const Gemm3Schedule& sch, cudaStream_t st) {

@@ -80,6 +80,32 @@ __device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity)
   }
 }
 
+// ---------------------------------------------------------------- thread-block cluster
+// One phase of the cluster barrier: every non-exited thread of the cluster arrives once, then waits.  Arrive releases the
+// thread's earlier memory accesses (shared memory included) to the cluster, wait acquires those of every other thread.
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire;" ::: "memory"); }
+// CTAs in this CTA's cluster (1 when the launch has no cluster dimension)
+__device__ __forceinline__ int cluster_nctas() {
+  uint32_t n;
+  asm("mov.u32 %0, %%cluster_nctarank;" : "=r"(n));
+  return static_cast<int>(n);
+}
+// shared::cluster address of the same shared-memory location in the CTA of cluster rank `rank`
+__device__ __forceinline__ uint32_t dsmem_map(uint32_t smem_addr, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
+  return r;
+}
+__device__ __forceinline__ float4 dsmem_ld_f4(uint32_t addr) {
+  float4 v;
+  asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];"
+               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+               : "r"(addr)
+               : "memory");
+  return v;
+}
+
 // ---------------------------------------------------------------- TMA
 constexpr uint64_t kEvictNormal = 0x1000000000000000ull;
 constexpr uint64_t kEvictFirst = 0x12F0000000000000ull;
