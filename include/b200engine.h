@@ -608,6 +608,30 @@ typedef struct {
   const int32_t* stop_ids;
 } b200_penalty_row;
 int b200_op_penalize(void* logits, int32_t ld, int32_t S, int32_t V, const b200_penalty_row* rows, void* edited, void* stream);
+/* The engine's token-history lists on buffers the caller owns, with the engine's device code.  recs (device):
+ * [n_slots][cap] records of four 32-bit words {id, count, bias (fp32), flags: 1 prompt, 2 stop, 4 bias}, each list sorted
+ * by id; lens (device int32 [n_slots]): the records in use.
+ * b200_op_penalty_list: builds list `slot` from row (host) as the engine does when it admits a request (the prompt and
+ * output only when some penalty is on; the stop ids only while num_output < min_tokens), writes it to recs[slot][0, n)
+ * and sets lens[slot] = n.  n > cap is B200_ERR_INVALID. */
+int b200_op_penalty_list(const b200_penalty_row* row, int32_t V, void* recs, int32_t* lens, int32_t n_slots, int32_t cap,
+                         int32_t slot, void* stream);
+/* One edited row of a launch on those lists: logits row `row`, list `slot`; repetition 0 = off.  history != 0: the update
+ * adds the row's sampled token to the list. */
+typedef struct {
+  int32_t row, slot;
+  float presence_penalty, frequency_penalty, repetition_penalty;
+  int32_t n_generated, min_tokens, history;
+} b200_penalty_slot_row;
+/* One penalize_update launch: for each of the n rows (host) with history, sampled[row] (host, [S], ids in [0, V)) joins
+ * list `slot`: its count + 1, or a new record {id, 1, 0, 0} in id order while the list has fewer than cap records.  Rows
+ * name rows in [0, S) and distinct slots in [0, n_slots). */
+int b200_op_penalize_update(const b200_penalty_slot_row* rows, int32_t n, const int32_t* sampled, int32_t S, int32_t V,
+                            void* recs, int32_t* lens, int32_t n_slots, int32_t cap, void* stream);
+/* b200_op_penalize on those lists: row i of rows (host) edits bf16 logits row rows[i].row ([S, ld], device, in place;
+ * distinct rows) from list rows[i].slot; every id of a named list is in [0, V).  edited as in b200_op_penalize. */
+int b200_op_penalize_slots(void* logits, int32_t ld, int32_t S, int32_t V, const b200_penalty_slot_row* rows, int32_t n,
+                           const void* recs, const int32_t* lens, int32_t n_slots, int32_t cap, void* edited, void* stream);
 /* work: int32[num_work][4] = {q_tok0, q_count, q_pos0, seq}; kv_layer: [block][2][kv_heads][16][128]; kv_heads divides
  * q_heads and G = q_heads / kv_heads is 1..16.  Decode attention: every item has 1 <= q_count <= 16 / G consecutive query
  * positions (a speculative verify), position j masked causally at q_pos0 + j, and the item's K/V read once for all of

@@ -220,6 +220,9 @@ SYMBOLS = {
     "b200_op_argmax": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _vp]),
     "b200_op_sample": (C.c_int, [_vp, _i32, _vp, _i32, _i32, _vp, _vp]),
     "b200_op_penalize": (C.c_int, [_vp, _i32, _i32, _i32, C.POINTER(PenaltyRow), _vp, _vp]),
+    "b200_op_penalty_list": (C.c_int, [C.POINTER(PenaltyRow), _i32, _vp, _vp, _i32, _i32, _i32, _vp]),
+    "b200_op_penalize_update": (C.c_int, [_vp, _i32, _pi32, _i32, _i32, _vp, _vp, _i32, _i32, _vp]),
+    "b200_op_penalize_slots": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _i32, _vp, _vp, _i32, _i32, _vp, _vp]),
     "b200_op_logprobs": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "b200_op_logprobs_rank": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "b200_op_paged_attn": (C.c_int, [_vp, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _f, _i32, _vp]),

@@ -299,6 +299,167 @@ int b200_op_sample(const void* logits, int32_t ld, const b200_sample_row* rows, 
   return rc ? cuda_fail("sample_rows", rc) : 0;
 }
 
+namespace {
+// One request's record list as the engine builds it at admission (the prompt and output only when a penalty is on, the
+// stop ids only while fewer than min_tokens tokens exist) and its PenaltyRow for logits row and list `s`.  False when an
+// id is outside [0, V) or a list is malformed.
+bool penalty_list_of(const b200_penalty_row& r, int V, int s, std::vector<PenaltyRec>* list, PenaltyRow* prow) {
+  auto ids_ok = [&](const int32_t* p, int n) {
+    if (n < 0 || (n > 0 && !p)) return false;
+    for (int i = 0; i < n; ++i) if (p[i] < 0 || p[i] >= V) return false;
+    return true;
+  };
+  if (!ids_ok(r.prompt, r.num_prompt) || !ids_ok(r.output, r.num_output) || !ids_ok(r.logit_bias_ids, r.num_logit_bias) ||
+      !ids_ok(r.stop_ids, r.num_stop_ids) || (r.num_logit_bias > 0 && !r.logit_bias_values) || !(r.repetition_penalty >= 0.f))
+    return false;
+  const float rp = r.repetition_penalty > 0.f ? r.repetition_penalty : 1.f;
+  const bool history = r.presence_penalty != 0.f || r.frequency_penalty != 0.f || rp != 1.f;
+  *prow = PenaltyRow{s, s, r.presence_penalty, r.frequency_penalty, rp, r.num_output, r.min_tokens, history ? 1 : 0};
+  penalty_records(r.prompt, r.num_prompt, r.output, r.num_output, history, r.logit_bias_ids, r.logit_bias_values,
+                  r.num_logit_bias, r.stop_ids, r.num_output < r.min_tokens ? r.num_stop_ids : 0, list);
+  return true;
+}
+
+// The rows of a slot-addressed launch (host memory) as PenaltyRows, checked against the caller's lists: every row in
+// [0, S) and every slot in [0, n_slots), each at most once where `unique_rows` / `unique_slots` ask it (two CTAs on one
+// logits row or one list would race), and lens[slot] in [0, cap].  ids_V > 0: every id below lens[slot] of a named list
+// is in [0, ids_V) as well (the edit writes logits[row][id]).  Copies lens (and those lists) to the host.
+int slot_rows_of(const char* what, const b200_penalty_slot_row* rows, int n, int S, const void* recs, const int32_t* lens,
+                 int n_slots, int cap, bool unique_rows, bool unique_slots, int ids_V, std::vector<PenaltyRow>* out) {
+  static_assert(sizeof(b200_penalty_slot_row) == sizeof(PenaltyRow), "b200_penalty_slot_row is PenaltyRow on the wire");
+  if (n < 0 || (n > 0 && !rows) || S < 1 || !recs || !lens || n_slots < 1 || cap < 1) {
+    set_error("%s: bad arguments (n=%d S=%d n_slots=%d cap=%d)", what, n, S, n_slots, cap);
+    return B200_ERR_INVALID;
+  }
+  std::vector<int> h_lens(n_slots);
+  if (cudaMemcpy(h_lens.data(), lens, h_lens.size() * sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess)
+    return cuda_fail(what, -2);
+  std::vector<char> row_seen(S, 0), slot_seen(n_slots, 0);
+  out->resize(n);
+  for (int i = 0; i < n; ++i) {
+    const b200_penalty_slot_row& r = rows[i];
+    if (r.row < 0 || r.row >= S || r.slot < 0 || r.slot >= n_slots) {
+      set_error("%s: row %d names logits row %d of %d, list %d of %d", what, i, r.row, S, r.slot, n_slots);
+      return B200_ERR_INVALID;
+    }
+    if ((unique_rows && row_seen[r.row]) || (unique_slots && slot_seen[r.slot])) {
+      set_error("%s: row %d repeats logits row %d or list %d", what, i, r.row, r.slot);
+      return B200_ERR_INVALID;
+    }
+    if (!(r.repetition_penalty >= 0.f) || h_lens[r.slot] < 0 || h_lens[r.slot] > cap) {
+      set_error("%s: row %d has repetition %g or list %d of length %d (cap %d)", what, i, r.repetition_penalty, r.slot,
+                h_lens[r.slot], cap);
+      return B200_ERR_INVALID;
+    }
+    if (ids_V > 0 && !slot_seen[r.slot]) {
+      std::vector<PenaltyRec> list(h_lens[r.slot]);
+      if (cudaMemcpy(list.data(), static_cast<const PenaltyRec*>(recs) + static_cast<size_t>(r.slot) * cap,
+                     list.size() * sizeof(PenaltyRec), cudaMemcpyDeviceToHost) != cudaSuccess)
+        return cuda_fail(what, -2);
+      for (const PenaltyRec& e : list)
+        if (e.id < 0 || e.id >= ids_V) {
+          set_error("%s: list %d holds id %d outside [0, %d)", what, r.slot, e.id, ids_V);
+          return B200_ERR_INVALID;
+        }
+    }
+    row_seen[r.row] = slot_seen[r.slot] = 1;
+    (*out)[i] = PenaltyRow{r.row, r.slot, r.presence_penalty, r.frequency_penalty,
+                           r.repetition_penalty > 0.f ? r.repetition_penalty : 1.f, r.n_generated, r.min_tokens, r.history};
+  }
+  return 0;
+}
+}  // namespace
+
+int b200_op_penalty_list(const b200_penalty_row* row, int32_t V, void* recs, int32_t* lens, int32_t n_slots, int32_t cap,
+                         int32_t slot, void* stream) {
+  if (int rc = require_device()) return rc;
+  std::vector<PenaltyRec> list;
+  PenaltyRow prow;
+  if (!row || !recs || !lens || V < 1 || cap < 1 || slot < 0 || slot >= n_slots || !penalty_list_of(*row, V, slot, &list, &prow)) {
+    set_error("b200_op_penalty_list: bad arguments (V=%d slot=%d n_slots=%d cap=%d) or a token id outside [0, V)", V, slot,
+              n_slots, cap);
+    return B200_ERR_INVALID;
+  }
+  const int n = static_cast<int>(list.size());
+  if (n > cap) {
+    set_error("b200_op_penalty_list: record list of %d entries exceeds %d", n, cap);
+    return B200_ERR_INVALID;
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaError_t ce = cudaMemcpyAsync(static_cast<PenaltyRec*>(recs) + static_cast<size_t>(slot) * cap, list.data(),
+                                   static_cast<size_t>(n) * sizeof(PenaltyRec), cudaMemcpyHostToDevice, st);
+  if (ce == cudaSuccess) ce = cudaMemcpyAsync(lens + slot, &n, sizeof(int), cudaMemcpyHostToDevice, st);
+  if (cudaStreamSynchronize(st) != cudaSuccess || ce != cudaSuccess) return cuda_fail("b200_op_penalty_list", -2);
+  return 0;
+}
+
+int b200_op_penalize_update(const b200_penalty_slot_row* rows, int32_t n, const int32_t* sampled, int32_t S, int32_t V,
+                            void* recs, int32_t* lens, int32_t n_slots, int32_t cap, void* stream) {
+  if (int rc = require_device()) return rc;
+  std::vector<PenaltyRow> prow;
+  if (int rc = slot_rows_of("b200_op_penalize_update", rows, n, S, recs, lens, n_slots, cap, true, true, 0, &prow)) return rc;
+  if (!sampled || V < 1) {
+    set_error("b200_op_penalize_update: bad arguments (V=%d)", V);
+    return B200_ERR_INVALID;
+  }
+  for (int s = 0; s < S; ++s)
+    if (sampled[s] < 0 || sampled[s] >= V) {
+      set_error("b200_op_penalize_update: sampled[%d] = %d is outside [0, %d)", s, sampled[s], V);
+      return B200_ERR_INVALID;
+    }
+  if (n == 0) return 0;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  PenaltyRow* d_rows = nullptr;
+  int* d_sampled = nullptr;
+  cudaError_t ce = cudaMalloc(&d_rows, prow.size() * sizeof(PenaltyRow));
+  if (ce == cudaSuccess) ce = cudaMalloc(&d_sampled, static_cast<size_t>(S) * sizeof(int));
+  if (ce == cudaSuccess) ce = cudaMemcpyAsync(d_rows, prow.data(), prow.size() * sizeof(PenaltyRow), cudaMemcpyHostToDevice, st);
+  if (ce == cudaSuccess) ce = cudaMemcpyAsync(d_sampled, sampled, static_cast<size_t>(S) * sizeof(int), cudaMemcpyHostToDevice, st);
+  int rc = ce == cudaSuccess ? 0 : -2;
+  if (!rc) rc = penalize_update(d_rows, n, d_sampled, static_cast<PenaltyRec*>(recs), lens, cap, st);
+  if (cudaStreamSynchronize(st) != cudaSuccess) rc = -2;   // before the host rows and the scratch go away
+  cudaFree(d_rows);
+  cudaFree(d_sampled);
+  return rc ? cuda_fail("penalize_update", rc) : 0;
+}
+
+// penalize_rows, then (edited given) the copy and penalize_restore, on S rows of logits; `lists` holds cap records per
+// row's slot, the lengths in `lens`.  Device memory throughout; frees its own scratch.
+static int penalize_launch(void* logits, int ld, int S, const std::vector<PenaltyRow>& prow, const PenaltyRec* recs,
+                           const int* lens, int cap, void* edited, cudaStream_t st) {
+  const int n = static_cast<int>(prow.size());
+  PenaltyRow* d_rows = nullptr;
+  uint16_t* d_save = nullptr;
+  cudaError_t ce = cudaMalloc(&d_rows, prow.size() * sizeof(PenaltyRow));
+  if (ce == cudaSuccess) ce = cudaMalloc(&d_save, static_cast<size_t>(n) * cap * sizeof(uint16_t));
+  if (ce == cudaSuccess) ce = cudaMemcpyAsync(d_rows, prow.data(), prow.size() * sizeof(PenaltyRow), cudaMemcpyHostToDevice, st);
+  int rc = ce == cudaSuccess ? 0 : -2;
+  if (!rc) rc = penalize_rows(logits, ld, d_rows, n, recs, lens, cap, d_save, st);
+  if (!rc && edited) {
+    ce = cudaMemcpyAsync(edited, logits, static_cast<size_t>(S) * ld * 2, cudaMemcpyDeviceToDevice, st);
+    rc = ce == cudaSuccess ? penalize_restore(logits, ld, d_rows, n, recs, lens, cap, d_save, st) : -2;
+  }
+  if (cudaStreamSynchronize(st) != cudaSuccess) rc = -2;   // before the host rows and the scratch go away
+  cudaFree(d_rows);
+  cudaFree(d_save);
+  return rc;
+}
+
+int b200_op_penalize_slots(void* logits, int32_t ld, int32_t S, int32_t V, const b200_penalty_slot_row* rows, int32_t n,
+                           const void* recs, const int32_t* lens, int32_t n_slots, int32_t cap, void* edited, void* stream) {
+  if (int rc = require_device()) return rc;
+  if (!logits || V < 1 || ld < V) {
+    set_error("b200_op_penalize_slots: bad arguments (S=%d V=%d ld=%d)", S, V, ld);
+    return B200_ERR_INVALID;
+  }
+  std::vector<PenaltyRow> prow;
+  if (int rc = slot_rows_of("b200_op_penalize_slots", rows, n, S, recs, lens, n_slots, cap, true, false, V, &prow)) return rc;
+  if (n == 0) return 0;
+  int rc = penalize_launch(logits, ld, S, prow, static_cast<const PenaltyRec*>(recs), lens, cap, edited,
+                           static_cast<cudaStream_t>(stream));
+  return rc ? cuda_fail("penalize_rows", rc) : 0;
+}
+
 int b200_op_penalize(void* logits, int32_t ld, int32_t S, int32_t V, const b200_penalty_row* rows, void* edited, void* stream) {
   if (int rc = require_device()) return rc;
   if (!logits || (S > 0 && !rows) || S < 0 || V < 1 || ld < V) {
@@ -311,22 +472,10 @@ int b200_op_penalize(void* logits, int32_t ld, int32_t S, int32_t V, const b200_
   std::vector<PenaltyRow> prow(S);
   int cap = 1;
   for (int s = 0; s < S; ++s) {
-    const b200_penalty_row& r = rows[s];
-    auto ids_ok = [&](const int32_t* p, int n) {
-      if (n < 0 || (n > 0 && !p)) return false;
-      for (int i = 0; i < n; ++i) if (p[i] < 0 || p[i] >= V) return false;
-      return true;
-    };
-    if (!ids_ok(r.prompt, r.num_prompt) || !ids_ok(r.output, r.num_output) || !ids_ok(r.logit_bias_ids, r.num_logit_bias) ||
-        !ids_ok(r.stop_ids, r.num_stop_ids) || (r.num_logit_bias > 0 && !r.logit_bias_values) || !(r.repetition_penalty >= 0.f)) {
+    if (!penalty_list_of(rows[s], V, s, &lists[s], &prow[s])) {
       set_error("b200_op_penalize: row %d has a token id outside [0, %d) or a bad list", s, V);
       return B200_ERR_INVALID;
     }
-    const float rp = r.repetition_penalty > 0.f ? r.repetition_penalty : 1.f;
-    prow[s] = PenaltyRow{s, s, r.presence_penalty, r.frequency_penalty, rp, r.num_output, r.min_tokens, 0};
-    const bool history = r.presence_penalty != 0.f || r.frequency_penalty != 0.f || rp != 1.f;
-    penalty_records(r.prompt, r.num_prompt, r.output, r.num_output, history, r.logit_bias_ids, r.logit_bias_values,
-                    r.num_logit_bias, r.stop_ids, r.num_output < r.min_tokens ? r.num_stop_ids : 0, &lists[s]);
     cap = std::max(cap, static_cast<int>(lists[s].size()));
   }
   std::vector<PenaltyRec> recs(static_cast<size_t>(S) * cap);
@@ -337,27 +486,15 @@ int b200_op_penalize(void* logits, int32_t ld, int32_t S, int32_t V, const b200_
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   PenaltyRec* d_recs = nullptr;
-  PenaltyRow* d_rows = nullptr;
   int* d_lens = nullptr;
-  uint16_t* d_save = nullptr;
   cudaError_t ce = cudaMalloc(&d_recs, recs.size() * sizeof(PenaltyRec));
-  if (ce == cudaSuccess) ce = cudaMalloc(&d_rows, prow.size() * sizeof(PenaltyRow));
   if (ce == cudaSuccess) ce = cudaMalloc(&d_lens, lens.size() * sizeof(int));
-  if (ce == cudaSuccess) ce = cudaMalloc(&d_save, static_cast<size_t>(S) * cap * sizeof(uint16_t));
   if (ce == cudaSuccess) ce = cudaMemcpyAsync(d_recs, recs.data(), recs.size() * sizeof(PenaltyRec), cudaMemcpyHostToDevice, st);
-  if (ce == cudaSuccess) ce = cudaMemcpyAsync(d_rows, prow.data(), prow.size() * sizeof(PenaltyRow), cudaMemcpyHostToDevice, st);
   if (ce == cudaSuccess) ce = cudaMemcpyAsync(d_lens, lens.data(), lens.size() * sizeof(int), cudaMemcpyHostToDevice, st);
-  int rc = ce == cudaSuccess ? 0 : -2;
-  if (!rc) rc = penalize_rows(logits, ld, d_rows, S, d_recs, d_lens, cap, d_save, st);
-  if (!rc && edited) {
-    ce = cudaMemcpyAsync(edited, logits, static_cast<size_t>(S) * ld * 2, cudaMemcpyDeviceToDevice, st);
-    rc = ce == cudaSuccess ? penalize_restore(logits, ld, d_rows, S, d_recs, d_lens, cap, d_save, st) : -2;
-  }
+  int rc = ce == cudaSuccess ? penalize_launch(logits, ld, S, prow, d_recs, d_lens, cap, edited, st) : -2;
   if (cudaStreamSynchronize(st) != cudaSuccess) rc = -2;   // before the host lists and the scratch go away
   cudaFree(d_recs);
-  cudaFree(d_rows);
   cudaFree(d_lens);
-  cudaFree(d_save);
   return rc ? cuda_fail("penalize_rows", rc) : 0;
 }
 

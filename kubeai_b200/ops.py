@@ -172,10 +172,18 @@ def penalize(logits, rows, restore=True):
     frequency_penalty, repetition_penalty (1 or 0 = off), min_tokens, prompt, output, logit_bias ({id: bias}) and stop_ids.
     restore=True: returns the edited rows and puts the raw values back into `logits`; False: edits `logits` in place and
     returns it."""
-    from ._lib import PenaltyRow
     _chk(logits)
     S, V = logits.shape
-    keep, arr = [], (PenaltyRow * max(S, 1))()
+    keep, arr = _penalty_rows(rows)
+    edited = torch.empty_like(logits) if restore else None
+    check(lib().b200_op_penalize(_p(logits), logits.stride(0), S, V, arr, _p(edited), _stream()))
+    return edited if restore else logits
+
+
+def _penalty_rows(rows):
+    """(the numpy arrays the rows point into, ctypes PenaltyRow array) of penalize()'s row dicts."""
+    from ._lib import PenaltyRow
+    keep, arr = [], (PenaltyRow * max(len(rows), 1))()
 
     def ptr(a, ct):
         keep.append(a)
@@ -192,8 +200,52 @@ def penalize(logits, rows, restore=True):
                             num_prompt=len(prompt), prompt=ptr(prompt, C.c_int32), num_output=len(output),
                             output=ptr(output, C.c_int32), num_logit_bias=len(bid), logit_bias_ids=ptr(bid, C.c_int32),
                             logit_bias_values=ptr(bval, C.c_float), num_stop_ids=len(stops), stop_ids=ptr(stops, C.c_int32))
+    return keep, arr
+
+
+def penalty_lists(n_slots, cap, device="cuda"):
+    """Record lists for penalty_list / penalize_update / penalize_slots: (recs int32 [n_slots, cap, 4], each record
+    (id, count, bias as fp32 bits, flags), lens int32 [n_slots]), zeroed."""
+    return (torch.zeros(n_slots, cap, 4, dtype=torch.int32, device=device),
+            torch.zeros(n_slots, dtype=torch.int32, device=device))
+
+
+def penalty_list(recs, lens, slot, V, row):
+    """Build list `slot` of (recs, lens) from one penalize() row dict, as the engine does when it admits the request
+    (b200_op_penalty_list)."""
+    _chk(recs, torch.int32), _chk(lens, torch.int32)
+    keep, arr = _penalty_rows([row])
+    check(lib().b200_op_penalty_list(arr, V, _p(recs), _p(lens), recs.shape[0], recs.shape[1], slot, _stream()))
+
+
+_SLOT_ROW = np.dtype([("row", "<i4"), ("slot", "<i4"), ("presence", "<f4"), ("frequency", "<f4"), ("repetition", "<f4"),
+                      ("n_generated", "<i4"), ("min_tokens", "<i4"), ("history", "<i4")])
+
+
+def _slot_rows(rows):
+    """b200_penalty_slot_rows of (row, slot, presence, frequency, repetition, n_generated, min_tokens, history) tuples."""
+    return np.array([tuple(r) for r in rows], dtype=_SLOT_ROW)
+
+
+def penalize_update(recs, lens, rows, sampled, V):
+    """One penalize_update launch (b200_op_penalize_update): for each (row, slot, presence, frequency, repetition,
+    n_generated, min_tokens, history) tuple with history, sampled[row] (host ints, one per logits row) joins list `slot`."""
+    _chk(recs, torch.int32), _chk(lens, torch.int32)
+    a = _slot_rows(rows)
+    s = np.ascontiguousarray(sampled, dtype=np.int32)
+    check(lib().b200_op_penalize_update(a.ctypes.data, len(a), s.ctypes.data_as(C.POINTER(C.c_int32)), len(s), V, _p(recs),
+                                        _p(lens), recs.shape[0], recs.shape[1], _stream()))
+
+
+def penalize_slots(logits, rows, recs, lens, restore=True):
+    """penalize() on the lists of (recs, lens) (b200_op_penalize_slots): each (row, slot, ...) tuple, as in
+    penalize_update, edits logits row `row` from list `slot`.  restore as in penalize()."""
+    _chk(logits), _chk(recs, torch.int32), _chk(lens, torch.int32)
+    S, V = logits.shape
+    a = _slot_rows(rows)
     edited = torch.empty_like(logits) if restore else None
-    check(lib().b200_op_penalize(_p(logits), logits.stride(0), S, V, arr, _p(edited), _stream()))
+    check(lib().b200_op_penalize_slots(_p(logits), logits.stride(0), S, V, a.ctypes.data, len(a), _p(recs), _p(lens),
+                                       recs.shape[0], recs.shape[1], _p(edited), _stream()))
     return edited if restore else logits
 
 

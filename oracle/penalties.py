@@ -73,6 +73,38 @@ def named(V, prompt=(), output=(), presence=0.0, frequency=0.0, repetition=1.0, 
     return m
 
 
+PEN_PROMPT, PEN_STOP, PEN_BIAS = 1, 2, 4   # kPen* of kubeai_b200/csrc/kernels.h
+
+
+def records(prompt=(), output=(), history=True, logit_bias=None, stop_ids=(), min_tokens=0):
+    """The record list penalty_records builds (kubeai_b200/csrc/penalties.cu), as int32 [n, 4] rows (id, count, bias as
+    float32 bits, flags), sorted by id: one record per distinct id; the prompt (PEN_PROMPT) and the output (count) only
+    with `history`; the stop ids (PEN_STOP) only while len(output) < min_tokens; the last bias of an id, clamped to
+    [-100, 100] in float32 (PEN_BIAS).  penalize_update keeps a list equal to this with each sampled token appended to
+    `output` (the stop records stay while the list lives: pass the min_tokens the list was built under)."""
+    prompt = np.asarray(prompt, dtype=np.int64).ravel() if history else np.zeros(0, np.int64)
+    output_h = np.asarray(output, dtype=np.int64).ravel() if history else np.zeros(0, np.int64)
+    stops = np.asarray(stop_ids, dtype=np.int64).ravel() if len(output) < min_tokens else np.zeros(0, np.int64)
+    bias = {int(t): np.float32(min(np.float32(100.0), max(np.float32(-100.0), np.float32(b))))
+            for t, b in (logit_bias or {}).items()}
+    bid = np.array(sorted(bias), dtype=np.int64)
+    ids = np.unique(np.concatenate([prompt, output_h, stops, bid]))
+    out = np.zeros((ids.size, 4), dtype=np.int32)
+    out[:, 0] = ids
+    if output_h.size:
+        u, c = np.unique(output_h, return_counts=True)
+        out[np.searchsorted(ids, u), 1] = c
+    flags = np.zeros(ids.size, dtype=np.int32)
+    flags[np.searchsorted(ids, np.unique(prompt))] |= PEN_PROMPT
+    flags[np.searchsorted(ids, np.unique(stops))] |= PEN_STOP
+    if bid.size:
+        pos = np.searchsorted(ids, bid)
+        flags[pos] |= PEN_BIAS
+        out[pos, 2] = np.array([bias[int(t)] for t in bid], dtype=np.float32).view(np.int32)
+    out[:, 3] = flags
+    return out
+
+
 def min_p_keep(z, min_p):
     """(kept mask, boundary slack) of min_p over one row of scaled logits z (float32 values): the slack is the distance in
     log space between log(min_p) and the nearest d_v = z_v - z_max."""

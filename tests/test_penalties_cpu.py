@@ -170,3 +170,118 @@ def test_min_tokens_above_max_tokens_is_refused():
         r = on.handle("POST", "/openai/v1/chat/completions", json.dumps(body))
         assert r.status == 400 and "min_tokens must be less than or equal to max_tokens=3" in r.json()["error"]
         assert on.handle("POST", "/openai/v1/chat/completions", json.dumps({**body, "min_tokens": 3})).status == 502
+
+
+# ------------------------------------------------------------------ the token history (penalties.cu update_kernel)
+THREADS = 256   # update_kernel's block size: the shift moves 256 records per chunk
+MUTANTS = ["lowest_chunk_first", "guard_i_gt_pos", "insert_after", "count_on_miss", "clear_on_hit", "insert_when_full"]
+
+
+def update_emulated(buf, lens, slot, t, cap, mutant=None):
+    """update_kernel for one history row in numpy: buf int64 [slots * cap + 1, 4] holds the lists back to back (the row
+    past the last list stands for whatever follows the buffer), lens [slots].  Thread 0 binary-searches the first record
+    with id >= t and counts a hit; on a miss with n < cap the records [pos, n) move up by one in 256-record chunks,
+    highest chunk first (each chunk is read by all threads, a barrier, then written), and {t, 1, 0, 0} goes to pos.
+    `mutant` names one of MUTANTS, a wrong variant the checks must reject."""
+    base, n = slot * cap, int(lens[slot])
+    lst = buf[base:]
+    lo, hi = 0, n
+    while lo < hi:
+        mid = (lo + hi) >> 1
+        if lst[mid, 0] < t:
+            lo = mid + 1
+        else:
+            hi = mid
+    found = lo < n and lst[lo, 0] == t
+    if found:
+        lst[lo, 1] += 1
+        if mutant == "clear_on_hit":
+            lst[lo, 2:] = 0
+        return
+    if mutant == "count_on_miss" and lo < n:
+        lst[lo, 1] += 1
+    if n >= cap and mutant != "insert_when_full":
+        return
+    pos = lo + 1 if mutant == "insert_after" and lo < n else lo
+    his = list(range(n, pos, -THREADS))
+    if mutant == "lowest_chunk_first":
+        his.reverse()
+    tid = np.arange(THREADS)
+    for hi in his:
+        i = hi - THREADS + tid
+        mine = ((i > pos) if mutant == "guard_i_gt_pos" else (i >= pos)) & (i < hi)
+        e = lst[i[mine]].copy()           # every thread reads, __syncthreads, every thread writes
+        lst[i[mine] + 1] = e
+    lst[pos] = (t, 1, 0, 0)
+    lens[slot] = n + 1
+
+
+def history_cases(rng):
+    """(prompt, output, stream, bias, stops, min_tokens, V, cap): lists from empty to several chunks, streams that mix
+    repeats, fresh ids, prompt-only, bias-only and stop-only ids, and lists that reach their cap."""
+    cases = []
+    for V, n_p, n_o, n_s, cap in ((64, 0, 0, 40, 4096), (5000, 1500, 200, 300, 4096), (3000, 700, 0, 400, 4096),
+                                  (1200, 1100, 50, 300, 800), (300, 250, 20, 200, 200)):
+        prompt = rng.integers(0, V, n_p).tolist()
+        output = rng.integers(0, V, n_o).tolist()
+        bias = {int(t): float(rng.standard_normal() * 80) for t in rng.integers(0, V, 30)}
+        stops = rng.integers(0, V, 8).tolist()
+        seen = list(set(prompt) | set(output) | set(bias) | set(stops)) or [0]
+        stream = np.where(rng.random(n_s) < 0.5, rng.choice(seen, n_s), rng.integers(0, V, n_s)).tolist()
+        cases.append((prompt, output, stream, bias, stops, 10 ** 6, V, cap))
+    return cases
+
+
+def run_history(mutant):
+    """Apply every case's stream token by token to two neighbouring lists (slot 1 with the case, slot 0 poisoned and
+    never named): True iff every step gives records(prompt, output + stream so far) exactly, with the rest of the buffer,
+    the other slot and the row past the buffer untouched."""
+    from oracle.penalties import records
+    rng = np.random.default_rng(17)
+    for prompt, output, stream, bias, stops, min_tokens, V, cap in history_cases(rng):
+        kw = dict(history=True, logit_bias=bias, stop_ids=stops, min_tokens=min_tokens)
+        first = records(prompt, output, **kw)
+        if len(first) > cap:
+            continue
+        buf = rng.integers(-2 ** 31, 2 ** 31, (2 * cap + 1, 4))
+        buf[cap:cap + len(first)] = first
+        lens = np.array([int(rng.integers(0, cap)), len(first)])
+        poison = buf.copy()
+        out, held = list(output), set(first[:, 0].tolist())
+        for t in stream:
+            update_emulated(buf, lens, 1, t, cap, mutant)
+            if t in held or len(held) < cap:      # a full list drops a new id and keeps its length
+                out.append(t)
+                held.add(t)
+            want = records(prompt, out, **kw)
+            n = len(want)
+            if lens[1] != n or not np.array_equal(buf[cap:cap + n], want):
+                return False
+            if not (np.array_equal(buf[:cap], poison[:cap]) and np.array_equal(buf[cap + n:], poison[cap + n:])):
+                return False
+    return True
+
+
+def test_update_emulation_equals_records_step_by_step():
+    """One update per sampled token keeps the list equal to the oracle's list of the longer output, across chunk
+    boundaries, single- and multi-chunk shifts and full lists."""
+    assert run_history(None)
+
+
+@pytest.mark.parametrize("mutant", MUTANTS)
+def test_update_checks_reject_mutant(mutant):
+    assert not run_history(mutant), f"{mutant} passed the history checks"
+
+
+def test_records_build_rules():
+    from oracle.penalties import PEN_BIAS, PEN_PROMPT, PEN_STOP, records
+    r = records([5, 3, 5], [3, 9, 9, 9], history=True, logit_bias={7: 250.0, 3: -0.5, 9: -1e9}, stop_ids=[1, 7],
+                min_tokens=5)
+    assert r[:, 0].tolist() == [1, 3, 5, 7, 9]
+    assert r[:, 1].tolist() == [0, 1, 0, 0, 3]
+    assert r[:, 3].tolist() == [PEN_STOP, PEN_PROMPT | PEN_BIAS, PEN_PROMPT, PEN_BIAS | PEN_STOP, PEN_BIAS]
+    assert r[:, 2].view(np.float32).tolist() == [0.0, -0.5, 0.0, 100.0, -100.0]
+    # no history: only the bias and stop records; min_tokens reached: no stop records
+    assert records([5], [3], history=False, logit_bias={2: 1.0}, stop_ids=[4], min_tokens=2)[:, 0].tolist() == [2, 4]
+    assert records([5], [3], history=True, stop_ids=[4], min_tokens=1)[:, 0].tolist() == [3, 5]
+    assert records().shape == (0, 4)
